@@ -54,6 +54,8 @@ def parse():
                     help="experimental: replay one CUDA graph per optimiser step (actor.cuda_graph_update)")
     ap.add_argument("--rollout", default="auto", choices=["auto", "tc", "fused", "graph"],
                     help="rollout implementation: persistent fused kernel, per-kernel CUDA graph, or the library default")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -68,11 +70,12 @@ def measured_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s - ceilings, not reached figures
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -187,73 +190,6 @@ def cpu_iteration_rate(a, n_envs, steps, warmup):
     return n_envs * a.T / mean, mean, cores, phases
 
 
-def reference_functions_check(a):
-    """When /root/reference exists (build container only - never on the GPU box): time the reference's OWN
-    calculate_adv_and_returns (GAE) and policy_loss (actor_critic, forward + backward) through tests/golden/ref_loader.py
-    beside the oracle port on the same inputs, to show port ~= reference. Returns None when the reference is absent."""
-    try:
-        sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-        import ref_loader
-
-        if not ref_loader.reference_available():
-            return None
-        ref = ref_loader.load_reference()
-    except Exception as e:  # pragma: no cover
-        return {"error": repr(e)}
-    import torch
-
-    from oracle import rl_oracle as O
-
-    T, B, A = a.T, min(a.B, 512), a.act
-    g = torch.Generator().manual_seed(0)
-    rewards, values = torch.randn(T, B, 1, generator=g), torch.randn(T + 1, B, 1, generator=g)
-    dones = torch.rand(T + 1, B, 1, generator=g) < 0.01
-    dones[0] = False
-    n = T * B
-    old = -1 + 0.3 * torch.randn(n, A, generator=g)
-    adv, ret, pv = (torch.randn(n, 1, generator=g) for _ in range(3))
-
-    def timed(fn, reps=3):
-        fn()
-        t0 = time.perf_counter()
-        for _ in range(reps):
-            fn()
-        return (time.perf_counter() - t0) / reps
-
-    def ref_adv():
-        return ref.registry.calculate_adv_and_returns(task_type="embodied", adv_type="gae", rewards=rewards, dones=dones,
-                                                      values=values, gamma=0.99, gae_lambda=0.95, group_size=8,
-                                                      reward_type="action_level", num_action_chunks=1, loss_mask=None,
-                                                      loss_mask_sum=None)
-
-    def port_adv():
-        return O.adv_and_returns_embodied("gae", rewards, dones, values, gamma=0.99, gae_lambda=0.95)
-
-    def loss_inputs():
-        new = (old + 0.05 * torch.randn(n, A, generator=g)).requires_grad_(True)
-        val = (pv + 0.1 * torch.randn(n, 1, generator=g)).requires_grad_(True)
-        return new, val
-
-    def ref_loss():
-        new, val = loss_inputs()
-        loss, _ = ref.registry.policy_loss(task_type="embodied", loss_type="actor_critic", logprob_type="action_level",
-                                           reward_type="action_level", single_action_dim=A, logprobs=new, values=val,
-                                           old_logprobs=old, advantages=adv, returns=ret, prev_values=pv,
-                                           clip_ratio_high=0.2, clip_ratio_low=0.2, value_clip=0.2, huber_delta=10.0,
-                                           loss_mask=None, loss_mask_sum=None, max_episode_steps=128, critic_warmup=False)
-        loss.backward()
-
-    def port_loss():
-        new, val = loss_inputs()
-        loss, _ = O.policy_loss_embodied("actor_critic", new, old, adv, "action_level", A, values=val, prev_values=pv,
-                                         returns=ret, clip_ratio_low=0.2, clip_ratio_high=0.2, value_clip=0.2,
-                                         huber_delta=10.0)
-        loss.backward()
-
-    return {"shape": f"T={T} B={B} A={A}", "gae_s": {"reference": timed(ref_adv), "port": timed(port_adv)},
-            "loss_fwd_bwd_s": {"reference": timed(ref_loss), "port": timed(port_loss)}}
-
-
 def run_reference(a):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -287,31 +223,20 @@ def run_reference(a):
                          "phases_s": phases, "envs_timed": n_envs},
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
-    chk = reference_functions_check(a)
-    if chk is not None:
-        line["cpu_baseline"]["port_vs_reference_functions"] = chk
     print(json.dumps(line), flush=True)
 
 
 # ------------------------------------------------------------------------------------------------
 # our arm
 # ------------------------------------------------------------------------------------------------
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures
-# (profiles/r01_ncu_mlp_step_v3_table.txt, profiles/r01_ncu_gae_v4_summary.txt); only valid at the captured shape.
-NCU_TRAFFIC = {
-    # profiles/r02_ncu_final_table.txt (ncu --set full, per launch; GEMMs: grouped two-tower launches at 262144 rows, per tower = half)
-    ("tc_gemm_fwd", 262144): (537.4e6 + 484.0e6) / 2,   # 268.7 MB read + 242.0 MB written back before the kernel ends
-    ("tc_wgrad", 262144): (1074.6e6 + 4.5e6) / 2,
-    ("gae_scan", 512, 4096): 18.9e6,    # reads only: the 16.8 MB of results are still in L2 when the kernel ends
-    ("ppo", 262144): 64.4e6 + 3.0e6,    # 2x the algorithmic 32.5 MB: every gathered 4-byte scalar pulls a 32-byte sector
-    ("logits_fwd", 4096, 32000): 524.6e6 + 3.7e6,
-    ("logits_bwd", 4096, 32000): 524.5e6 + 478.7e6,
-}
+# dram__bytes_read.sum + dram__bytes_write.sum per launch from `ncu --set full` captures at the benchmarked shapes
+# (key: kernel, shape); only valid at the captured shape.  None recorded on the H100 yet.
+NCU_TRAFFIC = {}
 
 
 def kernel_rooflines(a, peaks, torch):
     """Live CUDA-event timing of the HBM-bound kernels at the workload's shapes. Each kernel is launched
-    from a captured CUDA graph over ROT independent input sets whose total size exceeds L2 (126 MB), so
+    from a captured CUDA graph over ROT independent input sets whose total size exceeds L2 (50 MB), so
     every launch streams from HBM; per-launch time = graph time / launches (includes inter-kernel gaps)."""
     from rlinf_b200 import ops
 
@@ -416,7 +341,7 @@ def kernel_rooflines(a, peaks, torch):
                     "algorithmic_bytes": nbytes, "rows": Nl, "vocab": V}
     del lg, dlg
 
-    # ---- tcgen05 fp16-split GEMMs of the MLP towers at the mini-batch shape (the shipped kernels, csrc/tc_gemm_h.cu) ----
+    # ---- wgmma fp16-split GEMMs of the MLP towers at the mini-batch shape (the shipped kernels, csrc/tc_gemm_h.cu) ----
     n = mb
     K = 256
     Amat = torch.randn(n, K, device=dev)
@@ -461,6 +386,21 @@ def _update_phase_bytes(n, obs, act, H):
     fwd = 2 * (X + U + 2 * U + 2 * U) + 2 * U
     bwd = 4 * U + 2 * (2 * U + 3 * U + 2 * U + 3 * U + (U + X))
     return fwd + bwd
+
+
+def dump_outputs(out_dir, run, metrics, torch):
+    """Rollout batch (fixed seeded sample of 64 environments), parameters and metrics of the last timed step."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    idx = torch.randperm(run.buffer.B, generator=torch.Generator().manual_seed(0))[:64].sort().values.cuda()
+    b = run.buffer.as_batch()
+    fi = b.pop("forward_inputs")
+    for k, t in list(b.items()) + [(f"forward_inputs.{k}", v) for k, v in fi.items()]:
+        np.save(os.path.join(out_dir, f"rollout.{k}.npy"), t.index_select(1, idx).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "params.npy"), run.actor.model.flat_params.float().cpu().numpy())
+    for k, v in (metrics or {}).items():
+        np.save(os.path.join(out_dir, "metric." + k.replace("/", ".") + ".npy"), np.asarray(float(v), dtype=np.float64))
 
 
 def run_ours(a):
@@ -530,6 +470,8 @@ def run_ours(a):
     t_wall = time.perf_counter() - t_wall0
     total_ms = ev[0].elapsed_time(ev[3 * a.steps])
     log(f"timed {a.steps} steps: {total_ms:.1f} ms")
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, run, metrics, torch)
     rollout_ms = sum((ev[3 * i].elapsed_time(ev[3 * i + 1])) for i in range(a.steps)) / a.steps
     launches = lib.rb200_launch_count() - launches0 + graph_nodes * a.steps
     clocks = sampler.stop() if sampler else None
@@ -591,7 +533,7 @@ def run_ours(a):
         "config": {"workload": workload_name(a), "B": a.B, "T": a.T, "obs_dim": a.obs, "act_dim": a.act,
                    "global_batch_size": cfg.actor.global_batch_size, "micro_batch_size": cfg.actor.micro_batch_size,
                    "parallelism": f"dp{a.gpus} over envs, 1 NCCL all-reduce of the flat grad buffer / optimiser step",
-                   "l2": "per-step inputs (1.2 GB rollout batch / rank share) exceed the 126 MB L2; kernel "
+                   "l2": "per-step inputs (1.2 GB rollout batch / rank share) exceed the 50 MB L2; kernel "
                          "micro-timings rotate >300 MB of inputs"},
         "phases_ms": {"rollout": rollout_ms, "update": ms_per_step - rollout_ms},
         "wall_ms_per_step": t_wall / a.steps * 1e3,
@@ -611,10 +553,10 @@ def run_ours(a):
         bwd = 2 * (O * H + 2 * H * H) * 2 + 2 * (2 * H * H) * 2  # wgrad (3 layers) + dgrad (2 layers), two towers
         flops_update = (fwd + bwd) * n * a.update_epoch
         upd_s = (ms_per_step - rollout_ms) * 1e-3
-        ceiling = peaks["bf16_tflops_sustained"] / 3.0  # fp32-accurate product = 3 kind::f16 MMAs
+        ceiling = peaks["bf16_tflops_sustained"] / 3.0  # fp32-accurate product = 3 fp16 MMAs
         bytes_update = _update_phase_bytes(n, O, A, H) * a.update_epoch
         line["roofline"] = {
-            "kernel": "whole update phase (tc_h_gemm_kernel / tc_h_wgrad_kernel fp16-split tcgen05 GEMMs + heads + loss + AdamW)",
+            "kernel": "whole update phase (tc_h_gemm_kernel / tc_h_wgrad_kernel fp16-split wgmma GEMMs + heads + loss + AdamW)",
             "bound": "hbm", "achieved": bytes_update / upd_s / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
             "frac": bytes_update / upd_s / 1e9 / peaks["hbm_gbs"], "traffic": None,
             "algorithmic_bytes": bytes_update, "tensor_tflops": flops_update / upd_s / 1e12,
@@ -630,16 +572,16 @@ def run_ours(a):
                 line["roofline_update_phase"] = line["roofline"]
                 # dominant kernel of the step, timed alone with CUDA events
                 line["roofline"] = {
-                    "kernel": "rb::tch::tc_h_gemm_kernel (tcgen05 kind::f16, 2-way fp16 split = fp32-accurate GEMM of the MLP "
+                    "kernel": "rb::tch::tc_h_gemm_kernel (wgmma, 2-way fp16 split = fp32-accurate GEMM of the MLP "
                               "towers; forward/dgrad), mini-batch shape, one tower",
                     "bound": "hbm", "achieved": g["achieved"], "peak": g["peak"], "unit": "GB/s", "frac": g["frac"],
                     "traffic": g["traffic"], "algorithmic_bytes": g["algorithmic_bytes"],
                     "tensor_tflops": g["tensor_tflops"], "frac_of_fp16_split_ceiling": g["frac_of_fp16_split_ceiling"],
                     "us_per_launch": g["us_per_launch"], "algorithmic_flops": g["algorithmic_flops"],
                     "note": "achieved = algorithmic bytes (A [n,256] fp32 read + C [n,256] fp32 written) / live CUDA-event time "
-                            "per launch; peak = measured HBM copy bandwidth.  2*n*256*256 flops over 2 KB per row = 64 "
-                            "flop/B: at 3 kind::f16 MMAs per product the tensor time (peak/3) is below the HBM time of the "
-                            "fp32 operands, so HBM bounds the kernel (DESIGN.md section 4). " + g["note"]}
+                            "per launch; peak = HBM bandwidth (peaks source in the line).  2*n*256*256 flops over 2 KB per row = 64 "
+                            "flop/B: at 3 fp16 MMAs per product the tensor time (peak/3) is below the HBM time of the "
+                            "fp32 operands, so HBM bounds the kernel. " + g["note"]}
                 line["roofline_tc_wgrad"] = w
                 line["roofline_hbm_kernels"] = kr
             except Exception as e:  # pragma: no cover

@@ -1,5 +1,5 @@
 /*
- * rlinf_b200.h - C ABI of librlinf_b200.so: the B200-native (sm_100a) drop-in for the
+ * rlinf_b200.h - C ABI of librlinf_b200.so: the H100-native (sm_90a) drop-in for the
  * data-parallel hot path of RLinf's actor-learner (advantages, PPO/GRPO loss,
  * MLP policy forward/backward, grad-clip + AdamW, rollout sampling).
  *
@@ -277,7 +277,7 @@ int rb200_mlp_layout_init(rb200_mlp_layout* L, int obs_dim, int act_dim, int val
 /* scratch sizes (floats) for n rows: `acts` and `work` of forward/backward/sample/value each need this many */
 int64_t rb200_mlp_fwd_scratch_floats(const rb200_mlp_layout* L, int64_t n);
 
-/* Tensor-core operand cache: exact-TF32 (hi, lo) copies (and transposes) of the hidden-layer weights.
+/* Tensor-core operand cache: packed fp16 (hi, lo) tiles of the hidden-layer weights (forward and dgrad packs).
  * rb200_mlp_wsplit_floats() floats; refresh with rb200_mlp_prepare_weights() after every parameter update.
  * Passing wsplit == NULL to the calls below selects the fp32 SIMT GEMMs for every layer. */
 int64_t rb200_mlp_wsplit_floats(const rb200_mlp_layout* L);
@@ -286,9 +286,10 @@ int rb200_mlp_prepare_weights(const rb200_mlp_layout* L, const float* params, fl
 
 /* Forward for training: states [n,obs] (row i at idx?idx[i]:i), action [n,act] (same gather).
  * Writes logprobs [n,act], entropy [n,act] (NULL ok), values [n,value_dim] (NULL ok) and keeps
- * the activations needed by backward in `acts`. Hidden layers run on tcgen05 (3xTF32) when wsplit is given
+ * the activations needed by backward in `acts`. Hidden layers run on wgmma (2-way fp16 split) when wsplit is given
  * and the layer's K is a multiple of 32 (layer 1 additionally needs idx == NULL). Activations are plain fp32; the
- * tensor-core kernels split them into exact-TF32 (hi, lo) operands in shared memory. */
+ * tensor-core kernels split them into fp16 (hi, lo) operands.  (The 3xTF32 entries of earlier versions -
+ * rb200_tc_gemm, rb200_tc_wgrad, rb200_split_tf32 - and the two probe hooks are gone.) */
 int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params, const float* wsplit,
                       const float* states, const float* action, const int64_t* idx, int64_t n,
                       float* logprobs, float* entropy, float* values, float* acts, float* work,
@@ -309,20 +310,7 @@ int rb200_mlp_sample(const rb200_mlp_layout* L, const float* params, const float
                      const uint64_t* counter_dev, int64_t n, float* action, float* logprobs, float* values,
                      float* work, rb200_stream_t stream);
 
-/* x[n] -> exact-TF32 pair hi[n], lo[n] with hi + lo ~= x (2^-22 relative): the operand split of the 3xTF32 GEMMs
- * (applied to the weights by rb200_mlp_prepare_weights and, on the fly, to activations inside the GEMM kernels). */
-int rb200_split_tf32(const float* x, float* hi, float* lo, int64_t n, rb200_stream_t stream);
-
-/* 3xTF32 tensor-core GEMM building block of the MLP towers (unit-test entry):
- * C[M,256] = A[M,K] . B[256,K]^T, fp32 in/out, K % 32 == 0; `work` = 512*K floats (split copy of B). */
-int rb200_tc_gemm(const float* A, const float* B, float* C, int64_t M, int K, float* work,
-                  rb200_stream_t stream);
-
-/* Weight-gradient counterpart (unit-test entry): dW[256,IN] += Z[n,256]^T . H[n,IN], IN % 32 == 0, IN <= 256;
- * `work` is unused (may be NULL). */
-int rb200_tc_wgrad(const float* Z, const float* H, float* dW, int64_t n, int IN, float* work,
-                   rb200_stream_t stream);
-/* round 2: the same two unit-test entries for the fp16-split kernel::f16 kernels (csrc/tc_gemm_h.cu).
+/* Unit-test entries of the fp16-split tensor-core GEMMs of the MLP towers (csrc/tc_gemm_h.cu, wgmma, fp32 in/out).
  * mode 0: C = A[M,K] . B[256,K]^T; mode 1 (dgrad form, K = 256): C = A[M,256] . B[256,256].  amax: device float holding
  * max|A| (or max|Z|), NULL = no operand scaling.  work: >= 512*K floats (packed fp16 weight tiles: forward + dgrad pack). */
 int rb200_tc_gemm_h(const float* A, const float* B, float* C, int64_t M, int K, int mode, const float* amax,
@@ -330,14 +318,9 @@ int rb200_tc_gemm_h(const float* A, const float* B, float* C, int64_t M, int K, 
 int rb200_tc_wgrad_h(const float* Z, const float* H, float* dW, int64_t n, int IN, const float* amax,
                      rb200_stream_t stream);
 
-/* Experiment switches (tools/ and tests only; default 0 = the shipped kernels): 1 = additionally mask the streamed operand's
- * hi part in shared memory in the 3xTF32 kernels (not needed: the tensor core truncates), 2 = round-1 layers in the fp32
- * SIMT fused rollout (one-k-step weight prefetch), 8 = round-1 3xTF32 GEMMs instead of the fp16-split ones, 32 = one
- * fp16-split GEMM launch per tower instead of the grouped launch, 64 = 8 transform warps in the fp16-split forward kernel,
- * bits 8-15 = TMA L2-prefetch distance of the 3xTF32 kernels in k-blocks (255 = off). */
+/* Experiment switches (tests only; default 0 = the shipped kernels): 2 = round-1 layers in the fp32 SIMT fused rollout
+ * (one-k-step weight prefetch). */
 int rb200_debug_set_flags(int flags);
-/* probe hook of the fp16-split GEMM (csrc/tc_gemm_h.cu): 16 int64 per-role wait / work cycle counters of CTA 0 */
-int rb200_tc_h_debug(void* prof16);
 
 /* Persistent fused rollout (csrc/rollout_fused.cu): the whole T-step loop of one rank - MLP actor/critic inference,
  * Normal sampling, synthetic-env dynamics with auto-reset and the truncation bootstrap of rewards - in ONE kernel;
@@ -362,17 +345,15 @@ int rb200_rollout_fused(const rb200_mlp_layout* L, const float* params, const fl
                         double noise_std, double reward_noise_std, rb200_stream_t stream);
 
 /* Persistent TENSOR-CORE rollout (csrc/rollout_tc.cu): same loop, buffers, row alignment and random streams as
- * rb200_rollout_fused, but every hidden layer of both towers and the env's s.W_s product run on tcgen05 (kind::f16,
+ * rb200_rollout_fused, but every hidden layer of both towers and the env's s.W_s product run on wgmma (fp16 in,
  * 2-way fp16 split with fp32 accumulation, computed transposed: D[hidden unit, env] = W . X^T, 32 environments per CTA,
- * activations handed from TMEM to the next layer's operand tile in shared memory); the truncation bootstrap
+ * activations handed from the accumulator registers to the next layer's operand tile in shared memory); the truncation bootstrap
  * V(final_obs) rides in 32 extra MMA columns of the next step's value tower.  The weights are streamed from a packed,
  * pre-split, pre-swizzled copy (rb200_rollout_tc_pack_bytes bytes, 16-byte aligned) that rb200_rollout_tc_prepare()
  * rebuilds from the flat parameters and the env's w_s [obs,obs] after every parameter update.
  * rb200_rollout_tc_supported() == 0 iff hidden == 256, value_dim == 1, act_dim <= 8, obs_dim % 32 == 0, obs_dim <= 128.
  * Replaces the same reference loop as rb200_rollout_fused (env_worker.py:1059-1349, huggingface_worker.py:678-781). */
 int rb200_rollout_tc_supported(const rb200_mlp_layout* L, int B);
-/* probe hook: ablation switches + 16 int64 wait-cycle counters of CTA 0 (flags = 0, prof16 = NULL: production kernel) */
-int rb200_rollout_tc_debug(int flags, void* prof16);
 int64_t rb200_rollout_tc_pack_bytes(const rb200_mlp_layout* L);
 int rb200_rollout_tc_prepare(const rb200_mlp_layout* L, const float* params, const float* w_s, void* pack,
                              rb200_stream_t stream);

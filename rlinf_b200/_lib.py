@@ -112,21 +112,16 @@ SIGNATURES = {
     "rb200_mlp_prepare_weights": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p]),
     "rb200_mlp_forward": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 5 + [c_int64] + [c_void_p] * 6),
     "rb200_mlp_backward": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 5 + [c_int64] + [c_void_p] * 7),
-    "rb200_split_tf32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "rb200_mlp_sample": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 4 + [c_uint64, c_uint64, c_void_p, c_int64] + [c_void_p] * 5),
-    "rb200_tc_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
-    "rb200_tc_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     "rb200_tc_gemm_h": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "rb200_tc_wgrad_h": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     "rb200_debug_set_flags": (c_int, [c_int]),
-    "rb200_tc_h_debug": (c_int, [c_void_p]),
     "rb200_rollout_fused_wt_floats": (c_int64, [C.POINTER(MlpLayout)]),
     "rb200_rollout_fused_supported": (c_int, [C.POINTER(MlpLayout), c_int]),
     "rb200_rollout_fused_prepare": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p]),
     "rb200_rollout_fused": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 19 + [c_uint64] * 3 + [c_int] * 5 +
                             [c_double] * 4 + [c_void_p]),
     "rb200_rollout_tc_supported": (c_int, [C.POINTER(MlpLayout), c_int]),
-    "rb200_rollout_tc_debug": (c_int, [c_int, c_void_p]),
     "rb200_rollout_tc_pack_bytes": (c_int64, [C.POINTER(MlpLayout)]),
     "rb200_rollout_tc_prepare": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_void_p]),
     "rb200_rollout_tc": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 5 +
@@ -168,7 +163,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise Rb200Error(
             f"{LIB_PATH} not found: build it with `python -m rlinf_b200.build` "
-            "(nvcc, sm_100a). rlinf_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a). rlinf_b200 has no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing -> loud
@@ -204,7 +199,7 @@ def stream_ptr(device=None):
 
 def default_device() -> torch.device:
     if not torch.cuda.is_available():
-        raise Rb200Error("rlinf_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise Rb200Error("rlinf_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 
 

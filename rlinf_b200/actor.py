@@ -92,13 +92,9 @@ class EmbodiedActor:
         self.rollout_batch: dict = {}
         self._perm_cache: dict = {}
         self.version = 0
-        # actor.cuda_graph_update: replay one CUDA graph per optimiser step instead of ~35 ctypes launches (validated
-        # on B200: bit-for-bit the same kernels; measured gain 48.4 -> 45.2 ms per update at 32 k samples / step - the
-        # step is kernel-bound, so this is a few percent, not the 40 % the round-1 notes expected)
+        # actor.cuda_graph_update: replay one CUDA graph per optimiser step instead of ~35 ctypes launches
         self._graph_update = self.cfg.actor.get("cuda_graph_update", False)  # True / False / "auto"
-        # Multi-rank graphed steps are EXPERIMENTAL and off unless actor.cuda_graph_multi_rank is set: on 2 x B200
-        # (torch 2.11 / NCCL 2.28.9) the 2-rank parity test with the NCCL all-reduce captured inside the step graph never
-        # completed (pytest timeout after 500 s, profiles/r02_two_rank_nccl.txt); the eager all-reduce path passes.
+        # Multi-rank graphed steps are EXPERIMENTAL and off unless actor.cuda_graph_multi_rank is set.
         self._graph_multi_rank = bool(self.cfg.actor.get("cuda_graph_multi_rank", False))
         self._capture_nccl = bool(self.cfg.actor.get("cuda_graph_capture_nccl", True))
         self._static_batch: dict = {}

@@ -4,7 +4,7 @@ Mirror of rlinf/algorithms/registry.py: `ADV_REGISTRY` (:30), `register_advantag
 `get_adv_and_returns` (:47), `LOSS_REGISTRY` (:56), `register_policy_loss` (:59),
 `get_policy_loss` (:71), `policy_loss` (:77-92), `calculate_adv_and_returns` (:95-124).
 Same names, kwargs, return conventions (embodied -> dict, reasoning -> tuple) and error behaviour;
-the registered callables launch the sm_100a kernels of librlinf_b200.so.
+the registered callables launch the sm_90a kernels of librlinf_b200.so.
 """
 from __future__ import annotations
 

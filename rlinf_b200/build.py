@@ -1,8 +1,8 @@
-"""Build librlinf_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build librlinf_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m rlinf_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so, the object files and the freshness stamp are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ LIB_PATH = os.path.join(PKG_DIR, "librlinf_b200.so")
 STAMP = os.path.join(PKG_DIR, ".librlinf_b200.stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3",
     "--expt-relaxed-constexpr",
@@ -81,7 +81,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed")
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC",
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
             "-o", LIB_PATH, *objs, "-lcudart_static" if False else "-lcudart"]
     subprocess.run(link, check=True)
     with open(STAMP, "w") as fh:

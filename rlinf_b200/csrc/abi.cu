@@ -22,6 +22,19 @@ double* device_scratch(int n_doubles_min) {
   }
   return ptr[dev];
 }
+float* partials_scratch(int64_t n_floats_min) {
+  static float* ptr[64] = {nullptr};
+  static int64_t cap[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
+  if (cap[dev] < n_floats_min) {  // grow-only, the old block is leaked (captured graphs may still reference it)
+    float* p = nullptr;
+    if (cudaMalloc(&p, sizeof(float) * (size_t)n_floats_min) != cudaSuccess) return nullptr;
+    ptr[dev] = p;
+    cap[dev] = n_floats_min;
+  }
+  return ptr[dev];
+}
 }  // namespace rb
 
 namespace rb { unsigned long long launches(); }

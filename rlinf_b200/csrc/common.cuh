@@ -1,4 +1,4 @@
-// Shared helpers for the rlinf_b200 kernels (sm_100a only).
+// Shared helpers for the rlinf_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -58,14 +58,16 @@ inline cudaStream_t as_stream(rb200_stream_t s) { return reinterpret_cast<cudaSt
 
 // Per-device scratch (reduction slots); allocated on first use, never freed.
 double* device_scratch(int n_doubles_min);  // defined in abi.cu; returns nullptr on failure
+// Per-device scratch for per-CTA partial sums (grow-only); nullptr on failure.
+float* partials_scratch(int64_t n_floats_min);
 
 inline int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];

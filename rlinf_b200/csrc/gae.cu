@@ -80,14 +80,13 @@ __device__ __forceinline__ void flush_stats(const Acc& a, const Acc& r, double* 
 //   warps 1-4   delta    : delta_t and the recurrence coefficient c_t = (gamma*lambda)*!done  (no dependence on g)
 //   warp 5      chain    : g_t = delta_t + c_t * g_{t+1}, strictly sequential, 2 dependent fp32 ops per step
 //   warps 6-9   epilogue : ret = g + V, adv = ret - V staged in smem, statistics, TMA tile stores
-// A single warp doing all of this is issue-bound (ncu round-1 v1: 46 us, ~107 cycles / step); splitting the work
+// A single warp doing all of this is issue-bound (~107 cycles / step); splitting the work
 // that does not depend on the carry across warps leaves ~9 cycles / step on the sequential warp.
 // Stage hand-off: full (TMA) -> dready (delta warps) -> gready (chain) -> empty (epilogue), all mbarriers.
 // Requires B % 16 == 0 (16-byte global strides for the byte tensors) and 16-byte aligned bases.
 // ---------------------------------------------------------------------------------------------
-// Box size (round 1): tools/tma_probe.cu pulls the three input arrays at 3.05 TB/s with [64 x 32] boxes but only
-// 1.76 TB/s with [16 x 32] boxes (per-box overhead), hence 64 steps per stage.  The loads are NOT what bounds this
-// kernel (a pure pull takes 8.3 us of the 16.7 us); the epilogue warps were - see the comment there.
+// Box size: small [16 x 32] boxes pay a per-box overhead (tools/tma_probe.cu), hence 64 steps per stage.  The loads are
+// NOT what bounds this kernel; the epilogue warps were - see the comment there.
 constexpr int kRW = 64;       // timesteps per TMA stage
 constexpr int kStagesWS = 4;  // 4 x 44.4 KB
 struct __align__(128) StageWS {
@@ -206,8 +205,7 @@ __global__ void __launch_bounds__(kWsThreads) gae_tma_kernel(const __grid_consta
     // instruction (time of v1-v3 == #STG per warp x ~60 cycles), so results are staged in shared memory (ret in
     // place of g, adv in the dead delta/coef buffer) and leave as two TMA tile stores per 64-step tile; (2) with the
     // stores gone the epilogue was issue-bound (~37 instructions per step on ONE warp per tile), hence 4 warps per
-    // tile and a branch-free statistics path.  A pure TMA pull of the same three inputs takes 8.3 us
-    // (tools/tma_probe.cu), so the loads are not what bounds this kernel.
+    // tile and a branch-free statistics path.
     const int e = warp - (kDW + 2);
     const int col = col0 + lane;
     const bool in_range = col < B;

@@ -4,12 +4,11 @@
 // ValueHead, rlinf/models/embodiment/modules/value_head.py:18-67 (3x256 tanh MLP -> value_dim, last layer
 // without bias); backward = what autograd derives from them.
 //
-// Hidden-layer GEMMs run on the tensor cores whenever the operand shapes allow TMA (K % 32 == 0, no row gather): by
-// default the fp16-split kernels (tc_gemm_h.cu: tcgen05 kind::f16, a = a_hi + a_lo in fp16, three MMAs per product,
-// fp32-level accuracy, both towers per launch), with debug flag 8 the round-1 3xTF32 kernels (tc_gemm.cu); the fp32 SIMT
-// GEMM (sgemm.cuh) covers the remaining shapes.  Activations and activation-gradients are stored once, as plain fp32
-// [n,256] (6 tanh outputs per forward, tanh' = 1 - h^2); the tensor-core kernels split them into (hi, lo) pairs on the
-// fly in shared memory.
+// Hidden-layer GEMMs run on the tensor cores whenever the operand shapes allow TMA (K % 32 == 0, no row gather): the
+// fp16-split kernels (tc_gemm_h.cu: wgmma, a = a_hi + a_lo in fp16, three MMAs per product, fp32-level accuracy, both
+// towers per launch); the fp32 SIMT GEMM (sgemm.cuh) covers the remaining shapes and callers without a weight cache.
+// Activations and activation-gradients are stored once, as plain fp32 [n,256] (6 tanh outputs per forward,
+// tanh' = 1 - h^2); the tensor-core kernels split them into (hi, lo) pairs on the fly.
 // The heads (256 -> act mean, 256 -> value) are fused with the Normal log-prob / entropy epilogue and their backward.
 #include <curand_kernel.h>
 
@@ -81,8 +80,8 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(HeadFwdArgs p) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
   const bool want_v = p.g3 && p.values;
   const int64_t row_stride = (int64_t)gridDim.x * nwarp;
-  // one warp per row; the NEXT row's 2 KB are requested before this row's dot products and shuffles (round 2: without
-  // the prefetch a warp alternated between a DRAM round trip and ~150 dependent instructions: 193 us for 537 MB)
+  // one warp per row; the NEXT row's 2 KB are requested before this row's dot products and shuffles (without the
+  // prefetch a warp alternates between a DRAM round trip and ~150 dependent instructions)
   float4 nh0 = make_float4(0.f, 0.f, 0.f, 0.f), nh1 = nh0, ng0 = nh0, ng1 = nh0;
   auto fetch = [&](int64_t r) {
     if (r < p.n) {
@@ -172,6 +171,7 @@ struct HeadBwdArgs {
   float* g_vb2;             // [256] += column sums of dy3 (value layer 3)
   float* amax_dz3;          // [1] atomicMax |dz3| (operand scaling of the fp16-split gradient GEMMs), or null
   float* amax_dy3;          // [1] atomicMax |dy3|, or null
+  float* part;              // [gridDim.x][acc length] per-block sums of the accumulators below (summed in block order)
   int64_t n;
   int act, vdim;
 };
@@ -181,29 +181,24 @@ struct HeadBwdArgs {
 template <bool REG>
 __global__ void __launch_bounds__(256) head_bwd_kernel(HeadBwdArgs p) {
   extern __shared__ float sm[];
-  // layout: mw [act][256] | vw [vdim][256] | acc_mw [act][256] | acc_vw [vdim][256] | acc_mb[32] | acc_ls[32] |
-  //         acc_b2[256] | acc_vb2[256]
+  // layout: mw [act][256] | vw [vdim][256] | per warp: acc_mw [act][256] | acc_vw [vdim][256] | acc_mb[32] | acc_ls[32] |
+  //         acc_b2[256] | acc_vb2[256]  (private copies: no two warps add into the same word, so the sums are deterministic)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+  const int acc_len = (p.act + p.vdim) * kH + 64 + 2 * kH;
   float* s_mw = sm;
   float* s_vw = s_mw + p.act * kH;
-  float* a_mw = s_vw + p.vdim * kH;
+  float* acc0 = s_vw + p.vdim * kH;
+  float* a_mw = acc0 + warp * acc_len;
   float* a_vw = a_mw + p.act * kH;
   float* a_mb = a_vw + p.vdim * kH;
   float* a_ls = a_mb + 32;
   float* a_b2 = a_ls + 32;
   float* a_vb2 = a_b2 + kH;
   const bool has_v = p.d_values != nullptr;
-  for (int i = threadIdx.x; i < p.act * kH; i += blockDim.x) {
-    s_mw[i] = p.mw[i];
-    a_mw[i] = 0.f;
-  }
-  for (int i = threadIdx.x; i < p.vdim * kH; i += blockDim.x) {
-    s_vw[i] = has_v ? p.vw3[i] : 0.f;
-    a_vw[i] = 0.f;
-  }
-  if (threadIdx.x < 64) a_mb[threadIdx.x] = 0.f;  // a_mb and a_ls are contiguous
-  for (int i = threadIdx.x; i < 2 * kH; i += blockDim.x) a_b2[i] = 0.f;  // a_b2 and a_vb2 are contiguous
+  for (int i = threadIdx.x; i < p.act * kH; i += blockDim.x) s_mw[i] = p.mw[i];
+  for (int i = threadIdx.x; i < p.vdim * kH; i += blockDim.x) s_vw[i] = has_v ? p.vw3[i] : 0.f;
+  for (int i = threadIdx.x; i < nwarp * acc_len; i += blockDim.x) acc0[i] = 0.f;
   __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
   float cb[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, cv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   float mz = 0.f, my = 0.f;  // running max |dz3|, |dy3|
   float rm[REG ? 8 : 1][8], rv[REG ? 2 : 1][8];
@@ -216,7 +211,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(HeadBwdArgs p) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) rv[c][j] = 0.f;
   // One warp per row, 152 registers in the REG variant -> 8 warps / SM: without help every row pays a full DRAM
-  // round trip (ncu round 1: 565 us for 1.05 GB).  The row inputs are therefore fetched two rows ahead.
+  // round trip.  The row inputs are therefore fetched two rows ahead.
   struct RowIn {
     float4 h0, h1, g0, g1;
     float x, mu, dlp, den, dv0, dv1;
@@ -379,18 +374,10 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(HeadBwdArgs p) {
     }
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < p.act * kH; i += blockDim.x)
-    if (a_mw[i] != 0.f) atomicAdd(&p.g_mw[i], a_mw[i]);
-  if (has_v)
-    for (int i = threadIdx.x; i < p.vdim * kH; i += blockDim.x)
-      if (a_vw[i] != 0.f) atomicAdd(&p.g_vw3[i], a_vw[i]);
-  if (threadIdx.x < p.act) {
-    atomicAdd(&p.g_mb[threadIdx.x], a_mb[threadIdx.x]);
-    atomicAdd(&p.g_logstd[threadIdx.x], a_ls[threadIdx.x]);
-  }
-  for (int i = threadIdx.x; i < kH; i += blockDim.x) {
-    atomicAdd(&p.g_b2[i], a_b2[i]);
-    if (has_v) atomicAdd(&p.g_vb2[i], a_vb2[i]);
+  for (int i = threadIdx.x; i < acc_len; i += blockDim.x) {
+    float s = 0.f;
+    for (int w = 0; w < nwarp; ++w) s += acc0[w * acc_len + i];
+    p.part[(size_t)blockIdx.x * acc_len + i] = s;
   }
 }
 
@@ -407,39 +394,27 @@ int head_grid(int64_t n) {
 struct TowerW {           // fp32 weights (SIMT path)
   const float *w0, *b0, *w1, *b1, *w2, *b2;
 };
-struct TowerWS {          // exact-TF32 (hi, lo) copies for the tensor cores (null => SIMT everywhere)
-  const float *w0h, *w0l, *w1h, *w1l, *w2h, *w2l;   // [256,in] as stored (forward:  X . W^T)
-  const float *w1th, *w1tl, *w2th, *w2tl;           // transposed [in=256, out=256] (dgrad: dZ . W)
-};
-
 // one hidden layer forward: out = tanh(in . W^T + b)
 int layer_forward(const float* in, const int64_t* idx, int64_t n, int in_dim, const float* w, const float* b,
-                  const float* wh, const float* wl, float* out, cudaStream_t st) {
-  const bool tc_ok = wh != nullptr && idx == nullptr && (in_dim % rb::tc::BK == 0);
-  if (tc_ok) {
-    rb::tc::Params p{};
-    p.M = n; p.K = in_dim; p.bias = b; p.c = out; p.epi = rb::tc::EPI_BIAS_TANH;
-    return rb::tc::launch(in, wh, wl, p, st);
-  }
+                  float* out, cudaStream_t st) {
   GemmArgs g{};
   g.M = n; g.N = kH; g.ldc = kH; g.k_per_split = 1 << 30;
   g.A = in; g.lda = in_dim; g.a_rows = idx; g.B = w; g.ldb = in_dim; g.K = in_dim; g.bias = b; g.C = out;
   return launch_gemm<A_KCONTIG, B_KCONTIG, EPI_BIAS_TANH>(g, 1, st);
 }
 
-// X -> H1 -> H2 -> H3 (each [n,256])
-int tower_forward(const float* X, const int64_t* idx, int64_t n, int in_dim, const TowerW& w, const TowerWS* ws,
-                  float* H1, float* H2, float* H3, cudaStream_t st) {
-  int e = layer_forward(X, idx, n, in_dim, w.w0, w.b0, ws ? ws->w0h : nullptr, ws ? ws->w0l : nullptr, H1, st);
+// X -> H1 -> H2 -> H3 (each [n,256]), fp32 SIMT
+int tower_forward(const float* X, const int64_t* idx, int64_t n, int in_dim, const TowerW& w, float* H1, float* H2,
+                  float* H3, cudaStream_t st) {
+  int e = layer_forward(X, idx, n, in_dim, w.w0, w.b0, H1, st);
   if (e) return e;
-  e = layer_forward(H1, nullptr, n, kH, w.w1, w.b1, ws ? ws->w1h : nullptr, ws ? ws->w1l : nullptr, H2, st);
+  e = layer_forward(H1, nullptr, n, kH, w.w1, w.b1, H2, st);
   if (e) return e;
-  return layer_forward(H2, nullptr, n, kH, w.w2, w.b2, ws ? ws->w2h : nullptr, ws ? ws->w2l : nullptr, H3, st);
+  return layer_forward(H2, nullptr, n, kH, w.w2, w.b2, H3, st);
 }
 
-// backward through the three hidden layers of one tower, given dZ3. tmpA/tmpB: [n,256] scratch.
-int tower_backward(const float* X, const int64_t* idx, int64_t n, int in_dim, const TowerW& w, const TowerWS* ws,
-                   const float* H1, const float* H2, const float* dZ3, float* tmpA, float* tmpB, float* g_w0,
+// backward through the three hidden layers of one tower, given dZ3 (fp32 SIMT). tmpA/tmpB: [n,256] scratch.
+int tower_backward(const float* X, const int64_t* idx, int64_t n, int in_dim, const TowerW& w, const float* H1, const float* H2, const float* dZ3, float* tmpA, float* tmpB, float* g_w0,
                    float* g_b0, float* g_w1, float* g_b1, float* g_w2, float* g_b2, cudaStream_t st) {
   const int64_t rows_per_split = 4096;
   const int splits = (int)((n + rows_per_split - 1) / rows_per_split);
@@ -455,42 +430,29 @@ int tower_backward(const float* X, const int64_t* idx, int64_t n, int in_dim, co
   auto wgrad = [&](const float* dZ, const float* Hin, const int64_t* in_rows, int in_ld, float* gw, float* gb,
                    bool need_colsum) -> int {
     // gw[256, in_ld] += dZ^T [256, n] . Hin [n, in_ld]
-    int ee;
-    if (ws && !in_rows && (in_ld % rb::tc::BK == 0) && in_ld <= 256) {  // tensor cores (3xTF32)
-      ee = rb::tc::wgrad(dZ, Hin, gw, n, in_ld, st);
-    } else {  // fp32 SIMT, split over samples, atomics
-      GemmArgs g{};
-      g.A = dZ; g.lda = kH; g.B = Hin; g.ldb = in_ld; g.b_rows = in_rows; g.C = gw;
-      g.ldc = in_ld; g.M = kH; g.N = in_ld; g.K = n; g.k_per_split = rows_per_split;
-      ee = launch_gemm<A_MCONTIG, B_NCONTIG, EPI_ATOMIC>(g, splits, st);
-    }
+    // split over samples, atomics
+    GemmArgs g{};
+    g.A = dZ; g.lda = kH; g.B = Hin; g.ldb = in_ld; g.b_rows = in_rows; g.C = gw;
+    g.ldc = in_ld; g.M = kH; g.N = in_ld; g.K = n; g.k_per_split = rows_per_split;
+    const int ee = launch_gemm<A_MCONTIG, B_NCONTIG, EPI_ATOMIC>(g, splits, st);
     if (ee || !need_colsum) return ee;
     return colsum(dZ, gb);
   };
-  auto dgrad = [&](const float* dZ, const float* W, const float* Wth, const float* Wtl, const float* Hprev,
-                   float* out, float* gb_prev) -> int {
-    // out = (dZ . W) * (1 - Hprev^2); the tensor-core epilogue also adds out's column sums to gb_prev
-    if (Wth) {
-      rb::tc::Params p{};
-      p.M = n; p.K = kH; p.h = Hprev; p.c = out; p.colsum = gb_prev; p.epi = rb::tc::EPI_TANHGRAD;
-      return rb::tc::launch(dZ, Wth, Wtl, p, st);
-    }
+  auto dgrad = [&](const float* dZ, const float* W, const float* Hprev, float* out) -> int {
+    // out = (dZ . W) * (1 - Hprev^2)
     GemmArgs g{};
     g.A = dZ; g.lda = kH; g.B = W; g.ldb = kH; g.C = out; g.ldc = kH; g.aux = Hprev;
     g.ldaux = kH; g.M = n; g.N = kH; g.K = kH; g.k_per_split = 1 << 30;
     return launch_gemm<A_KCONTIG, B_NCONTIG, EPI_TANHGRAD>(g, 1, st);
   };
-  const bool tc = ws != nullptr;  // tensor-core dgrad adds the bias gradients of layers 2 and 1 in its epilogue
   if ((e = wgrad(dZ3, H2, nullptr, kH, g_w2, g_b2, false))) return e;  // g_b2: head_bwd_kernel
-  if ((e = dgrad(dZ3, w.w2, ws ? ws->w2th : nullptr, ws ? ws->w2tl : nullptr, H2, tmpA, g_b1))) return e;  // dZ2
-  if ((e = wgrad(tmpA, H1, nullptr, kH, g_w1, g_b1, !tc))) return e;
-  if ((e = dgrad(tmpA, w.w1, ws ? ws->w1th : nullptr, ws ? ws->w1tl : nullptr, H1, tmpB, g_b0))) return e;  // dZ1
-  return wgrad(tmpB, X, idx, in_dim, g_w0, g_b0, !tc);
+  if ((e = dgrad(dZ3, w.w2, H2, tmpA))) return e;  // dZ2
+  if ((e = wgrad(tmpA, H1, nullptr, kH, g_w1, g_b1, true))) return e;
+  if ((e = dgrad(tmpA, w.w1, H1, tmpB))) return e;  // dZ1
+  return wgrad(tmpB, X, idx, in_dim, g_w0, g_b0, true);
 }
 
-// ---- round 2: fp16-split tensor-core path (tc_gemm_h.cu), both towers per launch -------------------------------------------
-// debug flag bit 3 (value 8) selects the round-1 3xTF32 kernels instead.
-inline bool half_mode() { return (rb::tc::g_debug_flags & 8) == 0; }
+// ---- fp16-split tensor-core path (tc_gemm_h.cu), both towers per launch ------------------------------------------------
 
 struct TowerWH {  // packed fp16 (hi, lo) tiles of w * 2^10 (rb::tch::split_weights); typed float* (they live in the wsplit buffer)
   const float *w0f, *w1f, *w2f;  // forward packs of layers 0..2
@@ -517,7 +479,7 @@ int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, 
     if ((e = rb::tch::launch(g, nt, n, in_dim, rb::tc::EPI_BIAS_TANH, 0, st))) return e;
   } else {
     for (int i = 0; i < nt; ++i)
-      if ((e = layer_forward(X, idx, n, in_dim, t[i].w.w0, t[i].w.b0, nullptr, nullptr, t[i].H1, st))) return e;
+      if ((e = layer_forward(X, idx, n, in_dim, t[i].w.w0, t[i].w.b0, t[i].H1, st))) return e;
   }
   for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{t[i].H1, t[i].wh.w1f, nullptr, t[i].H2, t[i].w.b1, nullptr, nullptr, nullptr, nullptr};
   if ((e = rb::tch::launch(g, nt, n, kH, rb::tc::EPI_BIAS_TANH, 0, st))) return e;
@@ -581,6 +543,11 @@ extern "C" int rb200_mlp_layout_init(rb200_mlp_layout* L, int obs_dim, int act_d
   L->bw2 = take((int64_t)hidden * hidden); L->bb2 = take(hidden);
   L->mw = take((int64_t)act_dim * hidden); L->mb = take(act_dim);
   L->total = (o + 3) & ~int64_t(3);
+  // size the per-CTA partial-sum scratch of the backward for this layout now, outside any CUDA-graph capture (largest
+  // of: head_bwd <= 4 blocks per SM, wgrad <= SMs / 2 chunk slots of 256 x 256, dgrad column sums); no device: no-op
+  const int64_t sms = rb::sm_count(), head = 4 * sms * ((act_dim + value_dim) * hidden + 64 + 2 * hidden);
+  const int64_t wg = sms / 2 * hidden * hidden;
+  if (!rb::partials_scratch(head > wg ? head : wg)) (void)cudaGetLastError();
   return RB200_OK;
 }
 
@@ -593,9 +560,9 @@ extern "C" int64_t rb200_mlp_fwd_scratch_floats(const rb200_mlp_layout* L, int64
   return 6 * act_floats(n) + n * L->act_dim + 64;
 }
 
-// wsplit layout (floats), per tower (value tower first, then backbone), every block 16-byte aligned:
-//   w0h w0l [256*obs] | w1h w1l w2h w2l [65536 each] | w1th w1tl w2th w2tl [65536 each]
-static inline int64_t wsplit_tower_floats(int obs) { return 2ll * kH * obs + 8ll * kH * kH; }
+// wsplit: the fp16-split weight cache, per tower (value tower first, then backbone), 4 bytes (hi + lo) per weight:
+//   forward packs of w0 [256*obs floats of storage], w1, w2 [65536 each] | dgrad packs of w1, w2 [65536 each]
+static inline int64_t wsplit_tower_floats(int obs) { return (int64_t)kH * obs + 4ll * kH * kH; }
 
 extern "C" int64_t rb200_mlp_wsplit_floats(const rb200_mlp_layout* L) {
   if (!L) return 0;
@@ -619,22 +586,9 @@ TowerW tower_w(const rb200_mlp_layout* L, const float* P, bool value) {
   }
   return w;
 }
-TowerWS tower_ws(const rb200_mlp_layout* L, const float* ws, bool value) {
-  const float* b = ws + (value ? 0 : wsplit_tower_floats(L->obs_dim));
-  const int64_t n0 = (int64_t)kH * L->obs_dim, nn = (int64_t)kH * kH;
-  TowerWS t;
-  t.w0h = b; t.w0l = b + n0;
-  const float* q = b + 2 * n0;
-  t.w1h = q; t.w1l = q + nn; t.w2h = q + 2 * nn; t.w2l = q + 3 * nn;
-  t.w1th = q + 4 * nn; t.w1tl = q + 5 * nn; t.w2th = q + 6 * nn; t.w2tl = q + 7 * nn;
-  return t;
-}
-// fp16-split cache, per tower (value tower first): forward packs of w0 [256*obs floats of storage], w1, w2 [65536 each],
-// then the dgrad packs of w1, w2; it needs less than the TF32 cache, so it lives in the same buffer
 TowerWH tower_wh(const rb200_mlp_layout* L, const float* ws, bool value) {
   const int64_t n0 = (int64_t)kH * L->obs_dim, nn = (int64_t)kH * kH;  // floats of storage (4 bytes per element: hi + lo)
-  const int64_t per_tower = n0 + 4 * nn;
-  const float* b = ws + (value ? 0 : per_tower);
+  const float* b = ws + (value ? 0 : wsplit_tower_floats(L->obs_dim));
   TowerWH t;
   t.w0f = b;
   t.w1f = b + n0;
@@ -645,42 +599,26 @@ TowerWH tower_wh(const rb200_mlp_layout* L, const float* ws, bool value) {
 }
 }  // namespace
 
-// Refresh the weight copies the tensor-core GEMMs read: packed fp16 (hi, lo) tiles in ONE launch (default), or the
-// exact-TF32 (hi, lo) copies of the round-1 kernels (debug flag 8; 2 x 10 tiny kernels). Call after every parameter update
-// (once per optimiser step / once per rollout).
+// Refresh the weight copies the tensor-core GEMMs read: packed fp16 (hi, lo) tiles of w * 2^10 for all hidden matrices,
+// in ONE launch.  Call after every parameter update (once per optimiser step / once per rollout).
 extern "C" int rb200_mlp_prepare_weights(const rb200_mlp_layout* L, const float* params, float* wsplit,
                                          rb200_stream_t stream) {
   int e = check_layout(L);
   if (e) return e;
   if (!params || !wsplit) return RB200_E_NULL;
-  cudaStream_t st = rb::as_stream(stream);
-  if (half_mode()) {  // fp16 (hi, lo) of w * 2^10 for all hidden matrices: ONE launch (round 1: 20 kernels)
-    rb::tch::SplitSpec sp[6];
-    int cnt = 0;
-    for (int v = 0; v < 2; ++v) {
-      if (v == 0 && L->value_dim == 0) continue;
-      const TowerW w = tower_w(L, params, v == 0);
-      const TowerWH t = tower_wh(L, wsplit, v == 0);
-      const int64_t n0 = (int64_t)kH * L->obs_dim, nn = (int64_t)kH * kH;
-      if (L->obs_dim % rb::tc::BK == 0)  // layer 0 runs on the tensor cores only then
-        sp[cnt++] = rb::tch::SplitSpec{w.w0, const_cast<float*>(t.w0f), nullptr, n0};
-      sp[cnt++] = rb::tch::SplitSpec{w.w1, const_cast<float*>(t.w1f), const_cast<float*>(t.w1d), nn};
-      sp[cnt++] = rb::tch::SplitSpec{w.w2, const_cast<float*>(t.w2f), const_cast<float*>(t.w2d), nn};
-    }
-    return rb::tch::split_weights(sp, cnt, st);
-  }
+  rb::tch::SplitSpec sp[6];
+  int cnt = 0;
   for (int v = 0; v < 2; ++v) {
     if (v == 0 && L->value_dim == 0) continue;
     const TowerW w = tower_w(L, params, v == 0);
-    const TowerWS t = tower_ws(L, wsplit, v == 0);
+    const TowerWH t = tower_wh(L, wsplit, v == 0);
     const int64_t n0 = (int64_t)kH * L->obs_dim, nn = (int64_t)kH * kH;
-    if ((e = rb::tc::split(w.w0, const_cast<float*>(t.w0h), const_cast<float*>(t.w0l), n0, st))) return e;
-    if ((e = rb::tc::split(w.w1, const_cast<float*>(t.w1h), const_cast<float*>(t.w1l), nn, st))) return e;
-    if ((e = rb::tc::split(w.w2, const_cast<float*>(t.w2h), const_cast<float*>(t.w2l), nn, st))) return e;
-    if ((e = rb::tc::split_transpose(w.w1, const_cast<float*>(t.w1th), const_cast<float*>(t.w1tl), kH, kH, st))) return e;
-    if ((e = rb::tc::split_transpose(w.w2, const_cast<float*>(t.w2th), const_cast<float*>(t.w2tl), kH, kH, st))) return e;
+    if (L->obs_dim % rb::tc::BK == 0)  // layer 0 runs on the tensor cores only then
+      sp[cnt++] = rb::tch::SplitSpec{w.w0, const_cast<float*>(t.w0f), nullptr, n0};
+    sp[cnt++] = rb::tch::SplitSpec{w.w1, const_cast<float*>(t.w1f), const_cast<float*>(t.w1d), nn};
+    sp[cnt++] = rb::tch::SplitSpec{w.w2, const_cast<float*>(t.w2f), const_cast<float*>(t.w2d), nn};
   }
-  return RB200_OK;
+  return rb::tch::split_weights(sp, cnt, rb::as_stream(stream));
 }
 
 extern "C" int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params, const float* wsplit,
@@ -697,19 +635,14 @@ extern "C" int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params,
   float *H1 = acts, *H2 = H1 + PF, *H3 = H2 + PF, *G1 = H3 + PF, *G2 = G1 + PF, *G3 = G2 + PF;
   float* mean = G3 + PF;
   const float* P = params;
-  const TowerWS bws = wsplit ? tower_ws(L, wsplit, false) : TowerWS{};
-  const TowerWS vws = wsplit ? tower_ws(L, wsplit, true) : TowerWS{};
-  if (wsplit && half_mode()) {
+  if (wsplit) {
     TowerIO t[2] = {};
     t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
     t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
     if ((e = towers_forward_h(states, idx, n, L->obs_dim, t, values ? 2 : 1, st))) return e;
   } else {
-    if ((e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, false), wsplit ? &bws : nullptr, H1, H2, H3, st)))
-      return e;
-    if (values &&
-        (e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, true), wsplit ? &vws : nullptr, G1, G2, G3, st)))
-      return e;
+    if ((e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
+    if (values && (e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
   }
   HeadFwdArgs h{};
   h.h3 = H3; h.g3 = values ? G3 : nullptr; h.mw = P + L->mw; h.mb = P + L->mb;
@@ -743,7 +676,7 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params
   h.g_mw = G + L->mw; h.g_mb = G + L->mb; h.g_logstd = G + L->logstd; h.g_vw3 = G + L->vw3;
   h.g_b2 = G + L->bb2; h.g_vb2 = G + L->vb2;
   h.n = n; h.act = L->act_dim; h.vdim = L->value_dim;
-  const bool use_h = wsplit && half_mode();
+  const bool use_h = wsplit != nullptr;
   float* amax = work + 6 * PF;  // 8 floats of the scratch tail: max|dZ3|,|dZ2|,|dZ1| of the policy tower, then the value tower
   if (use_h) {
     cudaError_t ce = cudaMemsetAsync(amax, 0, 8 * sizeof(float), st);
@@ -751,21 +684,45 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params
     h.amax_dz3 = amax;
     h.amax_dy3 = amax + 3;
   }
-  const size_t smem = sizeof(float) * ((size_t)2 * (L->act_dim + L->value_dim) * kH + 64 + 2 * kH);
+  const int acc_len = (L->act_dim + L->value_dim) * kH + 64 + 2 * kH, w_len = (L->act_dim + L->value_dim) * kH;
+  int nw = (232448 / 4 - w_len) / acc_len;  // warps per block: one accumulator copy each
+  nw = nw > 8 ? 8 : nw;
+  const size_t smem = sizeof(float) * ((size_t)w_len + (size_t)nw * acc_len);
   const bool reg = L->act_dim <= 8 && L->value_dim <= 2;
-  if (smem > 48 * 1024) {
-    cudaError_t ce = cudaFuncSetAttribute(head_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)smem);
+  const int grid = head_grid(n);
+  if (!(h.part = rb::partials_scratch((int64_t)grid * acc_len))) return RB200_E_UNSUPPORTED;
+  {
+    cudaError_t ce = cudaFuncSetAttribute(head_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (ce == cudaSuccess)
+      ce = cudaFuncSetAttribute(head_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (ce != cudaSuccess) return (int)ce;
   }
   if (reg)
-    head_bwd_kernel<true><<<head_grid(n), 256, smem, st>>>(h);
+    head_bwd_kernel<true><<<grid, 32 * nw, smem, st>>>(h);
   else
-    head_bwd_kernel<false><<<head_grid(n), 256, smem, st>>>(h);
+    head_bwd_kernel<false><<<grid, 32 * nw, smem, st>>>(h);
   rb::count_launch();
   {
     cudaError_t ce = cudaPeekAtLastError();
     if (ce != cudaSuccess) return (int)ce;
+  }
+  {  // per-block sums -> gradients, in block order
+    rb::tch::SlotSums ss{};
+    ss.nslab = grid;
+    ss.stride = acc_len;
+    const int A = L->act_dim, V = L->value_dim;
+    auto seg = [&](int off, float* out, int len) {
+      ss.part[ss.count] = h.part + off; ss.out[ss.count] = out; ss.len[ss.count++] = len;
+    };
+    seg(0, h.g_mw, A * kH);
+    seg((A + V) * kH, h.g_mb, A);
+    seg((A + V) * kH + 32, h.g_logstd, A);
+    seg((A + V) * kH + 64, h.g_b2, kH);
+    if (d_values) {
+      seg(A * kH, h.g_vw3, V * kH);
+      seg((A + V) * kH + 64 + kH, h.g_vb2, kH);
+    }
+    if ((e = rb::tch::sum_slots(ss, st))) return e;
   }
   if (use_h) {
     TowerIO t[2] = {};
@@ -779,42 +736,16 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params
     t[1].g_w2 = G + L->vw2; t[1].g_b2 = G + L->vb2; t[1].amax = amax + 3;
     return towers_backward_h(states, idx, n, L->obs_dim, t, d_values ? 2 : 1, st);
   }
-  const TowerWS bws = wsplit ? tower_ws(L, wsplit, false) : TowerWS{};
-  const TowerWS vws = wsplit ? tower_ws(L, wsplit, true) : TowerWS{};
-  if ((e = tower_backward(states, idx, n, L->obs_dim, tower_w(L, P, false), wsplit ? &bws : nullptr, H1, H2,
+  if ((e = tower_backward(states, idx, n, L->obs_dim, tower_w(L, P, false), H1, H2,
                           dZ3, tA, tB, G + L->bw0, G + L->bb0, G + L->bw1, G + L->bb1, G + L->bw2, G + L->bb2, st)))
     return e;
   if (d_values &&
-      (e = tower_backward(states, idx, n, L->obs_dim, tower_w(L, P, true), wsplit ? &vws : nullptr, G1, G2,
+      (e = tower_backward(states, idx, n, L->obs_dim, tower_w(L, P, true), G1, G2,
                           dY3, uA, uB,
                           G + L->vw0, G + L->vb0, G + L->vw1, G + L->vb1, G + L->vw2, G + L->vb2, st)))
     return e;
   return RB200_OK;
 }
-
-namespace {
-// Rollout-sized batches (a few thousand rows) give each tower GEMM only n/128 CTAs: the actor and the value tower are
-// independent until the head kernel, so they run concurrently on a forked side stream (fork/join with events; legal
-// inside CUDA-graph capture, where it becomes two parallel branches of the graph).
-struct SideStream {
-  cudaStream_t s = nullptr;
-  cudaEvent_t fork = nullptr, join = nullptr;
-  bool ok = false;
-};
-SideStream& side_stream() {
-  static SideStream ss;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    if (cudaStreamCreateWithFlags(&ss.s, cudaStreamNonBlocking) == cudaSuccess &&
-        cudaEventCreateWithFlags(&ss.fork, cudaEventDisableTiming) == cudaSuccess &&
-        cudaEventCreateWithFlags(&ss.join, cudaEventDisableTiming) == cudaSuccess)
-      ss.ok = true;
-    if (!ss.ok) (void)cudaGetLastError();
-  }
-  return ss;
-}
-}  // namespace
 
 // work: 6 activation tensors; rb200_mlp_fwd_scratch_floats(L, n) floats is always enough
 extern "C" int rb200_mlp_sample(const rb200_mlp_layout* L, const float* params, const float* wsplit,
@@ -829,45 +760,14 @@ extern "C" int rb200_mlp_sample(const rb200_mlp_layout* L, const float* params, 
   const int64_t PF = act_floats(n);
   float *H1 = work, *H2 = H1 + PF, *H3 = H2 + PF, *G1 = H3 + PF, *G2 = G1 + PF, *G3 = G2 + PF;
   const float* P = params;
-  const TowerWS bws = wsplit ? tower_ws(L, wsplit, false) : TowerWS{};
-  const TowerWS vws = wsplit ? tower_ws(L, wsplit, true) : TowerWS{};
-  const bool use_h = wsplit != nullptr && half_mode();
-  if (use_h) {  // both towers in one grouped launch per layer (no side stream needed)
+  if (wsplit) {  // both towers in one grouped launch per layer
     TowerIO t[2] = {};
     t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
     t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
     if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, st))) return e;
-  }
-  // few tiles per GEMM -> run the two towers side by side
-  const bool fork = !use_h && values != nullptr && wsplit != nullptr && n <= (int64_t)64 * rb::sm_count();
-  SideStream* ss = nullptr;
-  if (fork) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    (void)cudaStreamIsCapturing(st, &cs);
-    static bool created_outside_capture = false;  // never create streams / events while capturing
-    if (cs == cudaStreamCaptureStatusNone || created_outside_capture) {
-      SideStream& r = side_stream();
-      created_outside_capture = true;
-      if (r.ok) ss = &r;
-    }
-  }
-  if (ss) {
-    cudaError_t ce = cudaEventRecord(ss->fork, st);
-    if (ce == cudaSuccess) ce = cudaStreamWaitEvent(ss->s, ss->fork, 0);
-    if (ce != cudaSuccess) return (int)ce;
-    if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true), &vws, G1, G2, G3, ss->s))) return e;
-    ce = cudaEventRecord(ss->join, ss->s);
-    if (ce != cudaSuccess) return (int)ce;
-  }
-  if (!use_h && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, false), wsplit ? &bws : nullptr, H1, H2,
-                                   H3, st)))
-    return e;
-  if (ss) {
-    cudaError_t ce = cudaStreamWaitEvent(st, ss->join, 0);
-    if (ce != cudaSuccess) return (int)ce;
-  } else if (!use_h && values && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true),
-                                          wsplit ? &vws : nullptr, G1, G2, G3, st))) {
-    return e;
+  } else {
+    if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
+    if (values && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
   }
   HeadFwdArgs h{};
   h.h3 = H3; h.g3 = values ? G3 : nullptr; h.mw = P + L->mw; h.mb = P + L->mb;
@@ -910,24 +810,14 @@ extern "C" int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, c
   cudaStream_t st = rb::as_stream(stream);
   const int64_t PF = act_floats(n);
   float *G1 = work, *G2 = G1 + PF, *G3 = G2 + PF;
-  const TowerWS vws = wsplit ? tower_ws(L, wsplit, true) : TowerWS{};
-  if (wsplit && half_mode()) {
+  if (wsplit) {
     TowerIO t[1] = {};
     t[0].w = tower_w(L, params, true); t[0].wh = tower_wh(L, wsplit, true); t[0].H1 = G1; t[0].H2 = G2; t[0].H3 = G3;
     if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, 1, st))) return e;
-  } else if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, params, true), wsplit ? &vws : nullptr, G1, G2,
-                                G3, st))) {
+  } else if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, params, true), G1, G2, G3, st))) {
     return e;
   }
   value_head_kernel<<<head_grid(n), 256, 0, st>>>(G3, params + L->vw3, values, n, L->value_dim);
   rb::count_launch();
   RB_RETURN_LAUNCH();
-}
-
-// x -> exact-TF32 (hi, lo) pair (hi + lo ~= x to 2^-22). Lets the caller split the shuffled observations once per
-// iteration instead of once per forward call.
-extern "C" int rb200_split_tf32(const float* x, float* hi, float* lo, int64_t n, rb200_stream_t stream) {
-  if (!x || !hi || !lo) return RB200_E_NULL;
-  if (n <= 0) return RB200_E_SHAPE;
-  return rb::tc::split(x, hi, lo, n, rb::as_stream(stream));
 }

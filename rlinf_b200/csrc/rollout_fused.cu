@@ -11,8 +11,8 @@
 // fused heads (Normal sample with Philox or supplied noise, log-prob, value), the env dynamics (s.W_s + a.W_a, tanh,
 // reward, termination / truncation, auto-reset) and the truncation bootstrap r += gamma * V(final_obs), which needs
 // an extra value-tower pass only in steps where one of the CTA's environments was flagged.
-// The graph version of the same loop (rollout.py) launches ~16 kernels per step, each with B/128 tiles on 148 SMs:
-// 105 us / step at B = 4096 and hardly less at B = 512 (8-GPU strong scaling); here a step costs E * 346k FMA per SM
+// The graph version of the same loop (rollout.py) launches ~16 kernels per step, each with B/128 tiles, so small
+// per-rank batches are launch-latency bound; here a step costs E * 346k FMA per SM
 // (B = 4096: E = 28) or the 1.3 MB weight stream from L2 (small E).
 // Same random streams as the per-kernel path: policy Philox(seed_p, row*act + a, offset + c_p + t), env
 // Philox(seed_e, row*32 + lane, (c_e + t) * 64) with the same draw order, so both paths generate the same episode
@@ -140,8 +140,8 @@ __device__ __forceinline__ void layer_tiled(const float* __restrict__ in_s, int 
 
 // ---- deeper software pipelining (the default since round 2; rb200_debug_set_flags bit 1 = round-1 kernels) ----------
 // Same arithmetic, same k-ascending fmaf order (bit-identical results), but the weight rows of the next D k-steps
-// are in flight instead of one: with 8 warps / SM the one-k-step prefetch leaves the L2 latency exposed (round 1:
-// 45 us / env step at E = 4 although the FMA work is ~2 us).  Requires K % (4 * D) == 0.
+// are in flight instead of one: with 8 warps / SM the one-k-step prefetch leaves the L2 latency exposed.  Requires
+// K % (4 * D) == 0.
 template <int EMAX, int D>
 __device__ __forceinline__ void layer_pf(const float* __restrict__ in_s, int K, const float* __restrict__ Wt,
                                          const float* __restrict__ bias, float* __restrict__ out_s, int j) {
@@ -499,8 +499,8 @@ int launch_fused_pf(const FusedArgs& a, int grid, cudaStream_t st) {
 
 template <int EMAX>
 int launch_fused(const FusedArgs& a, int grid, cudaStream_t st) {
-  // default: weight rows of the next 4 k-steps in flight (validated on B200 in round 2: bit-identical buffers for all
-  // four template instances, 23.1 -> 19.1 ms per 512-step rollout at 512 envs); debug bit 1 selects the round-1 kernels
+  // default: weight rows of the next 4 k-steps in flight (bit-identical buffers, tests/test_gpu_runner.py); debug bit 1
+  // selects the one-k-step prefetch
   if (rb::tc::g_debug_flags & 2) return launch_fused_pf<EMAX, 0>(a, grid, st);
   return launch_fused_pf<EMAX, 4>(a, grid, st);
 }

@@ -1,31 +1,19 @@
 // Persistent tensor-core rollout: the whole T-step actor/critic inference + synthetic-env loop of one rank in ONE kernel,
-// with every hidden layer (and the env's s.W_s product) on tcgen05.
-//
-// Reference loop replaced: EnvWorker.interact / MultiStepRolloutWorker.generate (rlinf/workers/env/env_worker.py:
-// 1059-1349, rlinf/workers/rollout/hf/huggingface_worker.py:678-781) for the MLP policy
-// (models/embodiment/mlp_policy/mlp_policy.py:256-321) with the device-resident synthetic env (rollout.cu); same buffers,
-// row alignment, random streams and draw order as rollout_fused.cu / the per-kernel CUDA-graph path.
-//
-// Why: rollout_fused.cu does the layers with fp32 SIMT FMAs (40 us / env step at 28 envs per SM) and the per-kernel
-// graph pays ~16 dependent launches per env step (105 us / step at any B).  Here CTA c owns environments
-// [32c, 32c+32) for the whole rollout and computes every layer TRANSPOSED on the tensor cores:
-//     D[hidden unit (M = 128 per tile), env (N = 32)] = W[128 x K] . X^T      (tcgen05.mma kind::f16, fp32 accumulate)
-// with the same 2-way fp16 split as tc_gemm_h.cu (w = w_hi + w_lo, x = x_hi + x_lo, three MMAs per product, 2^-22
-// truncation): weights are the A operand (pre-split, pre-swizzled, streamed from L2 by 16 KB bulk copies in exactly
-// the order the MMAs consume them), activations are the B operand (K-major SWIZZLE_64B tiles written by the epilogue
-// warps straight from TMEM: thread = hidden unit, 32 environment columns per tcgen05.ld).  Layer-3 outputs are written as
-// fp32 [env][256] instead and feed the exact-fp32 heads (mean / value dot products, Normal sampling).
-// Warp roles (448 threads): 0 = weight-stream producer, 1 = MMA issuer, 2-5 = actor tower epilogues + heads + sampling,
-// 6-9 = value tower epilogues + value head + truncation bootstrap, 10-13 = env warps (Philox noise one phase ahead,
-// env pre-activation out of TMEM, tanh / reward / termination / auto-reset, next observation operand).
-// Truncation bootstrap r += gamma * V(final_obs): the value tower of step t+1 runs with N = 64 columns when any of the
-// CTA's environments was flagged in step t (columns 32..63 = pre-reset observations); the weight stream is the same.
-// What bounds a step: the 1.3 MB weight stream per CTA (L2 -> SM), not the tensor pipe (504 MMAs of 16-32 clk).
+// every hidden layer (and the env's s.W_s product) on Hopper wgmma.  Replaces EnvWorker.interact /
+// MultiStepRolloutWorker.generate (rlinf/workers/env/env_worker.py:1059-1349, huggingface_worker.py:678-781) for the MLP
+// policy with the device-resident synthetic env; same buffers, row alignment, random streams and draw order as
+// rollout_fused.cu / the per-kernel CUDA-graph path.  CTA c owns environments [32c, 32c+32) and computes every layer
+// TRANSPOSED, D[hidden unit, env] = W . X^T, with the 2-way fp16 split of tc_gemm_h.cu (three MMAs per product).
+// Roles (416 threads): warpgroup 0 = env (Philox noise, x.W_s, dynamics finish, next observation operand), 1 = actor
+// tower (+ mean head, sampling), 2 = value tower (+ value head, truncation bootstrap), warp 12 = weight-stream producer
+// (one ring per warpgroup).  Each warpgroup issues its own layers and finishes them from its accumulator registers.
+// The truncation bootstrap rides in 32 extra columns (N = 64) of the next step's value tower.
 #include <cuda_fp16.h>
 #include <curand_kernel.h>
 
 #include "common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -39,13 +27,13 @@ constexpr int kNE = 32;        // environments per CTA (MMA N)
 constexpr int kMaxActTc = 8;   // action dims held in shared memory
 constexpr int kMaxObsTc = 128; // one M tile of the env product
 constexpr int kStageBytes = 16384, kHalfTile = 8192;  // [128 rows x 32 k] fp16 hi | lo
-constexpr int kStages = 5;  // (the MMA issue loop switches over the 5 slots)
-static_assert(kStages == 5, "rollout_tc issue switch");
-constexpr int kThreads = 14 * 32;
+// One weight ring per consuming warpgroup: with a shared ring a warpgroup a lap ahead would take a slot's old phase.
+constexpr int kStages = 5;
+constexpr int kEnvSlot0 = 0, kEnvSlots = 1, kActSlot0 = 1, kActSlots = 2, kValSlot0 = 3, kValSlots = 2;
+static_assert(kValSlot0 + kValSlots == kStages, "ring slots");
+constexpr int kThreads = 13 * 32;
 constexpr int kWScaleLog2 = 10;  // weights are stored as fp16 (hi, lo) of w * 2^10
 constexpr float kHalfLog2Pi = 0.91893853320467274178f;
-constexpr uint32_t kTmemCols = 256;
-constexpr uint32_t kAccA = 0, kAccV = 64, kAccEnv = 192;  // TMEM column offsets
 
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr int kOffRing = 0;
@@ -67,9 +55,8 @@ struct Misc {
   int flag[kNE];
   int el[kNE];
   int nflag;
-  uint32_t tmem_base;
   uint64_t full[kStages], empty[kStages];
-  uint64_t acc_a, acc_v, acc_env, opnd_a, opnd_v, vhead, obs_ready;
+  uint64_t vhead, obs_ready;
 };
 constexpr int kArgsBytes = 512;  // shared-memory copy of the kernel arguments for the out-of-line helpers
 constexpr int kSmemBytes = kOffMisc + (int)sizeof(Misc) + kArgsBytes + 1024;
@@ -99,50 +86,9 @@ struct TcArgs {
   int T, B, obs, act;
   int max_episode_steps, auto_reset, bootstrap_on_done;
   float gamma, p_term, noise_std, reward_noise_std;
-  int dbg;               // ablation switches for tools/rollout_tc_probe.py (0 in production), see rb200_rollout_tc_debug
-  long long* prof;       // [16] wait-cycle counters of CTA 0 (PROF instantiation only)
 };
 static_assert(sizeof(TcArgs) <= kArgsBytes, "TcArgs shared-memory copy");
 
-// ---- PTX wrappers (same instructions as tc_gemm_h.cu) ---------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-      ::"r"(d_tmem), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-      "%24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 // 1-D bulk copy global -> shared, completion counted on an mbarrier
 __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -150,24 +96,10 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// one lane of a converged warp; the compiler emits the tcgen05 instructions under it directly (a plain `lane == 0`
-// branch makes it wrap every UTCHMMA in an elect / loop-over-active-lanes sequence: ~9 instructions per MMA)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
 __device__ __forceinline__ void named_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 // byte offset of element (row, k in [0,32)) inside a [rows x 32 fp16] SWIZZLE_64B tile
 __device__ __forceinline__ uint32_t sw64_off(int row, int kk) {
   return (uint32_t)(row * 64 + ((((kk >> 3) ^ ((row >> 1) & 3))) << 4) + (kk & 7) * 2);
@@ -209,51 +141,6 @@ __host__ __device__ inline Segs make_segs(int obs) {
   s.v2 = s.a1 + 48;
   s.total = s.a1 + 64;
   return s;
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-
-// Layer epilogue of one tower, ONE out-of-line copy shared by the actor and the value warps (they run it at the same
-// time: shared instruction-cache lines): thread = hidden unit j = m*128 + q*32 + lane of both M tiles, `ncol`
-// environment columns per tile read from TMEM 8 at a time; out = tanh(acc * 2^-10 + bias) written either as the next
-// layer's operand (fp16 hi | lo, K-major SWIZZLE_64B tiles of `rows` environment rows, k-block = j / 32, k = lane) or,
-// for the last layer, as fp32 [env][256] for the heads.
-__device__ __noinline__ void tower_epilogue(uint32_t tq, int ncol, uint8_t* buf, uint32_t half_bytes, uint32_t kb_bytes,
-                                            int q, int lane, float b0, float b1, int last, int skip_math) {
-  const float out_scale = 1.0f / (float)(1 << kWScaleLog2);
-  // byte offset of (row r, k = lane) inside a k-block tile: r*64 + (((lane>>3) ^ ((r>>1)&3)) << 4) + (lane&7)*2; for
-  // r = 8*g + j the swizzle term depends on j only
-  uint32_t xl[4];
-#pragma unroll
-  for (int sft = 0; sft < 4; ++sft) xl[sft] = (uint32_t)((((lane >> 3) ^ sft) << 4) + (lane & 7) * 2);
-  float* f32 = reinterpret_cast<float*>(buf);
-#pragma unroll 1
-  for (int m = 0; m < 2; ++m) {
-    const float b = m ? b1 : b0;
-    const uint32_t kb_off = (uint32_t)(m * 4 + q) * kb_bytes;
-    const int j = m * 128 + q * 32 + lane;
-#pragma unroll 1
-    for (int g = 0; g < ncol / 8; ++g) {
-      uint32_t r[8];
-      tmem_ld8(tq + (uint32_t)(m * ncol + g * 8), r);
-      tmem_ld_wait();
-      if (skip_math) continue;
-      if (!last) {
-        const uint32_t base = kb_off + (uint32_t)g * 512u;
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          store_split(buf, half_bytes, base + (uint32_t)i * 64u + xl[(i >> 1) & 3], tanh_fast(__uint_as_float(r[i]) * out_scale + b));
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f32[(g * 8 + i) * kH + j] = tanh_fast(__uint_as_float(r[i]) * out_scale + b);
-      }
-    }
-  }
 }
 
 // ---- Philox draws as out-of-line functions: inlined at every use (8 + 8 + 1 sites, ~700 instructions each) the kernel
@@ -303,7 +190,7 @@ __device__ __noinline__ float policy_draw(unsigned long long seed, unsigned long
 
 // Dynamics finish of 4 environments [w8*4, w8*4+4) by one warp (8 warps share a step: the actor group is idle once the
 // actions are sampled, so it takes half of the environments).  Array stages over the 4 environments - all loads, then
-// the math, then all stores - keep 4-16 independent chains in flight per lane.  zs = x.W_s out of TMEM, eps_s = this
+// the math, then all stores - keep 4-16 independent chains in flight per lane.  zs = x.W_s (env product), eps_s = this
 // step's N(0,1) draws, both fp32 [32][obs] in the (now free) actor buffer.  Same arithmetic order as env_finish_kernel
 // (rollout.cu) except tanh (MUFU-based tanh_fast, 3e-7 abs).
 __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obuf, uint32_t ob_half, const float* zs,
@@ -415,19 +302,94 @@ __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obu
   }
 }
 
-// wait on an mbarrier; the PROF instantiation accumulates the cycles spent waiting (tools/rollout_tc_probe.py)
-template <bool PROF>
-__device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity, long long& acc) {
-  if constexpr (PROF) {
-    const long long t0 = clock64();
-    mbar_wait(bar, parity);
-    acc += clock64() - t0;
-  } else {
-    mbar_wait(bar, parity);
+// D[hidden unit, env] = W . X^T for one layer, by one warpgroup: weight stages from its ring (k-block outer, 128-row tile
+// inner), X = fp16 hi | lo K-major tiles of N rows.  Accumulators stay in registers: the output overwrites X in place.
+template <int N, int NT>
+struct LayerAcc {
+  float d[NT][2][N / 2];
+};
+
+template <int N, int NT>
+__device__ __forceinline__ void layer_mma(LayerAcc<N, NT>& acc, Misc* ms, uint32_t ring_a, int slot0, int nslots,
+                                          uint32_t stage0, int nkb, uint32_t b_addr, uint32_t b_half, uint32_t b_kb_stride,
+                                          int lane) {
+#pragma unroll
+  for (int m = 0; m < NT; ++m)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) acc.d[m][h][i] = 0.f;
+#pragma unroll 1
+  for (int kb = 0; kb < nkb; ++kb) {
+    const uint32_t sb = b_addr + (uint32_t)kb * b_kb_stride;
+#pragma unroll
+    for (int m = 0; m < NT; ++m) {
+      const uint32_t idx = stage0 + (uint32_t)(kb * NT + m);
+      const uint32_t slot = (uint32_t)slot0 + idx % (uint32_t)nslots, ph = (idx / (uint32_t)nslots) & 1u;
+      mbar_wait(&ms->full[slot], ph);
+      const uint32_t a = ring_a + slot * kStageBytes;
+      rb::wg::fence();
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {  // two k-steps of 16 = 32 B along the 64-B rows
+        const uint64_t b_hi = rb::wg::desc(sb + k * 32, 16, 512, 2), b_lo = rb::wg::desc(sb + b_half + k * 32, 16, 512, 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {  // rows 64h .. 64h + 63 of the 128-row weight tile
+          const uint64_t a_hi = rb::wg::desc(a + h * 4096 + k * 32, 16, 512, 2);
+          const uint64_t a_lo = rb::wg::desc(a + kHalfTile + h * 4096 + k * 32, 16, 512, 2);
+          rb::wg::MmaSS<N>::run(acc.d[m][h], a_lo, b_hi, 1u);  // small terms first
+          rb::wg::MmaSS<N>::run(acc.d[m][h], a_hi, b_lo, 1u);
+          rb::wg::MmaSS<N>::run(acc.d[m][h], a_hi, b_hi, 1u);
+        }
+      }
+      rb::wg::commit();
+      rb::wg::wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ms->empty[slot]);
+    }
   }
 }
 
-template <bool PROF>
+// out = tanh(acc * 2^-10 + bias) as the next layer's fp16 operand or (last layer) fp32 [env][256]; units
+// j = 128 m + 64 h + 16 w + g (+ 8), environments e = 8 c + 2 t (+ 1).
+template <int N>
+__device__ __forceinline__ void layer_epilogue(const LayerAcc<N, 2>& acc, const float* bias, uint8_t* buf, uint32_t half_bytes,
+                                               uint32_t kb_bytes, int last, int w, int lane) {
+  const float out_scale = 1.0f / (float)(1 << kWScaleLog2);
+  const int g = lane >> 2, t = lane & 3;
+  float* f32 = reinterpret_cast<float*>(buf);
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int j = m * 128 + h * 64 + w * 16 + g + 8 * r;
+        const float b = __ldg(bias + j);
+#pragma unroll
+        for (int c = 0; c < N / 8; ++c)
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const int e = 8 * c + 2 * t + u;
+            const float v = tanh_fast(acc.d[m][h][4 * c + 2 * r + u] * out_scale + b);
+            if (last) f32[e * kH + j] = v;
+            else store_split(buf, half_bytes, (uint32_t)(j >> 5) * kb_bytes + sw64_off(e, j & 31), v);
+          }
+      }
+}
+
+// MMAs, barrier (the operand is read), epilogue, barrier (the next operand is complete).
+template <int N>
+__device__ __noinline__ void tower_layer(Misc* ms, uint32_t ring_a, int slot0, uint32_t stage0, int nkb, uint32_t b_addr,
+                                         uint32_t b_half, uint32_t b_kb_stride, const float* bias, uint8_t* buf,
+                                         uint32_t half_bytes, uint32_t kb_bytes, int last, int bar_id, int w, int lane) {
+  LayerAcc<N, 2> acc;
+  layer_mma<N, 2>(acc, ms, ring_a, slot0, 2, stage0, nkb, b_addr, b_half, b_kb_stride, lane);
+  named_sync(bar_id, 128);
+  layer_epilogue<N>(acc, bias, buf, half_bytes, kb_bytes, last, w, lane);
+  rb::tma::fence_proxy_async();
+  named_sync(bar_id, 128);
+}
+
 __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -451,6 +413,8 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
   const uint64_t c_e = p.counter_e ? p.counter_e[0] : 0ull;
   const float out_scale = 1.0f / (float)(1 << kWScaleLog2);
   const bool boot = p.auto_reset != 0;  // the value head exists (rb200_rollout_tc_supported)
+  const uint32_t ring_a = smem_u32(ring), obuf_a = smem_u32(obuf), abuf_a = smem_u32(abuf), vbuf_a = smem_u32(vbuf);
+  const uint32_t ob_half = (uint32_t)sg.nkb0 * 4096u;
 
   // ---- setup ----
   for (int i = tid; i < (int)(sizeof(TcArgs) / 4); i += kThreads)
@@ -458,28 +422,19 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&ms->full[s], 1);
-      mbar_init(&ms->empty[s], 1);
+      mbar_init(&ms->empty[s], 4);  // one arrival per warp of the consuming warpgroup
     }
-    mbar_init(&ms->acc_a, 1);
-    mbar_init(&ms->acc_v, 1);
-    mbar_init(&ms->acc_env, 1);
-    mbar_init(&ms->opnd_a, 4);
-    mbar_init(&ms->opnd_v, 4);
     mbar_init(&ms->vhead, 4);
     mbar_init(&ms->obs_ready, 1);
     ms->nflag = 0;
     rb::tma::fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(&ms->tmem_base, kTmemCols);
-    tmem_relinquish();
   }
   for (int i = tid; i < act * kH; i += kThreads) ms->mw[i] = P[p.L.mw + i];
   for (int i = tid; i < kH; i += kThreads) ms->vw[i] = P[p.L.vw3 + i];
   for (int i = tid; i < 2 * kNE * obs; i += kThreads) {  // rows 0..31 = current observation, rows 32..63 = zeros
     const int r = i / obs, c = i - r * obs;
     const float v = (r < nE) ? p.states[(size_t)(e0 + r) * obs + c] : 0.f;
-    store_split(obuf, (uint32_t)sg.nkb0 * 4096u, (uint32_t)(c >> 5) * 4096u + sw64_off(r, c & 31), v);
+    store_split(obuf, ob_half, (uint32_t)(c >> 5) * 4096u + sw64_off(r, c & 31), v);
   }
   for (int i = tid; i < kNE * kMaxActTc; i += kThreads) ms->act[i] = 0.f;
   if (tid < kNE) {
@@ -488,168 +443,55 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
     ms->rew[tid] = 0.f;
   }
   rb::tma::fence_proxy_async();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = ms->tmem_base;
-  long long pc[16];  // PROF: cycles spent per wait / section (dead code otherwise)
-#pragma unroll
-  for (int i = 0; i < 16; ++i) pc[i] = 0;
-  const long long t_start = PROF ? clock64() : 0;
-  const int dbg = PROF ? p.dbg : 0;  // ablations exist in the instrumented instantiation only
 
-  if (warp == 0) {
-    // ================= weight-stream producer =================
+  // per-step stream lengths (in stages) of the three consumers: env product, actor tower, value tower
+  const uint32_t n_env = (uint32_t)sg.nkb0, n_tower = 2u * (uint32_t)sg.nkb0 + 32u;
+  if (warp == 12) {
+    // ================= weight-stream producer: three rings, polled (no ring waits for another) =================
     if (lane == 0) {
-      uint32_t s = 0, ph = 0;
-      auto stream = [&](int stage0, int n) {
-        for (int i = 0; i < n; ++i, s = (s + 1 == kStages ? 0 : s + 1), ph ^= (s == 0 ? 1u : 0u)) {
-          wait_bar<PROF>(&ms->empty[s], ph ^ 1u, pc[0]);
-          if (dbg & 4) {  // ablation: no weight traffic (the ring keeps whatever it holds)
-            mbar_arrive(&ms->full[s]);
-            continue;
-          }
-          rb::tma::mbar_arrive_expect_tx(&ms->full[s], kStageBytes);
-          bulk_load(ring + s * kStageBytes, p.pack + (size_t)(stage0 + i) * kStageBytes, kStageBytes, &ms->full[s]);
-        }
-      };
-      for (int t = 0; t < T; ++t) stream(0, sg.total);
-      stream(sg.v0, 2 * sg.nkb0);  // tail: value tower on the last observation (bootstrap row T)
-      stream(sg.v1, 16);
-      stream(sg.v2, 16);
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer (the whole warp runs the schedule, one elected lane issues) =================
-    {
-      // The N = 32 MMAs are short (16-32 clk of tensor work): this single thread's issue rate is what bounds the
-      // tensor phase, so the loop is kept lean - ring slot / phase by counters, descriptors as {lo, hi} words with
-      // only the 14-bit address field changing (K-major SWIZZLE_64B: LBO 1, SBO 512 B, version 1, layout 4).
-      uint32_t slot = 0, ph = 0;
-      const uint32_t ring_a = smem_u32(ring), obuf_a = smem_u32(obuf), abuf_a = smem_u32(abuf), vbuf_a = smem_u32(vbuf);
-      constexpr uint32_t kDescHi = (uint32_t)(512 >> 4) | (1u << 14) | (4u << 29);  // bits 32..63 of desc_k_sw64
-      auto desc = [&](uint32_t addr) -> uint64_t {
-        return ((uint64_t)kDescHi << 32) | (uint64_t)(((addr & 0x3ffffu) >> 4) | (1u << 16));
-      };
-      // descriptors of the weight halves of every ring slot, computed once: the issue loop switches on the slot so
-      // that they are plain registers (one thread issues all 504 MMAs of a step; its instruction count per MMA is what
-      // bounds the tensor phase - the tensor pipe itself is ~12 % busy)
-      uint64_t ad_hi[kStages], ad_lo[kStages];
+      const uint32_t total[3] = {(uint32_t)T * n_env, (uint32_t)T * n_tower, (uint32_t)(T + 1) * n_tower};
+      const int slot0[3] = {kEnvSlot0, kActSlot0, kValSlot0}, nslots[3] = {kEnvSlots, kActSlots, kValSlots};
+      uint32_t j[3] = {0u, 0u, 0u};
+      while (j[0] < total[0] || j[1] < total[1] || j[2] < total[2]) {
 #pragma unroll
-      for (int i = 0; i < kStages; ++i) {
-        ad_hi[i] = desc(ring_a + i * kStageBytes);
-        ad_lo[i] = desc(ring_a + i * kStageBytes + kHalfTile);
-      }
-      auto issue6 = [&](uint32_t d_tmem, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, uint32_t idesc,
-                        uint32_t acc0) {
-        mma_f16(d_tmem, a_lo, b_hi, idesc, acc0);  // small terms first
-        mma_f16(d_tmem, a_hi, b_lo, idesc, 1u);
-        mma_f16(d_tmem, a_hi, b_hi, idesc, 1u);
-        mma_f16(d_tmem, a_lo + 2, b_hi + 2, idesc, 1u);  // next 16 fp16 = 32 B along the 64-B row
-        mma_f16(d_tmem, a_hi + 2, b_lo + 2, idesc, 1u);
-        mma_f16(d_tmem, a_hi + 2, b_hi + 2, idesc, 1u);
-      };
-      // one layer: D[tile m] (TMEM columns d_col + m*N) = W tile m [128 x 32*nkb] . operand[N rows x 32*nkb]^T
-      auto seg = [&](int ntile, int nkb, uint32_t b_hi_addr, uint32_t b_half, uint32_t b_kb_stride, uint32_t d_col, int N) {
-        const uint32_t idesc = idesc_f16(128, N);
-        // k-block outer, M tile inner: consecutive MMAs alternate between the two accumulator tiles
-        for (int kb = 0; kb < nkb; ++kb) {
-          const uint32_t sb = b_hi_addr + (uint32_t)kb * b_kb_stride;
-          const uint64_t b_hi = desc(sb), b_lo = desc(sb + b_half);
-          const uint32_t acc0 = kb > 0 ? 1u : 0u;
-          for (int m = 0; m < ntile; ++m) {
-            const uint32_t d_tmem = tmem_base + d_col + (uint32_t)(m * N);
-            wait_bar<PROF>(&ms->full[slot], ph, pc[1]);
-            fence_after_sync();
-            __syncwarp();
-            if (elect_one()) {
-              if (!(dbg & 2)) {  // (ablation: no tensor-core work)
-                switch (slot) {
-                  case 0: issue6(d_tmem, ad_hi[0], ad_lo[0], b_hi, b_lo, idesc, acc0); break;
-                  case 1: issue6(d_tmem, ad_hi[1], ad_lo[1], b_hi, b_lo, idesc, acc0); break;
-                  case 2: issue6(d_tmem, ad_hi[2], ad_lo[2], b_hi, b_lo, idesc, acc0); break;
-                  case 3: issue6(d_tmem, ad_hi[3], ad_lo[3], b_hi, b_lo, idesc, acc0); break;
-                  default: issue6(d_tmem, ad_hi[4], ad_lo[4], b_hi, b_lo, idesc, acc0); break;
-                }
-              }
-              mma_commit(&ms->empty[slot]);
-            }
-            if (++slot == kStages) {
-              slot = 0;
-              ph ^= 1u;
-            }
+        for (int q = 0; q < 3; ++q) {
+          if (j[q] >= total[q]) continue;
+          const uint32_t slot = (uint32_t)slot0[q] + j[q] % (uint32_t)nslots[q], ph = (j[q] / (uint32_t)nslots[q]) & 1u;
+          if (!rb::tma::mbar_try_wait(&ms->empty[slot], ph ^ 1u)) continue;
+          // pack stage of position j in this stream (pack order: env, a0, v0, a1, v1, a2, v2)
+          int stage;
+          if (q == 0) {
+            stage = sg.env + (int)(j[q] % n_env);
+          } else {
+            const int i = (int)(j[q] % n_tower), l0 = 2 * sg.nkb0;
+            const bool v = q == 2;
+            stage = i < l0 ? (v ? sg.v0 : sg.a0) + i : (i < l0 + 16 ? (v ? sg.v1 : sg.a1) + i - l0 : (v ? sg.v2 : sg.a2) + i - l0 - 16);
           }
-        }
-      };
-      const uint32_t ob_half = (uint32_t)sg.nkb0 * 4096u;
-      uint32_t p_obs = 0, p_vh = 0, p_oa = 0, p_ov = 0;
-      for (int t = 0; t <= T; ++t) {
-        const bool tail = (t == T);
-        if (t > 0) {
-          wait_bar<PROF>(&ms->obs_ready, p_obs, pc[2]);
-          p_obs ^= 1u;
-          fence_after_sync();
-        }
-        const int nv = (*reinterpret_cast<volatile int*>(&ms->nflag) > 0) ? 2 * kNE : kNE;
-        // segment order of the weight stream: ENV, A.L0, V.L0, A.L1, V.L1, A.L2, V.L2 (rolled: one copy of the issue code)
-#pragma unroll 1
-        for (int sgi = 0; sgi < 7; ++sgi) {
-          const bool is_v = sgi >= 2 && !(sgi & 1);
-          if (tail && !is_v) continue;
-          const int layer = sgi == 0 ? 0 : (sgi - 1) >> 1;
-          if (is_v) {
-            if (layer == 0) {
-              if (t > 0) {  // accumulator columns of the value tower are free once the previous value head has read them
-                wait_bar<PROF>(&ms->vhead, p_vh, pc[3]);
-                p_vh ^= 1u;
-              }
-            } else {
-              wait_bar<PROF>(&ms->opnd_v, p_ov, pc[5]);
-              p_ov ^= 1u;
-            }
-          } else if (layer > 0) {
-            wait_bar<PROF>(&ms->opnd_a, p_oa, pc[4]);
-            p_oa ^= 1u;
-          }
-          fence_after_sync();
-          seg(sgi == 0 ? 1 : 2, layer == 0 ? sg.nkb0 : 8, layer == 0 ? obuf_a : (is_v ? vbuf_a : abuf_a),
-              layer == 0 ? ob_half : (is_v ? (uint32_t)kVbufHalf : (uint32_t)kAbufHalf),
-              (layer == 0 || is_v) ? 4096u : 2048u, sgi == 0 ? kAccEnv : (is_v ? kAccV : kAccA), is_v ? nv : kNE);
-          __syncwarp();
-          if (elect_one()) mma_commit(sgi == 0 ? &ms->acc_env : (is_v ? &ms->acc_v : &ms->acc_a));
+          rb::tma::mbar_arrive_expect_tx(&ms->full[slot], kStageBytes);
+          bulk_load(ring + slot * kStageBytes, p.pack + (size_t)stage * kStageBytes, kStageBytes, &ms->full[slot]);
+          ++j[q];
         }
       }
     }
-  } else if (warp < 6) {
-    // ================= actor tower: epilogues, mean head, sampling =================
-    const int q = warp & 3, gt = tid - 64;
-    const uint32_t tq = tmem_base + ((uint32_t)(q * 32) << 16) + kAccA;
-    float bias[3][2];
-    {
-      const int64_t boff[3] = {p.L.bb0, p.L.bb1, p.L.bb2};
-      for (int l = 0; l < 3; ++l)
-        for (int m = 0; m < 2; ++m) bias[l][m] = P[boff[l] + m * 128 + q * 32 + lane];
-    }
+  } else if (warp >= 4 && warp < 8) {
+    // ================= actor tower: layers, mean head, sampling =================
+    const int w = warp & 3, gt = tid - 128;
+    const float* bias[3] = {P + p.L.bb0, P + p.L.bb1, P + p.L.bb2};
     float* h3 = reinterpret_cast<float*>(abuf);
-    uint32_t p_acc = 0;
+    uint32_t p_obs = 0;
     for (int t = 0; t < T; ++t) {
-#pragma unroll 1
-      for (int l = 0; l < 3; ++l) {
-        wait_bar<PROF>(&ms->acc_a, p_acc, pc[6]);
-        p_acc ^= 1u;
-        fence_after_sync();
-        const long long t_e0 = PROF ? clock64() : 0;
-        tower_epilogue(tq, kNE, abuf, kAbufHalf, 2048u, q, lane, bias[l][0], bias[l][1], l == 2, dbg & 8);
-        fence_before_sync();
-        if (l < 2) {
-          rb::tma::fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&ms->opnd_a);
-        } else {
-          named_sync(1, 128);
-        }
-        if constexpr (PROF) pc[13] += clock64() - t_e0;
+      if (t > 0) {
+        mbar_wait(&ms->obs_ready, p_obs);
+        p_obs ^= 1u;
       }
-      const long long t_h0 = PROF ? clock64() : 0;
+      const uint32_t base = (uint32_t)t * n_tower, l0 = 2u * (uint32_t)sg.nkb0;
+      tower_layer<kNE>(ms, ring_a, kActSlot0, base, sg.nkb0, obuf_a, ob_half, 4096u, bias[0], abuf, kAbufHalf, 2048u, 0, 1, w,
+                       lane);
+      tower_layer<kNE>(ms, ring_a, kActSlot0, base + l0, 8, abuf_a, kAbufHalf, 2048u, bias[1], abuf, kAbufHalf, 2048u, 0, 1,
+                       w, lane);
+      tower_layer<kNE>(ms, ring_a, kActSlot0, base + l0 + 16, 8, abuf_a, kAbufHalf, 2048u, bias[2], abuf, kAbufHalf, 2048u, 1,
+                       1, w, lane);
       // ---- mean head + Normal sample + log-prob: one (env, action) pair per thread.  Each thread does its own
       //      256-long dot product (float4 reads rotated by the lane so that a warp touches every bank once): no
       //      warp reductions, no shared-memory hand-off between head and sampling ----
@@ -687,48 +529,41 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
           ms->act[e * kMaxActTc + a] = xa;
         }
       }
-      if constexpr (PROF) pc[14] += clock64() - t_h0;
       // ---- env finish, shared with the env warps (barrier 4 = actor + env groups): #1 actions sampled / h3 dead,
       //      #2 zs + eps in the actor buffer, #3 next observation operand complete ----
       named_sync(4, 256);
       named_sync(4, 256);
-      env_finish4(*pa, ms, obuf, (uint32_t)sg.nkb0 * 4096u, reinterpret_cast<const float*>(abuf),
-                  reinterpret_cast<const float*>(abuf + kAbufHalf), warp - 2, lane, t, e0, nE, sg.nkb0, c_e, boot);
+      env_finish4(*pa, ms, obuf, ob_half, reinterpret_cast<const float*>(abuf), reinterpret_cast<const float*>(abuf + kAbufHalf),
+                  w, lane, t, e0, nE, sg.nkb0, c_e, boot);
       rb::tma::fence_proxy_async();
       named_sync(4, 256);
     }
-  } else if (warp < 10) {
-    // ================= value tower: epilogues, value head, truncation bootstrap =================
-    const int q = warp & 3, ew = warp - 6;
-    const uint32_t tq = tmem_base + ((uint32_t)(q * 32) << 16) + kAccV;
-    float bias[3][2];
-    {
-      const int64_t boff[3] = {p.L.vb0, p.L.vb1, p.L.vb2};
-      for (int l = 0; l < 3; ++l)
-        for (int m = 0; m < 2; ++m) bias[l][m] = P[boff[l] + m * 128 + q * 32 + lane];
-    }
+  } else if (warp >= 8) {
+    // ================= value tower: layers, value head, truncation bootstrap =================
+    const int w = warp & 3;
+    const float* bias[3] = {P + p.L.vb0, P + p.L.vb1, P + p.L.vb2};
     float* g3 = reinterpret_cast<float*>(vbuf);
-    uint32_t p_acc = 0;
-    int nv = kNE;
+    uint32_t p_obs = 0;
     for (int t = 0; t <= T; ++t) {
-#pragma unroll 1
-      for (int l = 0; l < 3; ++l) {
-        wait_bar<PROF>(&ms->acc_v, p_acc, pc[7]);
-        p_acc ^= 1u;
-        fence_after_sync();
-        if (l == 0) nv = (*reinterpret_cast<volatile int*>(&ms->nflag) > 0) ? 2 * kNE : kNE;
-        tower_epilogue(tq, nv, vbuf, kVbufHalf, 4096u, q, lane, bias[l][0], bias[l][1], l == 2, dbg & 8);
-        fence_before_sync();
-        if (l < 2) {
-          rb::tma::fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&ms->opnd_v);
-        } else {
-          named_sync(2, 128);
-        }
+      if (t > 0) {
+        mbar_wait(&ms->obs_ready, p_obs);
+        p_obs ^= 1u;
+      }
+      // the value tower runs with N = 64 columns when any environment was flagged for the truncation bootstrap
+      // (columns 32..63 = its pre-reset observation)
+      const int nv = (*reinterpret_cast<volatile int*>(&ms->nflag) > 0) ? 2 * kNE : kNE;
+      const uint32_t s0 = (uint32_t)t * n_tower, s1 = s0 + 2u * (uint32_t)sg.nkb0, s2 = s1 + 16u;
+      if (nv == kNE) {
+        tower_layer<kNE>(ms, ring_a, kValSlot0, s0, sg.nkb0, obuf_a, ob_half, 4096u, bias[0], vbuf, kVbufHalf, 4096u, 0, 2, w, lane);
+        tower_layer<kNE>(ms, ring_a, kValSlot0, s1, 8, vbuf_a, kVbufHalf, 4096u, bias[1], vbuf, kVbufHalf, 4096u, 0, 2, w, lane);
+        tower_layer<kNE>(ms, ring_a, kValSlot0, s2, 8, vbuf_a, kVbufHalf, 4096u, bias[2], vbuf, kVbufHalf, 4096u, 1, 2, w, lane);
+      } else {
+        tower_layer<2 * kNE>(ms, ring_a, kValSlot0, s0, sg.nkb0, obuf_a, ob_half, 4096u, bias[0], vbuf, kVbufHalf, 4096u, 0, 2, w, lane);
+        tower_layer<2 * kNE>(ms, ring_a, kValSlot0, s1, 8, vbuf_a, kVbufHalf, 4096u, bias[1], vbuf, kVbufHalf, 4096u, 0, 2, w, lane);
+        tower_layer<2 * kNE>(ms, ring_a, kValSlot0, s2, 8, vbuf_a, kVbufHalf, 4096u, bias[2], vbuf, kVbufHalf, 4096u, 1, 2, w, lane);
       }
       // ---- value head (columns 0..31: V(obs_t)) and bootstrap (columns 32..63: V(final_obs_{t-1}) where flagged) ----
-      for (int e = ew; e < nv; e += 4) {
+      for (int e = w; e < nv; e += 4) {
         if (e < kNE) {
           const float v = dot256(g3 + e * kH, ms->vw, lane);
           if (lane == 0 && e < nE) p.values[(size_t)t * B + e0 + e] = v;
@@ -747,18 +582,16 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
       if (lane == 0) mbar_arrive(&ms->vhead);
     }
   } else {
-    // ================= env warps: noise, dynamics finish, auto-reset, next observation operand =================
-    const int q = warp & 3, ew = warp - 10, gt = tid - 320;
-    const uint32_t tq = tmem_base + ((uint32_t)(q * 32) << 16) + kAccEnv;
+    // ================= env warps: noise, x.W_s, dynamics finish, auto-reset, next observation operand =================
+    const int ew = warp, gt = tid;
+    const int g = lane >> 2, tq = lane & 3;
     float* zs = reinterpret_cast<float*>(abuf);  // [32][obs] fp32, aliases the actor buffer (free between barrier #1 and the next L0)
     float* eps_s = reinterpret_cast<float*>(abuf + kAbufHalf);  // [32][obs] fp32 draws of this step
     const int nk = sg.nkb0;                       // observation columns per lane
-    const uint32_t ob_half = (uint32_t)sg.nkb0 * 4096u;
-    uint32_t p_env = 0, p_vh = 0;
+    uint32_t p_vh = 0;
     for (int t = 0; t < T; ++t) {
       // ---- 1. Philox draws of this step for my 8 environments (same streams / order as env_finish_kernel) ----
       float eps[8][4], eps_r[8], uu[8];
-      const long long t_n0 = PROF ? clock64() : 0;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         eps_r[i] = 0.f;
@@ -766,8 +599,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
 #pragma unroll
         for (int k = 0; k < 4; ++k) eps[i][k] = 0.f;
       }
-      if (dbg & 1) {  // ablation: no Philox draws
-      } else if (!p.env_noise) {
+      if (!p.env_noise) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int e = ew * 8 + i;
@@ -781,46 +613,42 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
           }
         }
       }
-      if constexpr (PROF) pc[11] += clock64() - t_n0;
-      // ---- 2. wait for the env accumulator and the value head, meet the actor group (#1: h3 dead, actions sampled),
-      //         then park x.W_s (TMEM -> fp32 [32][obs]) and this step's draws in the free actor buffer ----
-      wait_bar<PROF>(&ms->acc_env, p_env, pc[8]);
-      p_env ^= 1u;
-      wait_bar<PROF>(&ms->vhead, p_vh, pc[10]);  // the value head of this step has consumed flag / rew of the previous step
+      // ---- 2. x.W_s of this step (the observation operand is complete: barrier #3 of the previous step) ----
+      LayerAcc<kNE, 1> zacc;
+      layer_mma<kNE, 1>(zacc, ms, ring_a, kEnvSlot0, kEnvSlots, (uint32_t)t * n_env, sg.nkb0, obuf_a, ob_half, 4096u, lane);
+      // ---- 3. wait for the value head, meet the actor group (#1: h3 dead, actions sampled), then park x.W_s
+      //         (fp32 [32][obs]) and this step's draws in the free actor buffer ----
+      mbar_wait(&ms->vhead, p_vh);  // the value head of this step has consumed flag / rew of the previous step
       p_vh ^= 1u;
-      fence_after_sync();
-      const long long t_b0 = PROF ? clock64() : 0;
       named_sync(4, 256);
-      if constexpr (PROF) pc[9] += clock64() - t_b0;
-      const long long t_f0 = PROF ? clock64() : 0;
-      {
-        uint32_t r[32];
-        tmem_ld32(tq, r);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int e = ew * 8 + i;
+      for (int i = 0; i < 8; ++i) {
+        const int e = ew * 8 + i;
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (k < nk) eps_s[e * obs + lane + 32 * k] = eps[i][k];
-          if (lane == 0) {
-            ms->er[e] = eps_r[i];
-            ms->uu[e] = uu[i];
-          }
-        }
-        tmem_ld_wait();
-        const int c = q * 32 + lane;
-        if (c < obs) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) zs[e * obs + c] = __uint_as_float(r[e]) * out_scale;
+        for (int k = 0; k < 4; ++k)
+          if (k < nk) eps_s[e * obs + lane + 32 * k] = eps[i][k];
+        if (lane == 0) {
+          ms->er[e] = eps_r[i];
+          ms->uu[e] = uu[i];
         }
       }
-      fence_before_sync();
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int c = h * 64 + ew * 16 + g + 8 * r;  // observation column (row of the env product)
+          if (c < obs) {
+#pragma unroll
+            for (int cc = 0; cc < kNE / 8; ++cc)
+#pragma unroll
+              for (int u = 0; u < 2; ++u) zs[(8 * cc + 2 * tq + u) * obs + c] = zacc.d[0][h][4 * cc + 2 * r + u] * out_scale;
+          }
+        }
       named_sync(4, 256);
-      // ---- 3. finish 4 environments per warp (the actor group takes environments 0..15) ----
+      // ---- 4. finish 4 environments per warp (the actor group takes environments 0..15) ----
       env_finish4(*pa, ms, obuf, ob_half, zs, eps_s, 4 + ew, lane, t, e0, nE, nk, c_e, boot);
       rb::tma::fence_proxy_async();
       named_sync(4, 256);
-      if constexpr (PROF) pc[12] += clock64() - t_f0;
       if (gt == 0) {
         int n = 0;
         for (int e = 0; e < kNE; ++e) n += ms->flag[e];
@@ -830,20 +658,6 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
       }
     }
     if (gt < nE) p.elapsed[e0 + gt] = ms->el[gt];  // written by this group, ordered by the last named barrier
-  }
-
-  if constexpr (PROF) {
-    if (blockIdx.x == 0 && p.prof && lane == 0 && (warp == 0 || warp == 1 || warp == 2 || warp == 6 || warp == 10)) {
-      for (int i = 0; i < 15; ++i)
-        if (pc[i]) p.prof[i] = pc[i];
-      if (warp == 0) p.prof[15] = clock64() - t_start;
-    }
-  }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -901,18 +715,6 @@ __global__ void __launch_bounds__(256) pack_kernel(PackArgs a) {
 
 }  // namespace
 
-static int g_tc_dbg = 0;
-static long long* g_tc_prof = nullptr;
-
-// Probe hook (tools/rollout_tc_probe.py): ablation switches (1 = no Philox draws, 2 = no MMAs, 4 = no weight loads,
-// 8 = epilogues only read the accumulators) and a device buffer of 16 int64 receiving CTA 0's wait-cycle counters
-// (selects the instrumented instantiation).  flags = 0, prof = NULL restores the production kernel.
-extern "C" int rb200_rollout_tc_debug(int flags, void* prof16) {
-  g_tc_dbg = flags;
-  g_tc_prof = static_cast<long long*>(prof16);
-  return RB200_OK;
-}
-
 extern "C" int rb200_rollout_tc_supported(const rb200_mlp_layout* L, int B) {
   if (!L) return RB200_E_NULL;
   if (L->hidden != kH || L->act_dim <= 0 || L->act_dim > kMaxActTc || L->value_dim != 1) return RB200_E_UNSUPPORTED;
@@ -965,16 +767,13 @@ extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, 
   a.act = L->act_dim; a.max_episode_steps = max_episode_steps; a.auto_reset = auto_reset;
   a.bootstrap_on_done = bootstrap_on_done; a.gamma = (float)gamma; a.p_term = (float)p_term;
   a.noise_std = (float)noise_std; a.reward_noise_std = (float)reward_noise_std;
-  a.dbg = g_tc_dbg; a.prof = g_tc_prof;
   static bool attr_done = false;
   if (!attr_done) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    RB_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     attr_done = true;
   }
   const int grid = (B + kNE - 1) / kNE;
-  if (g_tc_prof) rollout_tc_kernel<true><<<grid, kThreads, kSmemBytes, rb::as_stream(stream)>>>(a);
-  else rollout_tc_kernel<false><<<grid, kThreads, kSmemBytes, rb::as_stream(stream)>>>(a);
+  rollout_tc_kernel<<<grid, kThreads, kSmemBytes, rb::as_stream(stream)>>>(a);
   rb::count_launch();
   RB_RETURN_LAUNCH();
 }

@@ -1,19 +1,10 @@
-// K3 tensor-core path, round 2: fp32-accurate GEMMs on tcgen05 `kind::f16` through a 2-way fp16 split.
+// fp32-accurate GEMMs of the MLP towers on Hopper wgmma (fp16 inputs, fp32 accumulators) through a 2-way fp16 split.
 //     a = a_hi + a_lo, b = b_hi + b_lo (fp16 numbers, 11 significant bits each; operands pre-scaled by a power of two so
 //     that both halves stay in fp16's normal range);  a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi   (dropped a_lo.b_lo ~ 2^-22)
-// Same three-MMA compensation as the round-1 3xTF32 kernels (tc_gemm.cu) with the same 2^-22 truncation, but
-//   * kind::f16 issues at twice the kind::tf32 rate, so an fp32-accurate product costs peak/3 instead of peak/6;
-//   * operands are 2 bytes in shared memory: the three MMAs re-read 72 KB per 128x256x32 k-block instead of 147 KB and
-//     the weight tiles TMA-fill 32 KB instead of 64 KB (round 1 was bound by exactly this shared-memory traffic);
-//   * the weights are packed per k-block as pre-swizzled fp16 (hi | lo) tiles - a K-major forward pack and an MN-major dgrad
-//     pack per matrix, written by one pack kernel - and fetched with ONE 32 KB bulk copy per k-block; the transposed fp32
-//     weight copies of round 1 and their 8 refresh kernels are gone;
-//   * one launch serves BOTH towers (policy backbone + value MLP have identical shapes): grouped tile scheduling halves
-//     the launches and fills the tail wave of small per-rank batches.
-// Activations / activation gradients stay plain fp32 in HBM (one copy); the streamed operand is TMA-landed as fp32
-// (SWIZZLE_128B) and split by transform warps into two fp16 SWIZZLE_64B tiles.  Gradients are tiny (1e-6 .. 1e-10):
-// their producer publishes max|x| and the consumer scales by 2^s (exact) so that the maximum sits at 2^13; the fp32
-// accumulator is scaled back in the epilogue (exact).
+// Weights come as pre-swizzled fp16 (hi | lo) packs per k-block; activations stay plain fp32 in HBM and are split in
+// registers; one launch serves both towers.
+// Gradients are tiny (1e-6 .. 1e-10): their producer publishes max|x| and the consumer scales by 2^s (exact) so that the
+// maximum sits at 2^13; the fp32 accumulator is scaled back in the epilogue (exact).
 // Reference op chains replaced: nn.Linear + tanh of MLPPolicy.backbone / ValueHead.mlp
 // (rlinf/models/embodiment/mlp_policy/mlp_policy.py:91-98, modules/value_head.py:37-45) and autograd's dgrad / wgrad.
 #include <cuda_fp16.h>
@@ -21,6 +12,7 @@
 #include "common.cuh"
 #include "tc_gemm.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace rb {
 namespace tch {
@@ -29,69 +21,20 @@ using rb::tc::BK;
 using rb::tc::BM;
 using rb::tc::BN;
 
-// Two rings (round 2, second half).  The first version kept the fp32 landing tile, its fp16 halves and the weight
-// tile in ONE 64 KB stage, 3 stages deep: a stage stayed busy for load latency (~3000 clk under HBM load) + transform
-// (~700) + MMA (768), i.e. ~1500 clk per k-block against 768 of MMA (tools/gemm_role_probe.py).  Now the fp32 landing
-// tiles have their own deep ring (freed as soon as the transform has read them: 6 x 16 KB of activations in flight per
-// SM) and the MMA operands (A hi | lo written by the transform, weight hi | lo landed by TMA) a shallow one.
-constexpr int kAStages = 4;         // fp32 landing ring of the streamed operand
-constexpr int kBStages = 2;         // fp16 A hi | lo slots (written by the transform)
-constexpr int kWStages = 3;         // weight tile ring (one 32 KB bulk copy each): with two slots the MMA waited ~650 clk
-                                    // per k-block for the weight tile (32 KB over L2 -> SM take ~2000 clk to arrive)
-constexpr int kA32 = BM * BK * 4;   // 16 KB fp32 landing tile of the streamed operand
-constexpr int kA16 = BM * BK * 2;   //  8 KB per fp16 half
-constexpr int kB16 = BN * BK * 2;   // 16 KB per fp16 half of the weight tile
-constexpr int kOpBytes = 2 * kA16;  // 16 KB: A hi | A lo
-constexpr int kWBytes = 2 * kB16;   // 32 KB: W hi | W lo
-constexpr int kRingBytes = kAStages * kA32 + kBStages * kOpBytes + kWStages * kWBytes;  // 64 + 32 + 96 = 192 KB
-constexpr int kXfWarpsDefault = 4;  // transform warps per CTA: template parameter XF of the forward / dgrad kernel (4 or 8)
-constexpr int kEpiWarps = 8;  // two per TMEM lane quarter, 128 of the 256 output columns each: the bias+tanh / (1-h^2)
-                              // epilogue of one warp per scheduler took 7.8 k cycles per tile against 6.1 k of MMA
-constexpr int threads_for(int xf) { return 32 * (2 + xf + kEpiWarps); }  // producer, MMA, transform, epilogue
-constexpr int kStagingBytes = kEpiWarps * 4096;  // one [32 x 32] fp32 staging tile per epilogue warp
-constexpr int kTmemCols = 512;
+// Forward / dgrad kernel (persistent, one CTA per SM): a producer warp fills a ring of stages (fp32 landing tile of the
+// streamed operand, [128 rows x 32 k] TMA SWIZZLE_128B, + the packed weight tile of the k-block, one 32 KB bulk copy);
+// warpgroups 0 / 1 own rows 0-63 / 64-127 of the 128 x 256 output tile, split their fp32 rows into fp16 hi / lo wgmma A
+// fragments in registers and keep the fp32 accumulator in registers through the epilogue.
+constexpr int kStages = 4;
+constexpr int kA32 = BM * BK * 4;              // 16 KB fp32 landing tile of the streamed operand
+constexpr int kB16 = BN * BK * 2;              // 16 KB per fp16 half of the weight tile
+constexpr int kWBytes = 2 * kB16;              // 32 KB: W hi | W lo
+constexpr int kStageBytes = kA32 + kWBytes;    // 48 KB
+constexpr int kRingBytes = kStages * kStageBytes;  // 192 KB
+constexpr int kThreads = 288;  // the block is resourced as three whole warpgroups: 168 registers per thread (a larger
+                               // register count fails to launch), so ptxas serialises the six wgmmas of a k-block
 constexpr int kWeightScaleLog2 = 10;  // weights are stored as fp16 (hi, lo) of w * 2^10 (|w| <~ 1: both halves normal)
 
-// ---- PTX wrappers (same instructions as tc_gemm.cu) ---------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tma::smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tma::smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-      ::"r"(d_tmem), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-      "%24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 // 1-D bulk copy global -> shared, completion counted on an mbarrier
 __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -99,30 +42,12 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(tma::smem_u32(bar))
                : "memory");
 }
+// barrier over the 256 consumer threads only (the producer warp runs ahead)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// ---- UMMA shared-memory descriptors (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp; canonical layouts in
-//      cute/atom/mma_traits_sm100.hpp:167-203).  start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) |
-//      layout_type [61,64): 2 = SWIZZLE_128B, 4 = SWIZZLE_64B ------------------------------------------------------------
-// K-major, SWIZZLE_64B: rows of 32 fp16 (64 B), 8-row groups 512 B apart (LBO unused for swizzled K-major).
-__device__ __forceinline__ uint64_t desc_k_sw64(uint32_t addr) {
-  return (uint64_t)((addr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
-// MN-major, SWIZZLE_128B: ((8,n),(8,k)) in 16-byte units = 64 fp16 along MN per row (128 B), 8 K-rows per atom (SBO = 1024 B
-// between atoms along K), MN groups of 64 elements LBO bytes apart.
-__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t addr, uint32_t lbo) {
-  return (uint64_t)((addr & 0x3ffffu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// MN-major, SWIZZLE_64B: ((4,n),(8,k)) = 32 fp16 along MN per row (64 B), 8 K-rows per atom (SBO = 512 B), MN groups LBO apart.
-__device__ __forceinline__ uint64_t desc_mn_sw64(uint32_t addr, uint32_t lbo) {
-  return (uint64_t)((addr & 0x3ffffu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) |
-         (4ull << 61);
-}
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 [4,6)=1, a/b format F16 = 0 [7,10),[10,13),
-// a_major bit 15, b_major bit 16 (0 = K, 1 = MN), N>>3 [17,23), M>>4 [24,29)
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+// Operand layouts: K-major SWIZZLE_64B (forward pack: 64-B rows, SBO 512), MN-major SWIZZLE_128B (dgrad pack: SBO 1024 B
+// between 8 K-rows, LBO 4096 B between 64-wide N groups), MN-major SWIZZLE_64B (wgrad H: SBO 512, LBO 2048).
+constexpr uint32_t kSw128 = 1, kSw64 = 2;
 
 __device__ __forceinline__ float tanh_fast(float x) {
   const float t = __expf(-2.0f * fabsf(x));
@@ -137,6 +62,15 @@ __device__ __forceinline__ int scale_log2_for(float amax) {
   if (!(amax > 0.0f) || e < -120) return 0;
   int s = 13 - e;
   return s > 100 ? 100 : (s < -100 ? -100 : s);
+}
+
+// (x0, x1) -> packed fp16 pairs hi = rn(x), lo = rn(x - hi)
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  const __half2 hh = __floats2half2_rn(x0, x1);
+  const float2 hf = __half22float2(hh);
+  const __half2 ll = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&hh);
+  lo = *reinterpret_cast<const uint32_t*>(&ll);
 }
 
 // fp32 [R rows x 32 floats] SWIZZLE_128B tile -> fp16 hi / lo [R rows x 32 halfs] SWIZZLE_64B tiles; item = (row, 8 floats)
@@ -167,30 +101,23 @@ __device__ __forceinline__ void split_tile(const uint8_t* __restrict__ src, uint
   }
 }
 
-// PROF instantiations (tools/gemm_role_probe.py): cycles each role of CTA 0 spends waiting / working
-template <bool PROF>
-__device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity, long long& acc) {
-  if constexpr (PROF) {
-    const long long t0 = clock64();
-    tma::mbar_wait(bar, parity);
-    acc += clock64() - t0;
-  } else {
-    tma::mbar_wait(bar, parity);
+// wgmma A fragment (m64k16, this thread's rows r0 / r0 + 8, k columns c0 + 2t + {0, 1, 8, 9}) of a row-major fp32
+// [rows x 32] SWIZZLE_128B landing tile, scaled and split into fp16 hi / lo
+__device__ __forceinline__ void a_frag_rows(const uint8_t* tile, int r0, int c0, float scale, uint32_t (&hi)[4],
+                                            uint32_t (&lo)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = r0 + (i & 1) * 8, c = c0 + (i >> 1) * 8;
+    const float2 x = *reinterpret_cast<const float2*>(tile + r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4);
+    split2(x.x * scale, x.y * scale, hi[i], lo[i]);
   }
 }
 
 struct __align__(16) Barriers {
-  uint64_t full_a[kAStages];   // fp32 landing tile arrived (TMA tx bytes)
-  uint64_t empty_a[kAStages];  // transform warps have read it
-  uint64_t xf[kBStages];       // transform warps have written A hi | lo
-  uint64_t empty_b[kBStages];  // MMAs reading the A slot have completed (tcgen05.commit)
-  uint64_t full_w[kWStages];   // weight tile arrived (bulk-copy tx bytes)
-  uint64_t empty_w[kWStages];  // MMAs reading the weight slot have completed (tcgen05.commit)
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad_[3];
-  alignas(16) float bias[BN];  // (read as float4) forward: the layer bias; dgrad: per-CTA column sums of the output (bias gradient of the producer)
+  uint64_t full[kStages];   // landing tile + weight tile arrived (tx bytes)
+  uint64_t empty[kStages];  // both consumer warpgroups' wgmmas reading the stage have completed (one arrival per warp)
+  alignas(16) float bias[BN];  // forward: the layer bias
+  float csum[8][BN];           // dgrad: column sums of the output per consumer warp (one writer per slot: deterministic)
 };
 
 struct Group {
@@ -199,35 +126,27 @@ struct Group {
   float* colsum;        // [256] += column sums of the output, or NULL
   const float* amax_in; // [1] max|A| published by A's producer (gradient GEMMs), or NULL = no scaling
   float* amax_out;      // [1] atomicMax of |output| for the next gradient GEMM, or NULL
+  float* c;             // [M,256] output
 };
 
 struct GemmParams {
-  CUtensorMap a[2], c[2];
+  CUtensorMap a[2];
   const uint8_t* wpack[2];  // packed weight tiles of each group (32 KB per k-block: hi | lo)
   Group g[2];
+  float* part;  // [gridDim.x][256] per-CTA column sums (summed in CTA order by sum_slots)
   int64_t M;
   int K;
   int epi;
-  int b_mn;  // 0: weights K-major (forward), 1: MN-major (dgrad: B(n = in, k = out) = W[out][in])
   int ngroups;
-  int flags;
-  long long* prof;  // [16] (PROF instantiation only)
 };
 
-template <bool PROF, int kXfWarps>
-__global__ void __launch_bounds__(threads_for(kXfWarps), 1) tc_h_gemm_kernel(const __grid_constant__ GemmParams P) {
-  constexpr int kThreads = threads_for(kXfWarps);
-  long long pc[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  const long long t_start = PROF ? clock64() : 0;
+template <int B_MN>
+__global__ void __launch_bounds__(kThreads, 1) tc_h_gemm_kernel(const __grid_constant__ GemmParams P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tma::smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* ring_a = smem;                       // kAStages x [128 rows x 32 fp32] SWIZZLE_128B
-  uint8_t* ring_w = smem + kAStages * kA32;                 // kWStages x (W hi | W lo), 1024-aligned (MN-major SWIZZLE_128B)
-  uint8_t* ring_b = ring_w + kWStages * kWBytes;            // kBStages x (A hi | A lo)
-  uint8_t* staging = smem + kRingBytes;
-  Barriers* bars = reinterpret_cast<Barriers*>(staging + kStagingBytes);
+  Barriers* bars = reinterpret_cast<Barriers*>(smem + kRingBytes);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int grp = blockIdx.x % P.ngroups;
   const int cta = blockIdx.x / P.ngroups, n_cta = gridDim.x / P.ngroups;
   const Group& G = P.g[grp];
@@ -235,278 +154,154 @@ __global__ void __launch_bounds__(threads_for(kXfWarps), 1) tc_h_gemm_kernel(con
   const int n_kb = P.K / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kAStages; ++s) {
-      tma::mbar_init(&bars->full_a[s], 1);
-      tma::mbar_init(&bars->empty_a[s], kXfWarps);
-    }
-    for (int s = 0; s < kBStages; ++s) {
-      tma::mbar_init(&bars->xf[s], kXfWarps);
-      tma::mbar_init(&bars->empty_b[s], 1);
-    }
-    for (int s = 0; s < kWStages; ++s) {
-      tma::mbar_init(&bars->full_w[s], 1);
-      tma::mbar_init(&bars->empty_w[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      tma::mbar_init(&bars->tmem_full[b], 1);
-      tma::mbar_init(&bars->tmem_empty[b], kEpiWarps);
+    for (int s = 0; s < kStages; ++s) {
+      tma::mbar_init(&bars->full[s], 1);
+      tma::mbar_init(&bars->empty[s], 8);
     }
     tma::fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(&bars->tmem_base, kTmemCols);
-    tmem_relinquish();
-  }
   for (int i = threadIdx.x; i < BN; i += kThreads) bars->bias[i] = (P.epi == rb::tc::EPI_BIAS_TANH) ? G.bias[i] : 0.f;
-  fence_before_sync();
+  for (int i = threadIdx.x; i < 8 * BN; i += kThreads) bars->csum[i / BN][i % BN] = 0.f;
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = bars->tmem_base;
-  // operand scaling: A by 2^sa (from the published amax), weights are stored * 2^kWeightScaleLog2
-  const int sa = G.amax_in ? scale_log2_for(__ldg(G.amax_in)) : 0;
-  const float a_scale = pow2i(sa);
-  const float out_scale = pow2i(-(sa + kWeightScaleLog2));
 
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (lane == 0) {
+  if (wg == 2) {
+    // ================= producer =================
+    if (threadIdx.x == 256) {
       tma::prefetch_desc(&P.a[grp]);
-      const int64_t my_tiles = n_tiles > cta ? (n_tiles - cta + n_cta - 1) / n_cta : 0;
-      const int64_t total = my_tiles * n_kb;
-      // two independent streams issued by one thread: poll both rings, load whichever has a free slot
-      int64_t ja = 0, jb = 0;
-      uint32_t sa = 0, pa = 0, sb = 0, pb = 0;
-      while (ja < total || jb < total) {
-        if (ja < total && tma::mbar_try_wait(&bars->empty_a[sa], pa ^ 1u)) {
-          const int kb = (int)(ja % n_kb);
-          const int m0 = (int)((cta + (ja / n_kb) * n_cta) * BM);
-          tma::mbar_arrive_expect_tx(&bars->full_a[sa], kA32);
-          tma::load_2d(ring_a + sa * kA32, &P.a[grp], kb * BK, m0, &bars->full_a[sa]);  // rows >= M are zero-filled
-          ++ja;
-          if (++sa == kAStages) { sa = 0; pa ^= 1u; }
+      uint32_t s = 0, ph = 0;
+      for (int64_t tile = cta; tile < n_tiles; tile += n_cta) {
+        for (int kb = 0; kb < n_kb; ++kb) {
+          tma::mbar_wait(&bars->empty[s], ph ^ 1u);
+          uint8_t* st = smem + s * kStageBytes;
+          tma::mbar_arrive_expect_tx(&bars->full[s], kStageBytes);
+          tma::load_2d(st, &P.a[grp], kb * BK, (int)(tile * BM), &bars->full[s]);  // rows >= M are zero-filled
+          bulk_load(st + kA32, P.wpack[grp] + (size_t)kb * kWBytes, kWBytes, &bars->full[s]);  // hi | lo
+          if (++s == kStages) { s = 0; ph ^= 1u; }
         }
-        if (jb < total && tma::mbar_try_wait(&bars->empty_w[sb], pb ^ 1u)) {
-          const int kb = (int)(jb % n_kb);
-          tma::mbar_arrive_expect_tx(&bars->full_w[sb], kWBytes);
-          bulk_load(ring_w + sb * kWBytes, P.wpack[grp] + (size_t)kb * kWBytes, kWBytes, &bars->full_w[sb]);  // hi | lo
-          ++jb;
-          if (++sb == kWStages) { sb = 0; pb ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = idesc_f16(BM, BN, 0, P.b_mn);
-      uint32_t it = 0, tcount = 0;
-      for (int64_t tile = cta; tile < n_tiles; tile += n_cta, ++tcount) {
-        const uint32_t buf = tcount & 1u;
-        const uint32_t bph = (tcount >> 1) & 1u;
-        wait_bar<PROF>(&bars->tmem_empty[buf], bph ^ 1u, pc[1]);
-        fence_after_sync();
-        const uint32_t d_tmem = tmem_base + buf * BN;
-        for (int kb = 0; kb < n_kb; ++kb, ++it) {
-          const int s = it % kBStages;
-          const uint32_t ph = (it / kBStages) & 1u;
-          const int sw = it % kWStages;
-          const uint32_t phw = (it / kWStages) & 1u;
-          wait_bar<PROF>(&bars->full_w[sw], phw, pc[2]);
-          wait_bar<PROF>(&bars->xf[s], ph, pc[3]);
-          fence_after_sync();
-          const uint32_t sa32 = tma::smem_u32(ring_b + s * kOpBytes);
-          const uint64_t a_hi = desc_k_sw64(sa32), a_lo = desc_k_sw64(sa32 + kA16);
-          const uint32_t sbase = tma::smem_u32(ring_w + sw * kWBytes);
-          const uint64_t b_hi = P.b_mn ? desc_mn_sw128(sbase, 4096) : desc_k_sw64(sbase);
-          const uint64_t b_lo = P.b_mn ? desc_mn_sw128(sbase + kB16, 4096) : desc_k_sw64(sbase + kB16);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t ka = (uint64_t)((k * 32) >> 4);                        // 16 fp16 = 32 B along a 64-B row
-            const uint64_t kbo = P.b_mn ? (uint64_t)((k * 2048) >> 4) : ka;       // MN-major: 16 K-rows of 128 B
-            const uint32_t acc = (kb > 0 || k > 0) ? 1u : 0u;
-            mma_f16(d_tmem, a_lo + ka, b_hi + kbo, idesc, acc);  // small terms first
-            mma_f16(d_tmem, a_hi + ka, b_lo + kbo, idesc, 1u);
-            mma_f16(d_tmem, a_hi + ka, b_hi + kbo, idesc, 1u);
-          }
-          mma_commit(&bars->empty_b[s]);
-          mma_commit(&bars->empty_w[sw]);
-        }
-        mma_commit(&bars->tmem_full[buf]);
-      }
-    }
-  } else if (warp < 2 + kXfWarps) {
-    // ================= transform warps: fp32 A tile -> (A_hi, A_lo) fp16 tiles =================
-    const int t = threadIdx.x - 64;
-    uint32_t sa = 0, pa = 0, sb = 0, pb = 0;
-    for (int64_t tile = cta; tile < n_tiles; tile += n_cta) {
-      for (int kb = 0; kb < n_kb; ++kb) {
-        wait_bar<PROF>(&bars->full_a[sa], pa, pc[4]);           // the fp32 tile has landed
-        wait_bar<PROF>(&bars->empty_b[sb], pb ^ 1u, pc[0]);     // the operand slot's previous MMAs are done
-        const long long t_w0 = PROF ? clock64() : 0;
-        uint8_t* dst = ring_b + sb * kOpBytes;
-        split_tile<32 * kXfWarps>(ring_a + sa * kA32, dst, dst + kA16, BM, t, a_scale);
-        tma::fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          tma::mbar_arrive(&bars->xf[sb]);
-          tma::mbar_arrive(&bars->empty_a[sa]);
-        }
-        if constexpr (PROF) pc[5] += clock64() - t_w0;
-        if (++sa == kAStages) { sa = 0; pa ^= 1u; }
-        if (++sb == kBStages) { sb = 0; pb ^= 1u; }
       }
     }
   } else {
-    // ================= epilogue warps =================
-    const int q = warp & 3;
-    const int ew = warp - (2 + kXfWarps);
-    const int c_lo = (ew >> 2) * (BN / 2);  // this warp's half of the output columns
-    float4 (*sh)[8] = reinterpret_cast<float4 (*)[8]>(staging + ew * 4096);
-    if (lane == 0) tma::prefetch_desc(&P.c[grp]);
-    const int rs = lane >> 3, c4 = lane & 7;
-    float4 hp[8];
-    auto load_h = [&](int64_t r0, int cc) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int64_t gr = r0 + i * 4 + rs;
-        hp[i] = gr < P.M ? __ldg(reinterpret_cast<const float4*>(G.h + gr * BN + cc) + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    };
-    if (P.epi == rb::tc::EPI_TANHGRAD && (int64_t)cta < n_tiles) load_h((int64_t)cta * BM + q * 32, c_lo);
+    // ================= consumers: 64 rows each =================
+    const int cw = wg;
+    const int g = lane >> 2, t = lane & 3;
+    const int r_lo = cw * 64 + (warp & 3) * 16 + g;  // this thread's tile rows r_lo and r_lo + 8
+    // operand scaling: A by 2^sa (from the published amax), weights are stored * 2^kWeightScaleLog2
+    const int sa = G.amax_in ? scale_log2_for(__ldg(G.amax_in)) : 0;
+    const float a_scale = pow2i(sa);
+    const float out_scale = pow2i(-(sa + kWeightScaleLog2));
     float vmax = 0.f;
-    uint32_t tcount = 0;
-    for (int64_t tile = cta; tile < n_tiles; tile += n_cta, ++tcount) {
-      const uint32_t buf = tcount & 1u;
-      const uint32_t bph = (tcount >> 1) & 1u;
-      wait_bar<PROF>(&bars->tmem_full[buf], bph, pc[6]);
-      const long long t_e0 = PROF ? clock64() : 0;
-      fence_after_sync();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN;
-      const int64_t row0 = tile * BM + q * 32;
-#pragma unroll 1
-      for (int c0 = c_lo; c0 < c_lo + BN / 2; c0 += 32) {
-        if (lane == 0) tma::store_wait_read();  // the previous tile store has finished reading the staging tile
-        __syncwarp();
-        uint32_t r[32];
-        tmem_ld32(taddr0 + c0, r);
-        if (P.epi == rb::tc::EPI_TANHGRAD) {
+    uint32_t s = 0, ph = 0;
+    for (int64_t tile = cta; tile < n_tiles; tile += n_cta) {
+      float acc[128];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = i * 4 + rs;
-            sh[rr][c4 ^ (rr & 7)] = hp[i];
-          }
-          __syncwarp();
-          if (c0 + 32 < c_lo + BN / 2) load_h(row0, c0 + 32);
-          else if (tile + n_cta < n_tiles) load_h((tile + n_cta) * BM + q * 32, c_lo);
-        }
-        tmem_ld_wait();
+      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < n_kb; ++kb) {
+        tma::mbar_wait(&bars->full[s], ph);
+        const uint8_t* st = smem + s * kStageBytes;
+        const uint32_t wbase = tma::smem_u32(st + kA32);
+        uint32_t ah[BK / 16][4], al[BK / 16][4];
 #pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          float4 v;
-          const float a0 = __uint_as_float(r[j4 * 4 + 0]) * out_scale, a1 = __uint_as_float(r[j4 * 4 + 1]) * out_scale;
-          const float a2 = __uint_as_float(r[j4 * 4 + 2]) * out_scale, a3 = __uint_as_float(r[j4 * 4 + 3]) * out_scale;
-          if (P.epi == rb::tc::EPI_STORE) {
-            v = make_float4(a0, a1, a2, a3);
-          } else if (P.epi == rb::tc::EPI_BIAS_TANH) {
-            const float4 b = *reinterpret_cast<const float4*>(&bars->bias[c0 + j4 * 4]);
-            v = make_float4(tanh_fast(a0 + b.x), tanh_fast(a1 + b.y), tanh_fast(a2 + b.z), tanh_fast(a3 + b.w));
-          } else {
-            const float4 h = sh[lane][j4 ^ (lane & 7)];
-            v = make_float4(a0 * (1.0f - h.x * h.x), a1 * (1.0f - h.y * h.y), a2 * (1.0f - h.z * h.z),
-                            a3 * (1.0f - h.w * h.w));
-            vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
-          }
-          sh[lane][j4 ^ (lane & 7)] = v;
+        for (int k = 0; k < BK / 16; ++k) a_frag_rows(st, r_lo, k * 16 + 2 * t, a_scale, ah[k], al[k]);
+        wg::fence();  // the A fragments were written by ordinary instructions
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          // forward: K-major SW64, the next 16 k are 32 B further along the 64-B rows; dgrad: MN-major SW128, 16 K-rows of 128 B
+          const uint64_t b_hi = B_MN ? wg::desc(wbase + k * 2048, 4096, 1024, kSw128) : wg::desc(wbase + k * 32, 16, 512, kSw64);
+          const uint64_t b_lo = B_MN ? wg::desc(wbase + kB16 + k * 2048, 4096, 1024, kSw128)
+                                     : wg::desc(wbase + kB16 + k * 32, 16, 512, kSw64);
+          wg::Mma<256, B_MN>::run(acc, al[k], b_hi, 1u);  // small terms first
+          wg::Mma<256, B_MN>::run(acc, ah[k], b_lo, 1u);
+          wg::Mma<256, B_MN>::run(acc, ah[k], b_hi, 1u);
         }
-        tma::fence_proxy_async();
+        wg::commit();
+        wg::wait<0>();
         __syncwarp();
-        if (lane == 0) {
-          tma::store_2d(&P.c[grp], &sh[0][0], c0, (int)row0);  // rows >= M are clipped
-          tma::store_commit();
-        }
-        if (G.colsum != nullptr && P.epi == rb::tc::EPI_TANHGRAD) {
-          const int ch = lane >> 2, el = lane & 3;
-          float cs = 0.f;
-#pragma unroll 8
-          for (int rr = 0; rr < 32; ++rr) cs += reinterpret_cast<const float*>(&sh[rr][ch ^ (rr & 7)])[el];
-          atomicAdd(&bars->bias[c0 + lane], cs);
-        }
+        if (lane == 0) tma::mbar_arrive(&bars->empty[s]);
+        if (++s == kStages) { s = 0; ph ^= 1u; }
       }
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tma::mbar_arrive(&bars->tmem_empty[buf]);
-      if constexpr (PROF) pc[7] += clock64() - t_e0;
+      // ---- epilogue straight from the accumulator registers: 8-byte stores, each quad of lanes writes 32 B of a row ----
+      const int64_t row0 = tile * BM + r_lo, row1 = row0 + 8;
+      const bool ok0 = row0 < P.M, ok1 = row1 < P.M;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + 2 * t;
+        float v0 = acc[4 * j] * out_scale, v1 = acc[4 * j + 1] * out_scale;
+        float v2 = acc[4 * j + 2] * out_scale, v3 = acc[4 * j + 3] * out_scale;
+        if (P.epi == rb::tc::EPI_BIAS_TANH) {
+          const float2 b = *reinterpret_cast<const float2*>(&bars->bias[col]);
+          v0 = tanh_fast(v0 + b.x); v1 = tanh_fast(v1 + b.y);
+          v2 = tanh_fast(v2 + b.x); v3 = tanh_fast(v3 + b.y);
+        } else if (P.epi == rb::tc::EPI_TANHGRAD) {
+          const float2 h0 = ok0 ? __ldg(reinterpret_cast<const float2*>(G.h + row0 * BN + col)) : make_float2(0.f, 0.f);
+          const float2 h1 = ok1 ? __ldg(reinterpret_cast<const float2*>(G.h + row1 * BN + col)) : make_float2(0.f, 0.f);
+          v0 = ok0 ? v0 * (1.0f - h0.x * h0.x) : 0.f; v1 = ok0 ? v1 * (1.0f - h0.y * h0.y) : 0.f;
+          v2 = ok1 ? v2 * (1.0f - h1.x * h1.x) : 0.f; v3 = ok1 ? v3 * (1.0f - h1.y * h1.y) : 0.f;
+          vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(v0), fabsf(v1)), fmaxf(fabsf(v2), fabsf(v3))));
+          if (G.colsum != nullptr) {
+            float c0 = v0 + v2, c1 = v1 + v3;
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+              c0 += __shfl_xor_sync(0xffffffffu, c0, o);
+              c1 += __shfl_xor_sync(0xffffffffu, c1, o);
+            }
+            if (g == 0) {
+              bars->csum[warp][col] += c0;
+              bars->csum[warp][col + 1] += c1;
+            }
+          }
+        }
+        if (ok0) *reinterpret_cast<float2*>(G.c + row0 * BN + col) = make_float2(v0, v1);
+        if (ok1) *reinterpret_cast<float2*>(G.c + row1 * BN + col) = make_float2(v2, v3);
+      }
     }
     if (G.amax_out != nullptr && P.epi == rb::tc::EPI_TANHGRAD) {
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
       if (lane == 0 && vmax > 0.f) atomicMax(reinterpret_cast<unsigned int*>(G.amax_out), __float_as_uint(vmax));
     }
-    if (lane == 0) tma::store_wait_all();
   }
-
-  if constexpr (PROF) {
-    if (blockIdx.x == 0 && P.prof && lane == 0 && (warp == 0 || warp == 1 || warp == 2 || warp == 2 + kXfWarps)) {
-      for (int i = 0; i < 8; ++i)
-        if (pc[i]) atomicAdd(reinterpret_cast<unsigned long long*>(P.prof + i), (unsigned long long)pc[i]);
-      if (warp == 0) atomicAdd(reinterpret_cast<unsigned long long*>(P.prof + 8), (unsigned long long)(clock64() - t_start));
-    }
-  }
-  fence_before_sync();
   __syncthreads();
-  if (G.colsum != nullptr && P.epi == rb::tc::EPI_TANHGRAD)
-    for (int i = threadIdx.x; i < BN; i += kThreads)
-      if (bars->bias[i] != 0.f) atomicAdd(G.colsum + i, bars->bias[i]);
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
+  if (P.part != nullptr)
+    for (int i = threadIdx.x; i < BN; i += kThreads) {
+      float s = 0.f;
+      for (int w = 0; w < 8; ++w) s += bars->csum[w][i];
+      P.part[(size_t)blockIdx.x * BN + i] = s;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Weight-gradient GEMM:  dW[256, IN] += sum_m dZ[m, :]^T . H[m, :]     (IN % 32 == 0, <= 256), both operands MN-major.
-// Per k-block of 32 samples: TMA lands fp32 boxes {32 floats, 32 samples} (SWIZZLE_128B), 8 transform warps split them
-// into fp16 SWIZZLE_64B groups [32 samples x 32 features] = the canonical MN-major SW64 layout with LBO = 2048 B between
-// 32-feature groups and SBO = 512 B between 8-sample atoms; one K=16 MMA step spans two atoms (1024 B).
-// Grid = ngroups x 2 output tiles (128 rows of dW) x sample chunks; fp32 atomics into dW.
+// Weight-gradient GEMM:  dW[256, IN] += sum_m dZ[m, :]^T . H[m, :]     (IN % 32 == 0, <= 256); the reduction index m
+// (sample) is the strided one for both operands.  Grid = ngroups x 2 output tiles (128 rows of dW) x sample chunks;
+// each CTA writes its chunk's partial to a slot, the slots are summed in chunk order.  dZ^T fragments go straight into
+// registers, H is split into fp16 MN-major tiles (two operand slots).
 // ---------------------------------------------------------------------------------------------------------------
-// Two rings, as in the forward kernel: fp32 landing tiles (dZ 16 KB + H 32 KB per k-block of 32 samples) three deep,
-// freed as soon as the transform has read them, and ONE fp16 operand slot (dZ hi | lo, H hi | lo: 48 KB) that transform
-// and MMA take turns on.  The first version kept both in one 96 KB stage, two deep: a stage was held for load latency +
-// transform + MMA and the period was (3000 + 500 + 768) / 2 clk per k-block.
 constexpr int kWgLand = 3;
-constexpr int kWgA32 = 128 * BK * 4, kWgA16 = 128 * BK * 2;  // 16 KB / 8 KB
-constexpr int kWgB32 = 256 * BK * 4, kWgB16 = 256 * BK * 2;  // 32 KB / 16 KB (sized for IN = 256)
-constexpr int kWgLandBytes = kWgA32 + kWgB32;                // 48 KB
-constexpr int kWgOpBytes = 2 * kWgA16 + 2 * kWgB16;          // 48 KB
-constexpr int kWgRingBytes = kWgLand * kWgLandBytes + kWgOpBytes;  // 192 KB
-constexpr int kWgXfWarps = 16;  // four per scheduler: the fp32 -> fp16 split of 48 KB per k-block took 1025 clk with 8 (tools/gemm_role_probe.py)
-constexpr int kWgThreads = 32 * (2 + 4 + kWgXfWarps);
+constexpr int kWgA32 = 128 * BK * 4;                          // 16 KB of dZ
+constexpr int kWgB32 = 256 * BK * 4, kWgB16 = 256 * BK * 2;   // 32 KB / 16 KB of H (sized for IN = 256)
+constexpr int kWgLandBytes = kWgA32 + kWgB32;                 // 48 KB
+constexpr int kWgOpBytes = 2 * kWgB16;                        // 32 KB: H hi | H lo
+constexpr int kWgRingBytes = kWgLand * kWgLandBytes + 2 * kWgOpBytes;  // 144 + 64 KB
 
 struct WgBarriers {
-  uint64_t full[kWgLand], empty[kWgLand];  // landing ring: TMA tx bytes / transform warps done reading
-  uint64_t xf, op_free;                    // operand slot: written by the transform / its MMAs have completed
-  uint64_t tmem_full;
-  uint32_t tmem_base, pad_;
+  uint64_t full[kWgLand], empty[kWgLand];  // landing ring: TMA tx bytes / consumers done reading (one arrival per warp)
 };
 
 struct WgradParams {
   CUtensorMap z[2], h[2];
   float* dW[2];
+  float* part;             // [chunk][group][256 x IN] per-CTA partials of dW (summed in chunk order by sum_slots)
   const float* amax_z[2];  // max|dZ| per group (or NULL)
   int64_t n;
-  int IN, kb_per_chunk, ngroups, flags;
-  long long* prof;  // [16] (PROF instantiation: slots 9..15)
+  int IN, kb_per_chunk, ngroups;
 };
 
-template <bool PROF>
-__global__ void __launch_bounds__(kWgThreads, 1) tc_h_wgrad_kernel(const __grid_constant__ WgradParams P) {
-  long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  const long long t_start = PROF ? clock64() : 0;
+template <int NW>  // wgmma N: 128 or 256 (columns >= IN are computed on padding and dropped)
+__global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_constant__ WgradParams P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tma::smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* op = smem + kWgLand * kWgLandBytes;  // dZ hi | dZ lo | H hi | H lo
+  uint8_t* op = smem + kWgLand * kWgLandBytes;  // 2 x (H hi | H lo)
   WgBarriers* bars = reinterpret_cast<WgBarriers*>(smem + kWgRingBytes);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int grp = blockIdx.x % P.ngroups;
   const int rest = blockIdx.x / P.ngroups;
   const int out_tile = rest & 1, chunk = rest >> 1;
@@ -516,41 +311,25 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_h_wgrad_kernel(const __grid_
   const int kb1 = (kb0 + P.kb_per_chunk < n_kb_total) ? kb0 + P.kb_per_chunk : n_kb_total;
   const int n_kb = kb1 - kb0;
   const uint32_t b32_bytes = (uint32_t)IN * BK * 4;
-  const uint32_t tmem_cols = IN <= 32 ? 32u : (IN <= 64 ? 64u : (IN <= 128 ? 128u : 256u));
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kWgLand; ++s) {
       tma::mbar_init(&bars->full[s], 1);
-      tma::mbar_init(&bars->empty[s], kWgXfWarps);
+      tma::mbar_init(&bars->empty[s], 8);
     }
-    tma::mbar_init(&bars->xf, kWgXfWarps);
-    tma::mbar_init(&bars->op_free, 1);
-    tma::mbar_init(&bars->tmem_full, 1);
     tma::fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(&bars->tmem_base, tmem_cols);
-    tmem_relinquish();
-  }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = bars->tmem_base;
-  const int sz = P.amax_z[grp] ? scale_log2_for(__ldg(P.amax_z[grp])) : 0;
-  const float z_scale = pow2i(sz), out_scale = pow2i(-sz);
+  if (n_kb <= 0) return;
 
-  if (n_kb > 0) {
-    if (warp == 0) {
-      // boxes {32 floats, 32 samples} with SWIZZLE_128B, one lane per box (a single plain [32 x 128|IN] box per operand
-      // was tried: 64 row requests instead of 384 per k-block, but the unswizzled landing tile costs more in the
-      // transform than the requests save: 191 vs 163 us, profiles/r02_tc_h_unit_timings.txt)
-      const int gB = IN / 32;
-      const int n_box = 4 + gB;
+  if (wg == 2) {
+    {  // producer warp
+      const int n_box = 4 + IN / 32;
       for (int it = 0; it < n_kb; ++it) {
         const int s = it % kWgLand;
         const uint32_t ph = (it / kWgLand) & 1u;
         if (lane == 0) {
-          wait_bar<PROF>(&bars->empty[s], ph ^ 1u, pc[0]);
+          tma::mbar_wait(&bars->empty[s], ph ^ 1u);
           tma::mbar_arrive_expect_tx(&bars->full[s], kWgA32 + b32_bytes);
         }
         __syncwarp();
@@ -561,86 +340,69 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_h_wgrad_kernel(const __grid_
           else tma::load_2d(st + kWgA32 + (lane - 4) * 4096, &P.h[grp], (lane - 4) * 32, m0, &bars->full[s]);
         }
       }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        const uint32_t idesc = idesc_f16(128, IN, 1, 1);
-        for (int it = 0; it < n_kb; ++it) {
-          wait_bar<PROF>(&bars->xf, (uint32_t)it & 1u, pc[1]);  // the operand slot holds k-block `it`
-          fence_after_sync();
-          const uint32_t sa = tma::smem_u32(op);
-          const uint32_t sb = sa + 2 * kWgA16;
-          const uint64_t a_hi = desc_mn_sw64(sa, 2048), a_lo = desc_mn_sw64(sa + kWgA16, 2048);
-          const uint64_t b_hi = desc_mn_sw64(sb, 2048), b_lo = desc_mn_sw64(sb + kWgB16, 2048);
+    }
+  } else {
+    const int cw = wg;
+    const int g = lane >> 2, t = lane & 3;
+    const int f_lo = cw * 64 + (warp & 3) * 16 + g;  // this thread's rows of the dW tile: f_lo and f_lo + 8
+    const int sz = P.amax_z[grp] ? scale_log2_for(__ldg(P.amax_z[grp])) : 0;
+    const float z_scale = pow2i(sz), out_scale = pow2i(-sz);
+    float acc[NW / 2];
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t koff = (uint64_t)((k * 1024) >> 4);  // next 16 samples = two 8-sample atoms
-            const uint32_t acc = (it > 0 || k > 0) ? 1u : 0u;
-            mma_f16(tmem_base, a_lo + koff, b_hi + koff, idesc, acc);
-            mma_f16(tmem_base, a_hi + koff, b_lo + koff, idesc, 1u);
-            mma_f16(tmem_base, a_hi + koff, b_hi + koff, idesc, 1u);
-          }
-          mma_commit(&bars->op_free);
-        }
-        mma_commit(&bars->tmem_full);
-      }
-    } else if (warp < 6) {
-      const int q = warp & 3;
-      tma::mbar_wait(&bars->tmem_full, 0);
-      fence_after_sync();
-      const int row = out_tile * 128 + q * 32 + lane;
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16);
-      float* dW = P.dW[grp];
-      for (int c0 = 0; c0 < IN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(taddr0 + c0, r);
-        tmem_ld_wait();
-        float* dst = dW + (size_t)row * IN + c0;
+    for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
+    for (int it = 0; it < n_kb; ++it) {
+      const int s = it % kWgLand;
+      const uint32_t ph = (it / kWgLand) & 1u;
+      tma::mbar_wait(&bars->full[s], ph);
+      const uint8_t* st = smem + s * kWgLandBytes;
+      uint8_t* hop = op + (it & 1) * kWgOpBytes;
+      // H groups of [32 samples x 32 floats] (4 KB) -> [32 samples x 32 halfs] (2 KB), contiguous on both sides.  The slot
+      // was last read by the wgmmas of k-block it - 2, which every consumer thread waited for before the barrier of it - 1.
+      split_tile<256>(st + kWgA32, hop, hop + kWgB16, (IN / 32) * 32, threadIdx.x, 1.0f);
+      tma::fence_proxy_async();
+      consumer_sync();
+      const uint32_t hb = tma::smem_u32(hop);
+      // dZ^T fragments: A(m = feature f, k = sample) = dZ box f / 32 at (sample, f % 32)
+      uint32_t ah[BK / 16][4], al[BK / 16][4];
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          atomicAdd(reinterpret_cast<float4*>(dst + j),
-                    make_float4(__uint_as_float(r[j]) * out_scale, __uint_as_float(r[j + 1]) * out_scale,
-                                __uint_as_float(r[j + 2]) * out_scale, __uint_as_float(r[j + 3]) * out_scale));
-      }
-      fence_before_sync();
-    } else {
-      const int t = threadIdx.x - 6 * 32;
-      for (int it = 0; it < n_kb; ++it) {
-        const int s = it % kWgLand;
-        const uint32_t ph = (it / kWgLand) & 1u;
-        wait_bar<PROF>(&bars->full[s], ph, pc[2]);                       // the fp32 tiles have landed
-        wait_bar<PROF>(&bars->op_free, ((uint32_t)it & 1u) ^ 1u, pc[3]);  // the MMAs of k-block it-1 have read the operand slot
-        const long long t_w0 = PROF ? clock64() : 0;
-        uint8_t* st = smem + s * kWgLandBytes;
-        uint8_t* b32 = st + kWgA32;
-        // groups of [32 samples x 32 floats] (4 KB) -> [32 samples x 32 halfs] (2 KB); consecutive groups are contiguous
-        // on both sides, so "rows" simply runs over groups * 32
-        split_tile<32 * kWgXfWarps>(st, op, op + kWgA16, 4 * 32, t, z_scale);
-        split_tile<32 * kWgXfWarps>(b32, op + 2 * kWgA16, op + 2 * kWgA16 + kWgB16, (IN / 32) * 32, t, 1.0f);
-        tma::fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          tma::mbar_arrive(&bars->xf);
-          tma::mbar_arrive(&bars->empty[s]);
+      for (int k = 0; k < BK / 16; ++k) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int f = f_lo + (i & 1) * 8, m = k * 16 + 2 * t + (i >> 1) * 8;
+          const uint8_t* box = st + (f >> 5) * 4096;
+          const int fc = f & 31;
+          const float x0 = *reinterpret_cast<const float*>(box + m * 128 + (((fc >> 2) ^ (m & 7)) << 4) + (fc & 3) * 4);
+          const float x1 =
+              *reinterpret_cast<const float*>(box + (m + 1) * 128 + (((fc >> 2) ^ ((m + 1) & 7)) << 4) + (fc & 3) * 4);
+          split2(x0 * z_scale, x1 * z_scale, ah[k][i], al[k][i]);
         }
-        if constexpr (PROF) pc[4] += clock64() - t_w0;
+      }
+      wg::fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t b_hi = wg::desc(hb + k * 1024, 2048, 512, kSw64);  // next 16 samples = two 8-sample atoms
+        const uint64_t b_lo = wg::desc(hb + kWgB16 + k * 1024, 2048, 512, kSw64);
+        wg::Mma<NW, 1>::run(acc, al[k], b_hi, 1u);
+        wg::Mma<NW, 1>::run(acc, ah[k], b_lo, 1u);
+        wg::Mma<NW, 1>::run(acc, ah[k], b_hi, 1u);
+      }
+      wg::commit();
+      wg::wait<0>();
+      __syncwarp();
+      if (lane == 0) tma::mbar_arrive(&bars->empty[s]);
+    }
+    float* slot = P.part + (size_t)(chunk * P.ngroups + grp) * 256 * IN;
+    const int row0 = out_tile * 128 + f_lo;
+#pragma unroll
+    for (int j = 0; j < NW / 8; ++j) {
+      const int col = 8 * j + 2 * t;
+      if (col < IN) {
+        *reinterpret_cast<float2*>(slot + (size_t)row0 * IN + col) =
+            make_float2(acc[4 * j] * out_scale, acc[4 * j + 1] * out_scale);
+        *reinterpret_cast<float2*>(slot + (size_t)(row0 + 8) * IN + col) =
+            make_float2(acc[4 * j + 2] * out_scale, acc[4 * j + 3] * out_scale);
       }
     }
-  }
-  if constexpr (PROF) {
-    if (blockIdx.x == 0 && P.prof && lane == 0 && (warp == 0 || warp == 1 || warp == 6)) {
-      for (int i = 0; i < 5; ++i)
-        if (pc[i]) atomicAdd(reinterpret_cast<unsigned long long*>(P.prof + 9 + i), (unsigned long long)pc[i]);
-      if (warp == 0) {
-        atomicAdd(reinterpret_cast<unsigned long long*>(P.prof + 14), (unsigned long long)(clock64() - t_start));
-        atomicAdd(reinterpret_cast<unsigned long long*>(P.prof + 15), (unsigned long long)n_kb);
-      }
-    }
-  }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, tmem_cols);
   }
 }
 
@@ -696,65 +458,57 @@ __global__ void __launch_bounds__(256) split_half_kernel(SplitJobs jobs) {
 
 // ---- host -----------------------------------------------------------------------------------------------------------
 int encode_f32_sw128(CUtensorMap* out, const float* base, uint64_t rows, uint64_t cols, uint32_t box_rows);
-int encode_f16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint32_t box_cols, uint32_t box_rows,
-               int swizzle_bytes);
-
-static long long* g_prof = nullptr;  // rb200_tc_h_debug
 
 int launch(const GemmLaunch* L, int ngroups, int64_t M, int K, int epi, int b_mn, cudaStream_t st) {
   if (ngroups < 1 || ngroups > 2 || K % BK != 0 || K <= 0 || M <= 0) return RB200_E_SHAPE;
-  // Two towers in one launch: measured on B200 (profiles/r02_tc_h_gemm_grouping.txt) grouped is never slower than one
-  // launch per tower (1.18 vs 1.21 ms per 6-GEMM forward at 262144 rows, 0.21 vs 0.24 ms at 32768 where it fills the
-  // tail wave).  Debug flag 32 forces one launch per tower.
-  if (ngroups == 2 && (rb::tc::g_debug_flags & 32)) {
-    int e = launch(L, 1, M, K, epi, b_mn, st);
-    return e ? e : launch(L + 1, 1, M, K, epi, b_mn, st);
-  }
   GemmParams P{};
-  P.M = M; P.K = K; P.epi = epi; P.b_mn = b_mn; P.ngroups = ngroups; P.flags = rb::tc::g_debug_flags;
+  P.M = M; P.K = K; P.epi = epi; P.ngroups = ngroups;
   for (int g = 0; g < ngroups; ++g) {
     const GemmLaunch& l = L[g];
     const uintptr_t al = reinterpret_cast<uintptr_t>(l.a) | reinterpret_cast<uintptr_t>(l.b_hi) |
                          reinterpret_cast<uintptr_t>(l.c) | reinterpret_cast<uintptr_t>(l.h);
     if (al & 15) return RB200_E_ALIGN;
-    int e = encode_f32_sw128(&P.a[g], l.a, (uint64_t)M, (uint64_t)K, BM);
+    if (encode_f32_sw128(&P.a[g], l.a, (uint64_t)M, (uint64_t)K, BM)) return RB200_E_UNSUPPORTED;
     P.wpack[g] = reinterpret_cast<const uint8_t*>(l.b_hi);
-    if (!e) e = encode_f32_sw128(&P.c[g], l.c, (uint64_t)M, BN, 32);
-    if (e) return RB200_E_UNSUPPORTED;
-    P.g[g] = Group{l.bias, l.h, l.colsum, l.amax_in, l.amax_out};
+    P.g[g] = Group{l.bias, l.h, l.colsum, l.amax_in, l.amax_out, l.c};
   }
   static bool attr_done = false;
-  constexpr int kSmem = kRingBytes + kStagingBytes + 1024 + (int)sizeof(Barriers);
+  constexpr int kSmem = kRingBytes + 1024 + (int)sizeof(Barriers);
   static_assert(kSmem <= 232448, "tc_h_gemm_kernel shared memory");
   if (!attr_done) {
-    cudaError_t ce = cudaFuncSetAttribute(tc_h_gemm_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (ce == cudaSuccess)
-      ce = cudaFuncSetAttribute(tc_h_gemm_kernel<false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (ce == cudaSuccess)
-      ce = cudaFuncSetAttribute(tc_h_gemm_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    cudaError_t ce = cudaFuncSetAttribute(tc_h_gemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    if (ce == cudaSuccess) ce = cudaFuncSetAttribute(tc_h_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (ce != cudaSuccess) return (int)ce;
     attr_done = true;
   }
-  P.prof = g_prof;
+  // one launch serves both towers (grouped tile scheduling): it fills the tail wave of small per-rank batches
   const int64_t n_tiles = (M + BM - 1) / BM;
-  const int sms = rb::sm_count();
-  int per_group = sms / ngroups;
+  int per_group = rb::sm_count() / ngroups;
   if (per_group > n_tiles) per_group = (int)n_tiles;
   if (per_group < 1) per_group = 1;
-  // transform warps: 4 (one per scheduler) or 8 (debug flag 64) - see DESIGN.md section 4
-  const bool xf8 = ((rb::tc::g_debug_flags & 64) != 0) != (kXfWarpsDefault == 8);
-  if (g_prof) tc_h_gemm_kernel<true, 4><<<per_group * ngroups, threads_for(4), kSmem, st>>>(P);
-  else if (xf8) tc_h_gemm_kernel<false, 8><<<per_group * ngroups, threads_for(8), kSmem, st>>>(P);
-  else tc_h_gemm_kernel<false, 4><<<per_group * ngroups, threads_for(4), kSmem, st>>>(P);
+  rb::tch::SlotSums ss{};
+  ss.nslab = per_group;
+  ss.stride = (int64_t)ngroups * BN;
+  if (epi == rb::tc::EPI_TANHGRAD)
+    for (int g = 0; g < ngroups; ++g)
+      if (L[g].colsum) {
+        if (!P.part && !(P.part = rb::partials_scratch((int64_t)per_group * ngroups * BN))) return RB200_E_UNSUPPORTED;
+        ss.part[ss.count] = P.part + g * BN;
+        ss.out[ss.count] = L[g].colsum;
+        ss.len[ss.count++] = BN;
+      }
+  if (b_mn) tc_h_gemm_kernel<1><<<per_group * ngroups, kThreads, kSmem, st>>>(P);
+  else tc_h_gemm_kernel<0><<<per_group * ngroups, kThreads, kSmem, st>>>(P);
   rb::count_launch();
   cudaError_t ce = cudaPeekAtLastError();
-  return ce == cudaSuccess ? 0 : (int)ce;
+  if (ce != cudaSuccess) return (int)ce;
+  return ss.count ? rb::tch::sum_slots(ss, st) : 0;
 }
 
 int wgrad(const WgradLaunch* L, int ngroups, int64_t n, int IN, cudaStream_t st) {
   if (ngroups < 1 || ngroups > 2 || n <= 0 || IN <= 0 || IN > 256 || IN % 32 != 0) return RB200_E_SHAPE;
   WgradParams P{};
-  P.n = n; P.IN = IN; P.ngroups = ngroups; P.flags = rb::tc::g_debug_flags;
+  P.n = n; P.IN = IN; P.ngroups = ngroups;
   for (int g = 0; g < ngroups; ++g) {
     const uintptr_t al = reinterpret_cast<uintptr_t>(L[g].z) | reinterpret_cast<uintptr_t>(L[g].h) |
                          reinterpret_cast<uintptr_t>(L[g].dW);
@@ -769,9 +523,8 @@ int wgrad(const WgradLaunch* L, int ngroups, int64_t n, int IN, cudaStream_t st)
   constexpr int kSmem = kWgRingBytes + 1024 + (int)sizeof(WgBarriers);
   static_assert(kSmem <= 232448, "tc_h_wgrad_kernel shared memory");
   if (!attr_done) {
-    cudaError_t ce = cudaFuncSetAttribute(tc_h_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (ce == cudaSuccess)
-      ce = cudaFuncSetAttribute(tc_h_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    cudaError_t ce = cudaFuncSetAttribute(tc_h_wgrad_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    if (ce == cudaSuccess) ce = cudaFuncSetAttribute(tc_h_wgrad_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (ce != cudaSuccess) return (int)ce;
     attr_done = true;
   }
@@ -780,9 +533,43 @@ int wgrad(const WgradLaunch* L, int ngroups, int64_t n, int IN, cudaStream_t st)
   if (chunks < 1) chunks = 1;
   if (chunks > n_kb) chunks = n_kb;
   P.kb_per_chunk = (n_kb + chunks - 1) / chunks;
-  P.prof = g_prof;
-  if (g_prof) tc_h_wgrad_kernel<true><<<ngroups * 2 * chunks, kWgThreads, kSmem, st>>>(P);
-  else tc_h_wgrad_kernel<false><<<ngroups * 2 * chunks, kWgThreads, kSmem, st>>>(P);
+  chunks = (n_kb + P.kb_per_chunk - 1) / P.kb_per_chunk;  // every chunk non-empty: each writes its slot
+  const int64_t slab = 256 * (int64_t)IN;
+  if (!(P.part = rb::partials_scratch(chunks * ngroups * slab))) return RB200_E_UNSUPPORTED;
+  const dim3 grid(ngroups * 2 * chunks);
+  if (IN <= 128) tc_h_wgrad_kernel<128><<<grid, kThreads, kSmem, st>>>(P);
+  else tc_h_wgrad_kernel<256><<<grid, kThreads, kSmem, st>>>(P);
+  rb::count_launch();
+  cudaError_t ce = cudaPeekAtLastError();
+  if (ce != cudaSuccess) return (int)ce;
+  rb::tch::SlotSums ss{};
+  ss.count = ngroups;
+  ss.nslab = chunks;
+  ss.stride = ngroups * slab;
+  for (int g = 0; g < ngroups; ++g) {
+    ss.part[g] = P.part + g * slab;
+    ss.out[g] = L[g].dW;
+    ss.len[g] = (int)slab;
+  }
+  return rb::tch::sum_slots(ss, st);
+}
+
+__global__ void __launch_bounds__(256) sum_slots_kernel(const SlotSums s) {
+  const int q = blockIdx.y;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < s.len[q]; i += gridDim.x * blockDim.x) {
+    float acc = 0.f;
+    for (int k = 0; k < s.nslab; ++k) acc += s.part[q][k * s.stride + i];
+    s.out[q][i] += acc;
+  }
+}
+
+int sum_slots(const SlotSums& s, cudaStream_t st) {
+  if (s.count < 1 || s.count > 8 || s.nslab < 1) return RB200_E_SHAPE;
+  int len = 0;
+  for (int q = 0; q < s.count; ++q) len = s.len[q] > len ? s.len[q] : len;
+  int blocks = (len + 255) / 256;
+  if (blocks > 4 * rb::sm_count()) blocks = 4 * rb::sm_count();
+  sum_slots_kernel<<<dim3(blocks, s.count), 256, 0, st>>>(s);
   rb::count_launch();
   cudaError_t ce = cudaPeekAtLastError();
   return ce == cudaSuccess ? 0 : (int)ce;
@@ -809,13 +596,16 @@ int split_weights(const SplitSpec* specs, int count, cudaStream_t st) {
 }
 
 }  // namespace tch
+
+namespace tc {
+int g_debug_flags = 0;
+
+}  // namespace tc
 }  // namespace rb
 
-// probe hook (tools/gemm_role_probe.py): 16 int64 receiving CTA 0's per-role wait / work cycles (forward / dgrad kernel:
-// 0 producer-wait-empty, 1 mma-wait-tmem_empty, 2 mma-wait-full, 3 mma-wait-xf, 4 xf-wait-full, 5 xf-work,
-// 6 epilogue-wait-tmem_full, 7 epilogue-work, 8 total); NULL restores the production kernels
-extern "C" int rb200_tc_h_debug(void* prof16) {
-  rb::tch::g_prof = static_cast<long long*>(prof16);
+// Experiment switches of the kernels (see tc_gemm.cuh); not part of the product surface.
+extern "C" int rb200_debug_set_flags(int flags) {
+  rb::tc::g_debug_flags = flags;
   return RB200_OK;
 }
 

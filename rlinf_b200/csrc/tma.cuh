@@ -1,4 +1,4 @@
-// Minimal TMA / mbarrier wrappers (inline PTX, sm_90+ syntax; compiled for sm_100a only).
+// Minimal TMA / mbarrier wrappers (inline PTX, compiled for sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -166,6 +166,7 @@ class RolloutBuffer:
 class RolloutWorker:
     """One rank's env + policy replica."""
 
+    # thresholds of rollout.fused_kernel: auto, carried over from an earlier GPU; not re-measured on the H100
     FUSED_AUTO_MAX_ENVS_PER_CTA = 16
     TC_AUTO_MIN_ENVS = 640
 
@@ -182,7 +183,7 @@ class RolloutWorker:
         self._calls = 0
         self.graph_kernel_count = 0  # kernels replayed per rollout once the CUDA graph exists
         # V(final_obs) of step t (bootstrap of truncated episodes) only feeds rewards[t]: it runs on a side stream,
-        # concurrently with the policy inference of step t+1 (both are 32-CTA GEMM chains on a 148-SM device)
+        # concurrently with the policy inference of step t+1 (both are 32-CTA GEMM chains on a 132-SM device)
         self._side = torch.cuda.Stream(device=policy.device) if policy.device.type == "cuda" else None
         # persistent fused kernel: needs the synthetic env's dynamics (w_s, w_a) and a supported MLP shape
         # "auto" | "tc" (tensor-core persistent kernel) | True / "simt" (fp32 SIMT persistent kernel) | False (per-kernel graph)
@@ -200,20 +201,12 @@ class RolloutWorker:
         if mode == "tc" and not tc_ok:
             raise ValueError("rollout.fused_kernel='tc' needs hidden 256, a value head, act_dim <= 8, obs_dim % 32 == 0 "
                              "and obs_dim <= 128 (rb200_rollout_tc_supported)")
-        # tensor-core persistent kernel (csrc/rollout_tc.cu): one launch per rollout, ~44 us per env step whatever B is
-        # (32 envs per CTA, measured 22.7 ms per 512-step rollout at B = 512 .. 4096).  The fp32 SIMT persistent kernel is
-        # faster while a CTA owns <= 4 environments (19 ms at B = 512), so "auto" picks the tensor-core kernel from
-        # TC_AUTO_MIN_ENVS environments per rank on.
         self._tc = tc_ok and (mode == "tc" or (mode == "auto" and int(buffer.B) >= self.TC_AUTO_MIN_ENVS))
         if mode == "simt":
             mode = True
         if self._tc:
             mode = False
         if mode == "auto":
-            # measured (round 1, T = 512, ms per rollout fused / per-kernel graph): B = 512: 23 / 53, 1024: 33 / 55,
-            # 2048: 46 / 55, 4096: 71 / 54 (88 before the register-tiled layer) - the fused kernel wins while a CTA owns <= 16 environments (small per-rank
-            # batches, where the per-kernel loop is launch-latency bound); at E = 28 its fp32 SIMT layers (weight-load latency with only
-            # 8 warps / SM) still lose to the tensor-core GEMM chain
             sms = torch.cuda.get_device_properties(policy.device).multi_processor_count
             mode = -(-int(buffer.B) // sms) <= self.FUSED_AUTO_MAX_ENVS_PER_CTA
         self._fused = bool(mode) and supported
@@ -238,7 +231,7 @@ class RolloutWorker:
         L.check(lib.rb200_counter_add(L.ptr(env.counter), buf.T, st), "counter_add")
 
     def _tc_rollout(self, policy_noise=None, env_noise=None):
-        """The whole T-step loop in one persistent tcgen05 kernel (csrc/rollout_tc.cu)."""
+        """The whole T-step loop in one persistent tensor-core kernel (csrc/rollout_tc.cu)."""
         lib = L.load()
         buf, pol, env = self.buf, self.policy, self.env
         st = L.stream_ptr()

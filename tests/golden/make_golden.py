@@ -216,7 +216,15 @@ def gen_indexing(ref, out):
     out["idx_big_checksum"] = np.array([int((big * torch.arange(big.numel())).sum() % (2**61 - 1))], dtype=np.int64)
 
 
+def policy_grads(params):
+    """Seeded gradients the fixture's three optimiser steps consume (the tests regenerate them)."""
+    g = torch.Generator().manual_seed(4)
+    return {n: 1e-2 * torch.randn(p.shape, generator=g) for n, p in params.items()}
+
+
 def gen_policy(ref, out):
+    from make_golden_r5 import snapshot
+
     torch.manual_seed(42)
     pol = ref.mlp_policy.MLPPolicy(obs_dim=12, action_dim=3, num_action_chunks=1, add_value_head=True, add_q_head=False)
     with torch.no_grad():  # make biases / logstd non-trivial
@@ -226,8 +234,9 @@ def gen_policy(ref, out):
         pol.actor_logstd.add_(0.1 * torch.randn_like(pol.actor_logstd))
     names = [n for n, _ in pol.named_parameters()]
     out["pol_names"] = np.array(names)
-    for n, p in pol.named_parameters():
-        out["pol_p_" + n] = _np(p)
+    p0 = {n: p.detach().clone() for n, p in pol.named_parameters()}
+    for n, p in p0.items():  # initial parameters: value head / policy halves in two files (each < 1 MB)
+        out[("pinit_v:" if n.startswith("value_head") else "pinit:") + "pol_p_" + n] = _np(p)
     g = torch.Generator().manual_seed(3)
     states = torch.randn(37, 12, generator=g)
     action = torch.randn(37, 3, generator=g)
@@ -242,7 +251,8 @@ def gen_policy(ref, out):
     s.backward()
     out["pol_wl"], out["pol_wv"], out["pol_we"] = _np(wl), _np(wv), _np(we)
     for n, p in pol.named_parameters():
-        out["pol_g_" + n] = _np(p.grad)
+        out.update({"pol_g_" + n + k: v for k, v in snapshot(p.grad).items()})
+        p.grad = policy_grads(p0)[n]
     # 3 AdamW steps with the reference's grouping / clipping semantics (no_shard path)
     actor = [p for n, p in pol.named_parameters() if "value_head" not in n]
     critic = [p for n, p in pol.named_parameters() if "value_head" in n]
@@ -256,7 +266,7 @@ def gen_policy(ref, out):
         # keep the same grads (deterministic known-answer)
     out["pol_gradnorms"] = np.array(norms)
     for n, p in pol.named_parameters():
-        out["pol_p3_" + n] = _np(p)
+        out.update({"pol_p3_" + n + k: v for k, v in snapshot(p).items()})
 
 
 def gen_next(ref, out):
@@ -389,9 +399,12 @@ def main():
                      (gen_filter_and_metrics, "filter"), (gen_next, "next")):
         out = {}
         fn(ref, out)
-        path = os.path.join(HERE, f"golden_{name}.npz")
-        np.savez_compressed(path, **out)
-        print(name, len(out), "arrays ->", path, os.path.getsize(path), "bytes")
+        for part in ("pinit_v", "pinit", ""):  # "<file suffix>:" key prefixes route arrays to golden_<name>_<suffix>.npz
+            sel = {k.split(":", 1)[-1]: out.pop(k) for k in list(out) if not part or k.startswith(part + ":")}
+            if sel:
+                path = os.path.join(HERE, f"golden_{name}{'_' + part if part else ''}.npz")
+                np.savez_compressed(path, **sel)
+                print(name, part, len(sel), "arrays ->", path, os.path.getsize(path), "bytes")
 
 
 if __name__ == "__main__":

@@ -306,7 +306,10 @@ def test_mlp_forward_backward_adamw_golden(golden):
     names = [str(n) for n in g["pol_names"]]
     pol = MLPPolicy(obs_dim=12, action_dim=3, num_action_chunks=1)
     assert [n for n, _ in pol.named_parameters()] == names
-    pol.load_state_dict({n: _t(g["pol_p_" + n]) for n in names})
+    from test_oracle_golden import _golden_view, _policy_grads, _policy_init
+
+    p0 = _policy_init(golden, names)
+    pol.load_state_dict(p0)
     states, action = _t(g["pol_states"]).cuda(), _t(g["pol_action"]).cuda()
     out = pol.forward_train(states, action)
     torch.testing.assert_close(out["logprobs"].cpu(), _t(g["pol_logprobs"]), rtol=RTOL, atol=1e-5)
@@ -316,15 +319,15 @@ def test_mlp_forward_backward_adamw_golden(golden):
     pol.backward(_t(g["pol_wl"]).cuda(), _t(g["pol_wv"]).cuda(), _t(g["pol_we"]).cuda())
     worst = 0.0
     for n, gr in pol.named_grads():
-        ref = _t(g["pol_g_" + n])
+        got, ref = _golden_view(g, "pol_g_" + n, gr.cpu())
         # parameter gradients are sums over samples with cancellation: the bar is 1e-4 relative per element plus 1e-5 of
         # the tensor's own scale (round 1 used rtol 1e-3; measured max |diff| / max |ref| is printed)
-        torch.testing.assert_close(gr.cpu(), ref, rtol=RTOL, atol=1e-5 * max(1.0, ref.abs().max().item()), msg=n)
-        worst = max(worst, ((gr.cpu() - ref).abs().max() / ref.abs().max().clamp_min(1e-30)).item())
+        torch.testing.assert_close(got, ref, rtol=RTOL, atol=1e-5 * max(1.0, ref.abs().max().item()), msg=n)
+        worst = max(worst, ((got - ref).abs().max() / ref.abs().max().clamp_min(1e-30)).item())
     print(f"max |dW - ref| / max |ref| over parameter tensors: {worst:.2e}")
-    # optimiser: 3 steps with the reference's own gradients
+    # optimiser: 3 steps with the fixture's seeded gradients
     for n, gr in pol.named_grads():
-        gr.copy_(_t(g["pol_g_" + n]))
+        gr.copy_(_policy_grads(p0)[n])
     opt = FlatAdamW(pol, lr=3e-4, value_lr=1e-3, clip_grad=0.5)
     norms = []
     for _ in range(3):
@@ -335,7 +338,7 @@ def test_mlp_forward_backward_adamw_golden(golden):
         pol.flat_grads.mul_(opt.state[2].float())
     np.testing.assert_allclose(norms, g["pol_gradnorms"], rtol=1e-5)
     for n, p in pol.named_parameters():
-        torch.testing.assert_close(p.cpu(), _t(g["pol_p3_" + n]), rtol=1e-5, atol=1e-7, msg=n)
+        torch.testing.assert_close(*_golden_view(g, "pol_p3_" + n, p.cpu()), rtol=1e-5, atol=1e-7, msg=n)
     assert opt.state[0].item() == 3
 
 

@@ -1,6 +1,6 @@
 """Round-2 GPU parity: branches of already-tested kernels that no test exercised in round 1 (entropy term, critic
 warm-up, rollout_epoch merge, non-finite gradient skip), the fused rollout instances the multi-GPU runs use, the
-config-2 shapes end to end (tcgen05 path), optimiser warm-up / LR schedules, and GRPO with auto_reset off."""
+config-2 shapes end to end (tensor-core path), optimiser warm-up / LR schedules, and GRPO with auto_reset off."""
 import os
 
 import numpy as np
@@ -231,7 +231,7 @@ def test_frozen_group_is_untouched_and_lr_table_follows_lr_scale():
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("B", [600, 1100, 2100, 4096])
 def test_fused_rollout_instances_vs_oracle(B):
-    """E = ceil(B/148) = 5, 8, 15, 28 environments per CTA: the <=8, <=16 and register-tiled instances the N = 2/4/8
+    """E = ceil(B/132) = 5, 9, 16, 32 environments per CTA on a 132-SM H100: the <=8, <=16 and register-tiled instances the N = 2/4/8
     scaling runs use, with injected noise: flags bit-exact, floats within 1e-4 of the oracle's loop."""
     from rlinf_b200.config import synthetic_ppo_config
     from rlinf_b200.runner import EmbodiedRunner
@@ -267,7 +267,7 @@ def test_fused_rollout_instances_vs_oracle(B):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# end to end at the config-2 network shapes (obs=128, act=8 -> every hidden GEMM on tcgen05)
+# end to end at the config-2 network shapes (obs=128, act=8 -> every hidden GEMM on the tensor cores)
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.skipif(os.environ.get("RB200_SLOW", "1") == "0", reason="RB200_SLOW=0 skips the ~1 min oracle run")
 def test_runner_update_vs_oracle_at_config2_network_shapes():
@@ -406,12 +406,12 @@ def test_two_rank_nccl_update_matches_oracle(tmp_path, graph):
     import sys
 
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     if graph and os.environ.get("RB200_EXPERIMENTAL", "0") != "1":
-        # measured on 2 x B200: with the NCCL all-reduce captured inside the step graph the run never completed (500 s
-        # timeout, profiles/r02_two_rank_nccl.txt); multi-rank graphed steps are therefore opt-in
-        # (actor.cuda_graph_multi_rank) and this variant only runs with RB200_EXPERIMENTAL=1
-        pytest.skip("experimental: multi-rank CUDA-graphed optimiser step (hangs on 2 x B200)")
+        # with the NCCL all-reduce captured inside the step graph the 2-rank run has not been seen to complete;
+        # multi-rank graphed steps are therefore opt-in (actor.cuda_graph_multi_rank) and this variant only runs with
+        # RB200_EXPERIMENTAL=1
+        pytest.skip("experimental: multi-rank CUDA-graphed optimiser step")
     s = socket.socket()
     s.bind(("127.0.0.1", 0))
     port = s.getsockname()[1]

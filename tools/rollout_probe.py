@@ -1,4 +1,4 @@
-"""ms per T-step rollout for the three implementations (tc = persistent tcgen05 kernel, fused = fp32 SIMT persistent
+"""ms per T-step rollout for the three implementations (tc = persistent wgmma kernel, fused = fp32 SIMT persistent
 kernel, graph = per-kernel CUDA graph), CUDA events, device Philox.  usage: python tools/rollout_probe.py [B ...]"""
 import sys
 import torch

@@ -1,5 +1,5 @@
 // Stand-alone probe: how fast can one strip-per-CTA kernel pull a [T,B] step-major tensor through TMA / LDG?
-// (Used to find what bounds the GAE kernel; build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o
+// (Used to find what bounds the GAE kernel; build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o
 //  tools/tma_probe tools/tma_probe.cu ; run on the GPU box.)
 #include <cuda.h>
 #include <cudaTypedefs.h>

@@ -10,7 +10,7 @@ for n, IN in [(32, 32), (64, 32), (256, 256)]:
     Z *= (torch.arange(n, device='cuda').float().view(n, 1) % 3 + 1)
     dW = torch.zeros(256, IN, device='cuda')
     work = torch.empty(2 * n * (256 + IN), device='cuda')
-    L.check(lib.rb200_tc_wgrad(L.ptr(Z), L.ptr(H), L.ptr(dW), n, IN, L.ptr(work), L.stream_ptr()), "w")
+    L.check(lib.rb200_tc_wgrad_h(L.ptr(Z), L.ptr(H), L.ptr(dW), n, IN, None, L.stream_ptr()), "w")
     torch.cuda.synchronize()
     ref = Z.double().T @ H.double()
     print(f"n={n} IN={IN} dW absmax {dW.abs().max().item():.4f} ref absmax {ref.abs().max().item():.4f} nonzero {int((dW != 0).sum())}/{dW.numel()}")
