@@ -366,6 +366,27 @@ int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void*
                      int bootstrap_on_done, double gamma, double p_term, double noise_std, double reward_noise_std,
                      rb200_stream_t stream);
 
+/* Chunked variant of the persistent tensor-core rollout (num_action_chunks = C > 1, act_dim = C*A): per chunk step
+ * one actor / value inference on obs_n, then C synthetic-env sub-steps without reset (sub-step c uses action columns
+ * [cA, (c+1)A)), flags OR-ed over the chunk and written to the chunk's last column, one auto-reset after the chunk and
+ * the truncation bootstrap on the last column - the semantics and random streams of rb200_synth_env_chunk_step plus
+ * rb200_bootstrap_rewards_ld.  T = chunk steps; buffers: states [T+1,B,obs], actions / logprobs [T,B,C*A],
+ * values [T+1,B,C], rewards [T,B,C], terminations / truncations / dones [T+1,B,C], final_values [B,C];
+ * policy_noise [T,B,C*A], env_noise [T,B,C*(obs+2)+obs] (per sub-step eps[obs] | eps_r | u, then reset[obs]).
+ * The pack comes from rb200_rollout_tc_prepare(), which accepts these layouts too.
+ * rb200_rollout_tc_chunked_supported() == 0 iff hidden == 256, obs_dim % 32 == 0, obs_dim <= 128,
+ * 2 <= C <= 8, act_dim = C*A with 1 <= A <= 8 and C*A <= 32, value_dim == C. */
+int rb200_rollout_tc_chunked_supported(const rb200_mlp_layout* L, int num_action_chunks, int B);
+int rb200_rollout_tc_chunked(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
+                             float* states, float* actions, float* logprobs, float* values, float* rewards,
+                             uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
+                             float* final_values, int32_t* elapsed, const float* policy_noise,
+                             const float* env_noise, const uint64_t* counter_policy, const uint64_t* counter_env,
+                             uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
+                             int num_action_chunks, int max_episode_steps, int auto_reset, int bootstrap_on_done,
+                             double gamma, double p_term, double noise_std, double reward_noise_std,
+                             rb200_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * SURVEY 8(f)3: token log-probabilities and entropies straight from the logits (csrc/logits.cu).
  * Replaces compute_logprobs_from_logits (rlinf/utils/utils.py:454-492, = -cross_entropy) and

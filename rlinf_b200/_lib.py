@@ -126,6 +126,9 @@ SIGNATURES = {
     "rb200_rollout_tc_prepare": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_void_p]),
     "rb200_rollout_tc": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 5 +
                          [c_double] * 4 + [c_void_p]),
+    "rb200_rollout_tc_chunked_supported": (c_int, [C.POINTER(MlpLayout), c_int, c_int]),
+    "rb200_rollout_tc_chunked": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 6 +
+                                 [c_double] * 4 + [c_void_p]),
     "rb200_logits_logprob_entropy_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                                  c_int, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "rb200_logits_logprob_entropy_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,

@@ -59,8 +59,26 @@ struct Misc {
   uint64_t vhead, obs_ready;
 };
 constexpr int kArgsBytes = 512;  // shared-memory copy of the kernel arguments for the out-of-line helpers
+constexpr int kOffArgs = kOffMisc + (((int)sizeof(Misc) + 15) & ~15);
 constexpr int kSmemBytes = kOffMisc + (int)sizeof(Misc) + kArgsBytes + 1024;
 static_assert(kSmemBytes <= 232448, "rollout_tc shared memory");
+
+// Chunked variant (num_action_chunks = C > 1, act = C*A): the C*A actions of a chunk step are kept behind the argument
+// copy (the C = 1 map above is unchanged); the mean head [C*A, 256] is read through L2 and the value head [C, 256]
+// takes the place of Misc::mw.
+constexpr int kMaxChunks = 8;
+constexpr int kMaxActChunk = 32;  // C*A
+struct ChunkSmem {
+  float act[kNE * kMaxActChunk];  // [env][C*A] actions of this chunk step
+  int orf[kNE];                   // term | trunc << 1 of the sub-steps so far (OR over the chunk)
+};
+constexpr int kOffChunk = kOffArgs + kArgsBytes;
+constexpr int kSmemBytesChunk = kOffChunk + (int)sizeof(ChunkSmem) + 1024;
+static_assert(kSmemBytesChunk <= 232448, "rollout_tc chunked shared memory");
+static_assert(kMaxChunks * kH <= kMaxActTc * kH, "chunked value head in Misc::mw");
+__device__ __forceinline__ ChunkSmem* chunk_smem(Misc* ms) {
+  return reinterpret_cast<ChunkSmem*>(reinterpret_cast<uint8_t*>(ms) + (kOffChunk - kOffMisc));
+}
 
 struct TcArgs {
   rb200_mlp_layout L;
@@ -70,22 +88,23 @@ struct TcArgs {
   float* states;         // [T+1, B, obs]
   float* actions;        // [T, B, act]
   float* logp;           // [T, B, act]
-  float* values;         // [T+1, B]
-  float* rewards;        // [T, B]
-  uint8_t* term;         // [T+1, B]
+  float* values;         // [T+1, B, C]
+  float* rewards;        // [T, B, C]
+  uint8_t* term;         // [T+1, B, C]
   uint8_t* trunc;
   uint8_t* done;
   float* final_obs;      // [B, obs]
-  float* final_values;   // [B]
+  float* final_values;   // [B, C]
   int32_t* elapsed;      // [B]
   const float* policy_noise;
   const float* env_noise;
   const uint64_t* counter_p;
   const uint64_t* counter_e;
   uint64_t seed_p, seed_e, offset_p;
-  int T, B, obs, act;
+  int T, B, obs, act;    // T = chunk steps, act = C*A
   int max_episode_steps, auto_reset, bootstrap_on_done;
   float gamma, p_term, noise_std, reward_noise_std;
+  int C;                 // num_action_chunks (1 in the unchunked kernel)
 };
 static_assert(sizeof(TcArgs) <= kArgsBytes, "TcArgs shared-memory copy");
 
@@ -193,10 +212,20 @@ __device__ __noinline__ float policy_draw(unsigned long long seed, unsigned long
 // the math, then all stores - keep 4-16 independent chains in flight per lane.  zs = x.W_s (env product), eps_s = this
 // step's N(0,1) draws, both fp32 [32][obs] in the (now free) actor buffer.  Same arithmetic order as env_finish_kernel
 // (rollout.cu) except tanh (MUFU-based tanh_fast, 3e-7 abs).
+// kChunk: t counts env sub-steps, chunk step n = t / C, sub-step c = t % C, with the semantics of
+// env_substep_kernel + chunk_finish_kernel: sub-step c uses action columns [cA, (c+1)A), no reset inside the chunk,
+// flags OR-ed over the chunk and written to column C-1 only, one auto-reset after the last sub-step.
+template <bool kChunk>
 __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obuf, uint32_t ob_half, const float* zs,
                                             const float* eps_s, int w8, int lane, int t, int e0, int nE, int nk,
                                             uint64_t c_e, bool boot) {
   const int obs = p.obs, B = p.B, T = p.T;
+  const int Cn = kChunk ? p.C : 1;
+  const int n = kChunk ? t / Cn : t, sub = t - n * Cn;
+  const bool last = !kChunk || sub == Cn - 1;
+  const int A = kChunk ? p.act / Cn : p.act;
+  const int nzw = Cn * (obs + 2) + obs;  // env_noise row: per sub-step eps[obs] | eps_r | u, then reset[obs]
+  ChunkSmem* cs = chunk_smem(ms);
   float v[4][4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
@@ -206,17 +235,23 @@ __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obu
       const int c = lane + 32 * k;
       float wa[kMaxActTc];
 #pragma unroll
-      for (int a = 0; a < kMaxActTc; ++a) wa[a] = a < p.act ? __ldg(p.w_a + a * obs + c) : 0.f;
+      for (int a = 0; a < kMaxActTc; ++a) wa[a] = a < A ? __ldg(p.w_a + a * obs + c) : 0.f;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int e = w8 * 4 + i;
-        const float4 a0 = *reinterpret_cast<const float4*>(ms->act + e * kMaxActTc);
-        const float4 a1 = *reinterpret_cast<const float4*>(ms->act + e * kMaxActTc + 4);
         float z = zs[e * obs + c];
-        z = fmaf(a0.x, wa[0], z); z = fmaf(a0.y, wa[1], z); z = fmaf(a0.z, wa[2], z); z = fmaf(a0.w, wa[3], z);
-        z = fmaf(a1.x, wa[4], z); z = fmaf(a1.y, wa[5], z); z = fmaf(a1.z, wa[6], z); z = fmaf(a1.w, wa[7], z);
+        if constexpr (kChunk) {
+          const float* ac = cs->act + e * kMaxActChunk + sub * A;
+#pragma unroll
+          for (int a = 0; a < kMaxActTc; ++a) z = fmaf(a < A ? ac[a] : 0.f, wa[a], z);
+        } else {
+          const float4 a0 = *reinterpret_cast<const float4*>(ms->act + e * kMaxActTc);
+          const float4 a1 = *reinterpret_cast<const float4*>(ms->act + e * kMaxActTc + 4);
+          z = fmaf(a0.x, wa[0], z); z = fmaf(a0.y, wa[1], z); z = fmaf(a0.z, wa[2], z); z = fmaf(a0.w, wa[3], z);
+          z = fmaf(a1.x, wa[4], z); z = fmaf(a1.y, wa[5], z); z = fmaf(a1.z, wa[6], z); z = fmaf(a1.w, wa[7], z);
+        }
         float ep = eps_s[e * obs + c];
-        if (p.env_noise && e < nE) ep = p.env_noise[((size_t)t * B + e0 + e) * (2 * obs + 2) + c];
+        if (p.env_noise && e < nE) ep = p.env_noise[((size_t)n * B + e0 + e) * nzw + sub * (obs + 2) + c];
         v[i][k] = tanh_fast(z + p.noise_std * ep);
       }
     }
@@ -237,16 +272,20 @@ __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obu
     const int e = w8 * 4 + i;
     float er = ms->er[e], u = ms->uu[e];
     if (p.env_noise && e < nE) {
-      const float* nz = p.env_noise + ((size_t)t * B + e0 + e) * (2 * obs + 2);
+      const float* nz = p.env_noise + ((size_t)n * B + e0 + e) * nzw + sub * (obs + 2);
       er = nz[obs];
       u = nz[obs + 1];
     }
     const int el = ms->el[e] + 1;
-    const bool term = u < p.p_term;
-    const bool trunc = p.max_episode_steps > 0 && el >= p.max_episode_steps;
+    bool term = u < p.p_term;
+    bool trunc = p.max_episode_steps > 0 && el >= p.max_episode_steps;
+    if (kChunk && sub > 0) {
+      term |= (cs->orf[e] & 1) != 0;
+      trunc |= (cs->orf[e] & 2) != 0;
+    }
     const bool done = term || trunc;
-    reset[i] = done && p.auto_reset;
-    const bool flagged = boot && (p.bootstrap_on_done ? done : trunc);
+    reset[i] = last && done && p.auto_reset;
+    const bool flagged = last && boot && (p.bootstrap_on_done ? done : trunc);
     rw[i] = -sq[i] / (float)obs + p.reward_noise_std * er;
     bits[i] = (term ? 1 : 0) | (trunc ? 2 : 0) | (done ? 4 : 0) | (flagged ? 8 : 0) | ((reset[i] ? 0 : el) << 4);
   }
@@ -257,14 +296,17 @@ __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obu
       const int e = w8 * 4 + i;
       if (e < nE) {
         const int64_t row = e0 + e;
-        const size_t o = (size_t)(t + 1) * B + row;
-        p.term[o] = bits[i] & 1;
-        p.trunc[o] = (bits[i] >> 1) & 1;
-        p.done[o] = (bits[i] >> 2) & 1;
+        const size_t o = ((size_t)(n + 1) * B + row) * Cn + sub;
+        const int fl = last ? bits[i] : 0;  // flags of a chunk go to its last column
+        p.term[o] = fl & 1;
+        p.trunc[o] = (fl >> 1) & 1;
+        p.done[o] = (fl >> 2) & 1;
+        if (kChunk) cs->orf[e] = bits[i] & 3;
         ms->el[e] = bits[i] >> 4;
         ms->flag[e] = (bits[i] >> 3) & 1;
         ms->rew[e] = rw[i];
-        if (!(bits[i] & 8)) p.rewards[(size_t)t * B + row] = rw[i];  // flagged: written by the value warps with the bootstrap
+        // flagged: written by the value warps with the bootstrap
+        if (!(bits[i] & 8)) p.rewards[((size_t)n * B + row) * Cn + sub] = rw[i];
       }
     }
   }
@@ -278,13 +320,16 @@ __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obu
     for (int k = 0; k < 4; ++k) nw[k] = v[i][k];
     if (reset[i]) {  // warp-uniform, rare (one env-step in ~80): fresh state from the same stream, same draw order
       if (p.env_noise) {
-        const float* nz = p.env_noise + ((size_t)t * B + row) * (2 * obs + 2);
+        const float* nz = p.env_noise + ((size_t)n * B + row) * nzw + Cn * (obs + 2);
 #pragma unroll
         for (int k = 0; k < 4; ++k)
-          if (k < nk) nw[k] = nz[obs + 2 + lane + 32 * k];
+          if (k < nk) nw[k] = nz[lane + 32 * k];
       } else {
-        const EnvDraws d = env_reset_draws(p.seed_e, (unsigned long long)row * 32ull + lane, (c_e + (uint64_t)t) * 64ull,
-                                           nk, lane == 0);
+        // chunked: chunk_finish_kernel's fresh window, 32 outputs behind the last sub-step's
+        const EnvDraws d = kChunk ? env_draws(p.seed_e, (unsigned long long)row * 32ull + lane,
+                                              (c_e * (uint64_t)Cn + (uint64_t)t) * 64ull + 32ull, nk, 0)
+                                  : env_reset_draws(p.seed_e, (unsigned long long)row * 32ull + lane,
+                                                    (c_e + (uint64_t)t) * 64ull, nk, lane == 0);
 #pragma unroll
         for (int k = 0; k < 4; ++k) nw[k] = d.e[k];
       }
@@ -293,10 +338,11 @@ __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obu
     for (int k = 0; k < 4; ++k) {
       if (k < nk) {
         const int c = lane + 32 * k;
-        if (t == T - 1) p.final_obs[(size_t)row * obs + c] = v[i][k];
-        store_split(obuf, ob_half, (uint32_t)k * 4096u + sw64_off(kNE + e, lane), v[i][k]);  // pre-reset observation
+        // inside a chunk only the next sub-step's operand (rows 0..31) is written
+        if (last && n == T - 1) p.final_obs[(size_t)row * obs + c] = v[i][k];
+        if (last) store_split(obuf, ob_half, (uint32_t)k * 4096u + sw64_off(kNE + e, lane), v[i][k]);  // pre-reset observation
         store_split(obuf, ob_half, (uint32_t)k * 4096u + sw64_off(e, lane), nw[k]);
-        p.states[((size_t)(t + 1) * B + row) * obs + c] = nw[k];
+        if (last) p.states[((size_t)(n + 1) * B + row) * obs + c] = nw[k];
       }
     }
   }
@@ -390,6 +436,9 @@ __device__ __noinline__ void tower_layer(Misc* ms, uint32_t ring_a, int slot0, u
   named_sync(bar_id, 128);
 }
 
+// kChunk: num_action_chunks = p.C > 1.  Per chunk step the towers run once; the env warpgroup runs C x.W_s products and
+// the env and actor warpgroups C dynamics finishes, the first one after the value tower has read the observation tile.
+template <bool kChunk>
 __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -429,8 +478,14 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
     ms->nflag = 0;
     rb::tma::fence_barrier_init();
   }
-  for (int i = tid; i < act * kH; i += kThreads) ms->mw[i] = P[p.L.mw + i];
-  for (int i = tid; i < kH; i += kThreads) ms->vw[i] = P[p.L.vw3 + i];
+  const int Cn = kChunk ? p.C : 1;
+  if constexpr (kChunk) {
+    for (int i = tid; i < Cn * kH; i += kThreads) ms->mw[i] = P[p.L.vw3 + i];  // value head [C, 256]
+    if (tid < kNE) chunk_smem(ms)->orf[tid] = 0;
+  } else {
+    for (int i = tid; i < act * kH; i += kThreads) ms->mw[i] = P[p.L.mw + i];
+    for (int i = tid; i < kH; i += kThreads) ms->vw[i] = P[p.L.vw3 + i];
+  }
   for (int i = tid; i < 2 * kNE * obs; i += kThreads) {  // rows 0..31 = current observation, rows 32..63 = zeros
     const int r = i / obs, c = i - r * obs;
     const float v = (r < nE) ? p.states[(size_t)(e0 + r) * obs + c] : 0.f;
@@ -450,7 +505,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
   if (warp == 12) {
     // ================= weight-stream producer: three rings, polled (no ring waits for another) =================
     if (lane == 0) {
-      const uint32_t total[3] = {(uint32_t)T * n_env, (uint32_t)T * n_tower, (uint32_t)(T + 1) * n_tower};
+      const uint32_t total[3] = {(uint32_t)(T * Cn) * n_env, (uint32_t)T * n_tower, (uint32_t)(T + 1) * n_tower};
       const int slot0[3] = {kEnvSlot0, kActSlot0, kValSlot0}, nslots[3] = {kEnvSlots, kActSlots, kValSlots};
       uint32_t j[3] = {0u, 0u, 0u};
       while (j[0] < total[0] || j[1] < total[1] || j[2] < total[2]) {
@@ -492,6 +547,39 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
                        w, lane);
       tower_layer<kNE>(ms, ring_a, kActSlot0, base + l0 + 16, 8, abuf_a, kAbufHalf, 2048u, bias[2], abuf, kAbufHalf, 2048u, 1,
                        1, w, lane);
+      if constexpr (kChunk) {
+        // ---- chunked mean head [C*A, 256] from L2: warp w takes actions w, w+4, ..., its weight row in registers,
+        //      one warp-reduced dot product per environment; lane e then samples (e, a) ----
+        float* cact = chunk_smem(ms)->act;
+        for (int a = w; a < act; a += 4) {
+          const float4* wr = reinterpret_cast<const float4*>(P + p.L.mw + (size_t)a * kH);
+          const float4 w0 = __ldg(wr + lane), w1 = __ldg(wr + 32 + lane);
+          float mine = 0.f;
+#pragma unroll 4
+          for (int e = 0; e < kNE; ++e) {
+            const float4 g0 = *reinterpret_cast<const float4*>(h3 + e * kH + lane * 4);
+            const float4 g1 = *reinterpret_cast<const float4*>(h3 + e * kH + 128 + lane * 4);
+            float s = g0.x * w0.x + g0.y * w0.y + g0.z * w0.z + g0.w * w0.w + g1.x * w1.x + g1.y * w1.y +
+                      g1.z * w1.z + g1.w * w1.w;
+            s = rb::warp_sum(s);
+            if (lane == e) mine = s;
+          }
+          if (lane < nE) {
+            const int64_t row = e0 + lane;
+            const float mean = mine + P[p.L.mb + a];
+            const float sd = expf(P[p.L.logstd + a]);
+            const float z = p.policy_noise ? p.policy_noise[((size_t)t * B + row) * act + a]
+                                           : policy_draw(p.seed_p, (unsigned long long)(row * act + a),
+                                                         p.offset_p + 4ull * (c_p + (uint64_t)t));
+            const float xa = mean + sd * z;
+            const float d = xa - mean;
+            const size_t o = ((size_t)t * B + row) * act + a;
+            p.actions[o] = xa;
+            p.logp[o] = -(d * d) / (2.0f * (sd * sd)) - logf(sd) - kHalfLog2Pi;
+            cact[lane * kMaxActChunk + a] = xa;
+          }
+        }
+      } else {
       // ---- mean head + Normal sample + log-prob: one (env, action) pair per thread.  Each thread does its own
       //      256-long dot product (float4 reads rotated by the lane so that a warp touches every bank once): no
       //      warp reductions, no shared-memory hand-off between head and sampling ----
@@ -529,14 +617,18 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
           ms->act[e * kMaxActTc + a] = xa;
         }
       }
+      }
       // ---- env finish, shared with the env warps (barrier 4 = actor + env groups): #1 actions sampled / h3 dead,
-      //      #2 zs + eps in the actor buffer, #3 next observation operand complete ----
+      //      #2 zs + eps in the actor buffer, #3 next observation operand complete (#2 and #3 once per sub-step) ----
       named_sync(4, 256);
-      named_sync(4, 256);
-      env_finish4(*pa, ms, obuf, ob_half, reinterpret_cast<const float*>(abuf), reinterpret_cast<const float*>(abuf + kAbufHalf),
-                  w, lane, t, e0, nE, sg.nkb0, c_e, boot);
-      rb::tma::fence_proxy_async();
-      named_sync(4, 256);
+      for (int c = 0; c < Cn; ++c) {
+        named_sync(4, 256);
+        env_finish4<kChunk>(*pa, ms, obuf, ob_half, reinterpret_cast<const float*>(abuf),
+                            reinterpret_cast<const float*>(abuf + kAbufHalf), w, lane, t * Cn + c, e0, nE, sg.nkb0, c_e,
+                            boot);
+        rb::tma::fence_proxy_async();
+        named_sync(4, 256);
+      }
     }
   } else if (warp >= 8) {
     // ================= value tower: layers, value head, truncation bootstrap =================
@@ -563,6 +655,24 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
         tower_layer<2 * kNE>(ms, ring_a, kValSlot0, s2, 8, vbuf_a, kVbufHalf, 4096u, bias[2], vbuf, kVbufHalf, 4096u, 1, 2, w, lane);
       }
       // ---- value head (columns 0..31: V(obs_t)) and bootstrap (columns 32..63: V(final_obs_{t-1}) where flagged) ----
+      //      chunked: C outputs per environment, the bootstrap uses output 0 and goes to the chunk's last column
+      if constexpr (kChunk) {
+        for (int e = w; e < nv; e += 4) {
+          const int eb = e < kNE ? e : e - kNE;
+          if (eb >= nE || (e >= kNE && !ms->flag[eb])) continue;  // warp-uniform
+          for (int c = 0; c < Cn; ++c) {
+            const float v = dot256(g3 + e * kH, ms->mw + c * kH, lane);
+            if (lane != 0) continue;
+            if (e < kNE) {
+              p.values[((size_t)t * B + e0 + e) * Cn + c] = v;
+            } else {
+              if (c == 0)
+                p.rewards[((size_t)(t - 1) * B + e0 + eb) * Cn + Cn - 1] = __fadd_rn(ms->rew[eb], __fmul_rn(p.gamma, v));
+              p.final_values[(size_t)(e0 + eb) * Cn + c] = v;
+            }
+          }
+        }
+      } else {
       for (int e = w; e < nv; e += 4) {
         if (e < kNE) {
           const float v = dot256(g3 + e * kH, ms->vw, lane);
@@ -578,6 +688,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
           }
         }
       }
+      }
       __syncwarp();
       if (lane == 0) mbar_arrive(&ms->vhead);
     }
@@ -589,8 +700,10 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
     float* eps_s = reinterpret_cast<float*>(abuf + kAbufHalf);  // [32][obs] fp32 draws of this step
     const int nk = sg.nkb0;                       // observation columns per lane
     uint32_t p_vh = 0;
-    for (int t = 0; t < T; ++t) {
-      // ---- 1. Philox draws of this step for my 8 environments (same streams / order as env_finish_kernel) ----
+    for (int t = 0; t < T * Cn; ++t) {  // env (sub-)steps
+      const int sub = kChunk ? t % Cn : 0;
+      // ---- 1. Philox draws of this step for my 8 environments (same streams / order as env_finish_kernel; chunked:
+      //         env_substep_kernel, window ((c_e + n) C + c) * 64) ----
       float eps[8][4], eps_r[8], uu[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -605,7 +718,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
           const int e = ew * 8 + i;
           if (e < nE) {
             const EnvDraws d = env_draws(p.seed_e, (unsigned long long)(e0 + e) * 32ull + lane,
-                                         (c_e + (uint64_t)t) * 64ull, nk, lane == 0);
+                                         (c_e * (uint64_t)Cn + (uint64_t)t) * 64ull, nk, lane == 0);
 #pragma unroll
             for (int k = 0; k < 4; ++k) eps[i][k] = d.e[k];
             eps_r[i] = d.er;
@@ -618,9 +731,13 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
       layer_mma<kNE, 1>(zacc, ms, ring_a, kEnvSlot0, kEnvSlots, (uint32_t)t * n_env, sg.nkb0, obuf_a, ob_half, 4096u, lane);
       // ---- 3. wait for the value head, meet the actor group (#1: h3 dead, actions sampled), then park x.W_s
       //         (fp32 [32][obs]) and this step's draws in the free actor buffer ----
-      mbar_wait(&ms->vhead, p_vh);  // the value head of this step has consumed flag / rew of the previous step
-      p_vh ^= 1u;
-      named_sync(4, 256);
+      //         (chunked: at the first sub-step; the later ones overwrite only the actor buffer and the observation
+      //         rows 0..31, which no tower reads before the next chunk step)
+      if (sub == 0) {
+        mbar_wait(&ms->vhead, p_vh);  // the value head of this step has consumed flag / rew of the previous step
+        p_vh ^= 1u;
+        named_sync(4, 256);
+      }
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int e = ew * 8 + i;
@@ -646,10 +763,10 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
         }
       named_sync(4, 256);
       // ---- 4. finish 4 environments per warp (the actor group takes environments 0..15) ----
-      env_finish4(*pa, ms, obuf, ob_half, zs, eps_s, 4 + ew, lane, t, e0, nE, nk, c_e, boot);
+      env_finish4<kChunk>(*pa, ms, obuf, ob_half, zs, eps_s, 4 + ew, lane, t, e0, nE, nk, c_e, boot);
       rb::tma::fence_proxy_async();
       named_sync(4, 256);
-      if (gt == 0) {
+      if (sub == Cn - 1 && gt == 0) {
         int n = 0;
         for (int e = 0; e < kNE; ++e) n += ms->flag[e];
         ms->nflag = n;
@@ -723,15 +840,34 @@ extern "C" int rb200_rollout_tc_supported(const rb200_mlp_layout* L, int B) {
   return RB200_OK;
 }
 
+extern "C" int rb200_rollout_tc_chunked_supported(const rb200_mlp_layout* L, int num_action_chunks, int B) {
+  if (!L) return RB200_E_NULL;
+  const int Cn = num_action_chunks;
+  if (L->hidden != kH || Cn < 2 || Cn > kMaxChunks || L->value_dim != Cn) return RB200_E_UNSUPPORTED;
+  if (L->act_dim <= 0 || L->act_dim > kMaxActChunk || L->act_dim % Cn != 0 || L->act_dim / Cn > kMaxActTc)
+    return RB200_E_UNSUPPORTED;
+  if (L->obs_dim < 32 || L->obs_dim > kMaxObsTc || (L->obs_dim % 32) != 0) return RB200_E_UNSUPPORTED;
+  if (B <= 0) return RB200_E_UNSUPPORTED;
+  return RB200_OK;
+}
+
+namespace {
+// the pack holds the hidden layers and W_s only: any layout one of the two kernels runs
+int pack_supported(const rb200_mlp_layout* L) {
+  if (rb200_rollout_tc_supported(L, 1) == RB200_OK) return RB200_OK;
+  return rb200_rollout_tc_chunked_supported(L, L->value_dim, 1);
+}
+}  // namespace
+
 extern "C" int64_t rb200_rollout_tc_pack_bytes(const rb200_mlp_layout* L) {
-  if (!L || rb200_rollout_tc_supported(L, 1)) return 0;
+  if (!L || pack_supported(L)) return 0;
   return (int64_t)make_segs(L->obs_dim).total * kStageBytes;
 }
 
 extern "C" int rb200_rollout_tc_prepare(const rb200_mlp_layout* L, const float* params, const float* w_s, void* pack,
                                         rb200_stream_t stream) {
   if (!L || !params || !w_s || !pack) return RB200_E_NULL;
-  int e = rb200_rollout_tc_supported(L, 1);
+  int e = pack_supported(L);
   if (e) return e;
   if (reinterpret_cast<uintptr_t>(pack) & 15) return RB200_E_ALIGN;
   PackArgs a{};
@@ -743,16 +879,16 @@ extern "C" int rb200_rollout_tc_prepare(const rb200_mlp_layout* L, const float* 
   RB_RETURN_LAUNCH();
 }
 
-extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
-                                float* states, float* actions, float* logprobs, float* values, float* rewards,
-                                uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
-                                float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
-                                const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
-                                uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps,
-                                int auto_reset, int bootstrap_on_done, double gamma, double p_term, double noise_std,
-                                double reward_noise_std, rb200_stream_t stream) {
-  int e = rb200_rollout_tc_supported(L, B);
-  if (e) return e;
+namespace {
+template <bool kChunk>
+int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
+                      float* states, float* actions, float* logprobs, float* values, float* rewards,
+                      uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs, float* final_values,
+                      int32_t* elapsed, const float* policy_noise, const float* env_noise,
+                      const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
+                      uint64_t seed_env, uint64_t offset_policy, int T, int B, int num_action_chunks,
+                      int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma, double p_term,
+                      double noise_std, double reward_noise_std, rb200_stream_t stream) {
   if (!params || !pack || !w_a || !states || !actions || !logprobs || !values || !rewards || !terminations ||
       !truncations || !dones || !final_obs || !final_values || !elapsed)
     return RB200_E_NULL;
@@ -766,14 +902,52 @@ extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, 
   a.seed_p = seed_policy; a.seed_e = seed_env; a.offset_p = offset_policy; a.T = T; a.B = B; a.obs = L->obs_dim;
   a.act = L->act_dim; a.max_episode_steps = max_episode_steps; a.auto_reset = auto_reset;
   a.bootstrap_on_done = bootstrap_on_done; a.gamma = (float)gamma; a.p_term = (float)p_term;
-  a.noise_std = (float)noise_std; a.reward_noise_std = (float)reward_noise_std;
+  a.noise_std = (float)noise_std; a.reward_noise_std = (float)reward_noise_std; a.C = num_action_chunks;
+  const int smem = kChunk ? kSmemBytesChunk : kSmemBytes;
   static bool attr_done = false;
   if (!attr_done) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc_kernel<kChunk>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done = true;
   }
   const int grid = (B + kNE - 1) / kNE;
-  rollout_tc_kernel<<<grid, kThreads, kSmemBytes, rb::as_stream(stream)>>>(a);
+  rollout_tc_kernel<kChunk><<<grid, kThreads, smem, rb::as_stream(stream)>>>(a);
   rb::count_launch();
   RB_RETURN_LAUNCH();
+}
+}  // namespace
+
+extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
+                                float* states, float* actions, float* logprobs, float* values, float* rewards,
+                                uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
+                                float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
+                                const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
+                                uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps,
+                                int auto_reset, int bootstrap_on_done, double gamma, double p_term, double noise_std,
+                                double reward_noise_std, rb200_stream_t stream) {
+  int e = rb200_rollout_tc_supported(L, B);
+  if (e) return e;
+  return launch_rollout_tc<false>(L, params, pack, w_a, states, actions, logprobs, values, rewards, terminations,
+                                  truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
+                                  counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B, 1,
+                                  max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term, noise_std,
+                                  reward_noise_std, stream);
+}
+
+extern "C" int rb200_rollout_tc_chunked(const rb200_mlp_layout* L, const float* params, const void* pack,
+                                        const float* w_a, float* states, float* actions, float* logprobs, float* values,
+                                        float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
+                                        float* final_obs, float* final_values, int32_t* elapsed,
+                                        const float* policy_noise, const float* env_noise,
+                                        const uint64_t* counter_policy, const uint64_t* counter_env,
+                                        uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
+                                        int num_action_chunks, int max_episode_steps, int auto_reset,
+                                        int bootstrap_on_done, double gamma, double p_term, double noise_std,
+                                        double reward_noise_std, rb200_stream_t stream) {
+  int e = rb200_rollout_tc_chunked_supported(L, num_action_chunks, B);
+  if (e) return e;
+  return launch_rollout_tc<true>(L, params, pack, w_a, states, actions, logprobs, values, rewards, terminations,
+                                 truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
+                                 counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B,
+                                 num_action_chunks, max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term,
+                                 noise_std, reward_noise_std, stream);
 }

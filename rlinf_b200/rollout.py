@@ -188,23 +188,33 @@ class RolloutWorker:
         # persistent fused kernel: needs the synthetic env's dynamics (w_s, w_a) and a supported MLP shape
         # "auto" | "tc" (tensor-core persistent kernel) | True / "simt" (fp32 SIMT persistent kernel) | False (per-kernel graph)
         mode = cfg.rollout.get("fused_kernel", "auto")
-        self.num_action_chunks = int(getattr(buffer, "num_action_chunks", 1))
-        if self.num_action_chunks > 1:
-            if mode in ("tc", "simt", True):
-                raise ValueError("the persistent rollout kernels implement num_action_chunks == 1; chunked policies use "
-                                 "the per-kernel loop (rollout.fused_kernel: false / auto)")
-            mode = False
+        self.num_action_chunks = Cn = int(getattr(buffer, "num_action_chunks", 1))
+        if Cn > 1 and mode in ("simt", True):
+            raise ValueError("the persistent fp32 SIMT rollout kernel implements num_action_chunks == 1; chunked "
+                             "policies use the tensor-core kernel (rollout.fused_kernel: tc / auto) or the per-kernel "
+                             "loop (rollout.fused_kernel: false)")
         on_dev_env = policy.device.type == "cuda" and hasattr(env, "w_s") and hasattr(env, "w_a")
-        supported = (on_dev_env
+        supported = (on_dev_env and Cn == 1
                      and L.load().rb200_rollout_fused_supported(C.byref(policy.layout), int(buffer.B)) == 0)
-        tc_ok = (on_dev_env and L.load().rb200_rollout_tc_supported(C.byref(policy.layout), int(buffer.B)) == 0)
-        if mode == "tc" and not tc_ok:
-            raise ValueError("rollout.fused_kernel='tc' needs hidden 256, a value head, act_dim <= 8, obs_dim % 32 == 0 "
-                             "and obs_dim <= 128 (rb200_rollout_tc_supported)")
-        self._tc = tc_ok and (mode == "tc" or (mode == "auto" and int(buffer.B) >= self.TC_AUTO_MIN_ENVS))
+        if Cn > 1:
+            tc_ok = (on_dev_env and L.load().rb200_rollout_tc_chunked_supported(C.byref(policy.layout), Cn,
+                                                                               int(buffer.B)) == 0)
+            if mode == "tc" and not tc_ok:
+                raise ValueError("rollout.fused_kernel='tc' with num_action_chunks > 1 needs hidden 256, obs_dim % 32 "
+                                 "== 0, obs_dim <= 128, 2 <= num_action_chunks <= 8, 1 <= action_dim <= 8, "
+                                 "num_action_chunks * action_dim <= 32 and one value per sub-step "
+                                 "(rb200_rollout_tc_chunked_supported)")
+        else:
+            tc_ok = (on_dev_env and L.load().rb200_rollout_tc_supported(C.byref(policy.layout), int(buffer.B)) == 0)
+            if mode == "tc" and not tc_ok:
+                raise ValueError("rollout.fused_kernel='tc' needs hidden 256, a value head, act_dim <= 8, obs_dim % 32 "
+                                 "== 0 and obs_dim <= 128 (rb200_rollout_tc_supported)")
+        # chunked: `auto` keeps the per-kernel loop, measured faster than the kernel at 256-4096 environments on an
+        # H100 80GB HBM3 at 700 W (DESIGN.md §6)
+        self._tc = tc_ok and (mode == "tc" or (mode == "auto" and Cn == 1 and int(buffer.B) >= self.TC_AUTO_MIN_ENVS))
         if mode == "simt":
             mode = True
-        if self._tc:
+        if self._tc or Cn > 1:  # chunked policies below the threshold: the per-kernel loop
             mode = False
         if mode == "auto":
             sms = torch.cuda.get_device_properties(policy.device).multi_processor_count
@@ -231,7 +241,8 @@ class RolloutWorker:
         L.check(lib.rb200_counter_add(L.ptr(env.counter), buf.T, st), "counter_add")
 
     def _tc_rollout(self, policy_noise=None, env_noise=None):
-        """The whole T-step loop in one persistent tensor-core kernel (csrc/rollout_tc.cu)."""
+        """The whole T-step loop in one persistent tensor-core kernel (csrc/rollout_tc.cu); T = chunk steps when
+        num_action_chunks > 1."""
         lib = L.load()
         buf, pol, env = self.buf, self.policy, self.env
         st = L.stream_ptr()
@@ -240,14 +251,17 @@ class RolloutWorker:
         pack = pol._buf("rollout_tc_pack", (nbytes + 3) // 4)
         L.check(lib.rb200_rollout_tc_prepare(lay, L.ptr(pol.flat_params), L.ptr(env.w_s), L.ptr(pack), st),
                 "rollout_tc_prepare")
-        L.check(lib.rb200_rollout_tc(
-            lay, L.ptr(pol.flat_params), L.ptr(pack), L.ptr(env.w_a), L.ptr(buf.states), L.ptr(buf.actions),
-            L.ptr(buf.prev_logprobs), L.ptr(buf.prev_values), L.ptr(buf.rewards), L.ptr(buf.terminations),
-            L.ptr(buf.truncations), L.ptr(buf.dones), L.ptr(buf.final_obs), L.ptr(buf.final_values),
-            L.ptr(env.elapsed), L.ptr(policy_noise), L.ptr(env_noise), L.ptr(self.counter), L.ptr(env.counter),
-            self.seed, env.seed, 0, buf.T, buf.B, env.max_episode_steps, int(self.auto_reset),
-            int(self.bootstrap_type != "standard"), self.gamma, env.p_term, env.noise_std, env.reward_noise_std, st),
-            "rollout_tc")
+        args = (lay, L.ptr(pol.flat_params), L.ptr(pack), L.ptr(env.w_a), L.ptr(buf.states), L.ptr(buf.actions),
+                L.ptr(buf.prev_logprobs), L.ptr(buf.prev_values), L.ptr(buf.rewards), L.ptr(buf.terminations),
+                L.ptr(buf.truncations), L.ptr(buf.dones), L.ptr(buf.final_obs), L.ptr(buf.final_values),
+                L.ptr(env.elapsed), L.ptr(policy_noise), L.ptr(env_noise), L.ptr(self.counter), L.ptr(env.counter),
+                self.seed, env.seed, 0, buf.T, buf.B)
+        tail = (env.max_episode_steps, int(self.auto_reset), int(self.bootstrap_type != "standard"), self.gamma,
+                env.p_term, env.noise_std, env.reward_noise_std, st)
+        if self.num_action_chunks > 1:
+            L.check(lib.rb200_rollout_tc_chunked(*args, self.num_action_chunks, *tail), "rollout_tc_chunked")
+        else:
+            L.check(lib.rb200_rollout_tc(*args, *tail), "rollout_tc")
         L.check(lib.rb200_counter_add(L.ptr(self.counter), buf.T, st), "counter_add")
         L.check(lib.rb200_counter_add(L.ptr(env.counter), buf.T, st), "counter_add")
 

@@ -1,21 +1,40 @@
 """ms per T-step rollout for the three implementations (tc = persistent wgmma kernel, fused = fp32 SIMT persistent
-kernel, graph = per-kernel CUDA graph), CUDA events, device Philox.  usage: python tools/rollout_probe.py [B ...]"""
+kernel, graph = per-kernel CUDA graph), CUDA events, device Philox.
+usage: python tools/rollout_probe.py [--chunks C] [--action-dim A] [B ...]
+With --chunks C > 1 (num_action_chunks; T stays 512 env steps = 512 / C chunk steps) only tc and graph run."""
+import argparse
+import os
+import subprocess
 import sys
+
 import torch
 sys.path.insert(0, '.')
 from rlinf_b200.config import synthetic_ppo_config
 from rlinf_b200.runner import EmbodiedRunner
 
-Bs = [int(x) for x in sys.argv[1:]] or [512, 1024, 2048, 4096]
+ap = argparse.ArgumentParser()
+ap.add_argument("--chunks", type=int, default=1)
+ap.add_argument("--action-dim", type=int, default=None, help="A per sub-step (default 8, or 32 // C when chunked)")
+ap.add_argument("B", type=int, nargs="*")
+args = ap.parse_args()
+Cn = args.chunks
+A = args.action_dim or (8 if Cn == 1 else min(8, 32 // Cn))
+Bs = args.B or [512, 1024, 2048, 4096]
 T = 512
+try:
+    power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+except OSError:
+    power = "unknown"
+print(f"{torch.cuda.get_device_name()} power limit {power}; obs 128, A {A}, C {Cn}, T {T} env steps", flush=True)
 for B in Bs:
     row = {}
-    import os
-    modes = (("tc", "tc"), ("fused", True), ("graph", False))
+    modes = (("tc", "tc"), ("fused", True), ("graph", False)) if Cn == 1 else (("tc", "tc"), ("graph", False))
     if os.environ.get("RB200_PROBE_MODES"):
         modes = tuple(m for m in modes if m[0] in os.environ["RB200_PROBE_MODES"].split(","))
     for name, mode in modes:
-        cfg = synthetic_ppo_config(B=B, T=T, obs_dim=128, action_dim=8, **{"rollout.fused_kernel": mode})
+        cfg = synthetic_ppo_config(B=B, T=T, obs_dim=128, action_dim=A, **{"rollout.fused_kernel": mode,
+                                                                            "actor.model.num_action_chunks": Cn})
         run = EmbodiedRunner(cfg)
         for _ in range(3):
             run.rollout_phase()
@@ -30,4 +49,4 @@ for B in Bs:
         row[name + "_chk"] = (float(b.rewards.mean()), float(b.prev_values.mean()), int(b.dones.sum()))
         del run
         torch.cuda.empty_cache()
-    print(f"B={B} T={T} ms/rollout: " + " ".join(f"{k}={v:.2f}" if isinstance(v, float) else f"{k}={v}" for k, v in row.items()), flush=True)
+    print(f"B={B} T={T} C={Cn} ms/rollout: " + " ".join(f"{k}={v:.2f}" if isinstance(v, float) else f"{k}={v}" for k, v in row.items()), flush=True)
