@@ -452,6 +452,31 @@ int rb200_bootstrap_rewards(float* rewards, const float* final_values, const uin
 int rb200_counter_add(uint64_t* counter_dev, uint64_t inc, rb200_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Policy evaluation (csrc/eval.cu; EmbodiedRunner.evaluate, rlinf/runners/embodied_runner.py:193-206,308-329).
+ * ---------------------------------------------------------------------------------------- */
+/* Eval-mode inference, _generate_actions(mode="eval") (mlp_policy.py:256-293): actor tower and mean head only,
+ * action [n,act] = mean; logprobs [n,act] = Normal(mean, exp(logstd)).log_prob(mean) (NULL = not computed);
+ * values [n,value_dim] = ValueHead(states) (NULL = value tower skipped).  No sampling, no RNG.
+ * work: rb200_mlp_fwd_scratch_floats(L, n) floats; wsplit as for rb200_mlp_sample (NULL = fp32 SIMT GEMMs). */
+int rb200_mlp_mean(const rb200_mlp_layout* L, const float* params, const float* wsplit, const float* states,
+                   int64_t n, float* action, float* logprobs, float* values, float* work, rb200_stream_t stream);
+/* Episode statistics of one chunk step of an evaluation rollout, one thread per env (ManiskillEnv._record_metrics /
+ * _reset_metrics / _handle_auto_reset, maniskill_env.py:225-271,327-390; EnvWorker.env_evaluate_step,
+ * env_worker.py:557-620).  rewards [B,C] fp32, done [B,C] (column C-1 = the chunk's done flag):
+ *   ret += rewards[c] for c = 0..C-1 in order (fp32);  len += C;
+ *   newly = auto_reset ? done : done && !prev_done;  prev_done |= done;
+ *   on newly: acc[b] += {1, ret, len, ret / (float)len} (fp64);
+ *   then, if auto_reset && done: ret = len = 0.
+ * ret [B] fp32, len [B] int32, prev_done [B] u8, acc [B,4] fp64 are zeroed by the caller at the start of an
+ * evaluation (ret / len / prev_done also at every env reset).  episode [B,3] (nullable): (return, length, reward) of
+ * the episode env b finished in this step, NaN in all three columns otherwise. */
+int rb200_episode_stats_step(const float* rewards, const uint8_t* done, int B, int C, int auto_reset, float* ret,
+                             int32_t* len, uint8_t* prev_done, double* acc, float* episode, rb200_stream_t stream);
+/* out[4] = {count, sum return, sum length, sum reward} over the B rows of acc [B,4], summed in a fixed order by one
+ * CTA (no atomics): repeated runs give bit-identical results. */
+int rb200_episode_stats_reduce(const double* acc, int B, double* out, rb200_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * a10 reward filter: replaces the filter_rewards block of EmbodiedFSDPActor._process_received_rollout_batch,
  *   workers/actor/embodied_fsdp_actor_worker.py:236-282 (= preprocess_embodied_batch, rlinf/utils/utils.py:803-830).
  *   rewards f32 [nc,B,C]; loss_mask bool [nc,B,C] or NULL; keep_env bool [B] (scratch/out);

@@ -149,6 +149,9 @@ SIGNATURES = {
     "rb200_grpo_video_advantages": (c_int, [c_void_p] * 4 + [c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "rb200_grpo_dynamic_turn_advantages": (c_int, [c_void_p] * 3 + [c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "rb200_sub": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "rb200_mlp_mean": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_int64] + [c_void_p] * 5),
+    "rb200_episode_stats_step": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int] + [c_void_p] * 6),
+    "rb200_episode_stats_reduce": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
 }
 
 _LIB: Optional[C.CDLL] = None

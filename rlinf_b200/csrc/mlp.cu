@@ -59,10 +59,10 @@ struct HeadFwdArgs {
   const float* noise;   // sample mode: [n,act] N(0,1) draws or null -> Philox
   uint64_t seed, offset;
   const uint64_t* counter;
-  int sample_mode;
+  int sample_mode;     // 0: given actions, 1: action ~ N(mean, std), 2: action = mean (eval mode)
   float* mean_out;     // [n,act] or null
-  float* action_out;   // sample mode
-  float* logprobs;     // [n,act]
+  float* action_out;   // sample modes
+  float* logprobs;     // [n,act] (null only in eval mode)
   float* entropy;      // [n,act] or null
   float* values;       // [n,vdim] or null
   int64_t n;
@@ -110,7 +110,10 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(HeadFwdArgs p) {
       const float ls = p.logstd[lane];
       const float sd = expf(ls);
       float x;
-      if (p.sample_mode) {
+      if (p.sample_mode == 2) {  // _generate_actions(mode="eval"): raw_action = action_mean.clone()
+        x = my_mean;
+        p.action_out[row * p.act + lane] = x;
+      } else if (p.sample_mode) {
         float z;
         if (p.noise) {
           z = p.noise[row * p.act + lane];
@@ -131,7 +134,7 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(HeadFwdArgs p) {
       // torch.distributions.Normal.log_prob: -((x-mu)^2)/(2 var) - log(sd) - log(sqrt(2 pi))
       const float d = x - my_mean;
       const float var = sd * sd;
-      p.logprobs[row * p.act + lane] = -(d * d) / (2.0f * var) - logf(sd) - kHalfLog2Pi;
+      if (p.logprobs) p.logprobs[row * p.act + lane] = -(d * d) / (2.0f * var) - logf(sd) - kHalfLog2Pi;
       if (p.entropy) p.entropy[row * p.act + lane] = 0.5f + kHalfLog2Pi + logf(sd);
       if (p.mean_out) p.mean_out[row * p.act + lane] = my_mean;
     }
@@ -779,6 +782,36 @@ extern "C" int rb200_mlp_sample(const rb200_mlp_layout* L, const float* params, 
   rb::count_launch();
   RB_RETURN_LAUNCH();
 }
+
+// Eval-mode inference (rb200_mlp_mean in eval.cu): actor tower (+ value tower when values != null) and the head with
+// action = mean.  Arguments are checked by the caller; work: rb200_mlp_fwd_scratch_floats(L, n) floats.
+namespace rb {
+int mlp_mean_forward(const rb200_mlp_layout* L, const float* params, const float* wsplit, const float* states,
+                     int64_t n, float* action, float* logprobs, float* values, float* work, cudaStream_t st) {
+  int e = check_layout(L);
+  if (e) return e;
+  const int64_t PF = act_floats(n);
+  float *H1 = work, *H2 = H1 + PF, *H3 = H2 + PF, *G1 = H3 + PF, *G2 = G1 + PF, *G3 = G2 + PF;
+  const float* P = params;
+  if (wsplit) {
+    TowerIO t[2] = {};
+    t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
+    t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
+    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, st))) return e;
+  } else {
+    if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
+    if (values && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
+  }
+  HeadFwdArgs h{};
+  h.h3 = H3; h.g3 = values ? G3 : nullptr; h.mw = P + L->mw; h.mb = P + L->mb;
+  h.logstd = P + L->logstd; h.vw3 = P + L->vw3; h.sample_mode = 2; h.action_out = action; h.logprobs = logprobs;
+  h.values = values; h.n = n; h.act = L->act_dim; h.vdim = L->value_dim;
+  const size_t smem = sizeof(float) * (size_t)(L->act_dim + (values ? L->value_dim : 0)) * kH;
+  head_fwd_kernel<<<head_grid(n), 256, smem, st>>>(h);
+  rb::count_launch();
+  RB_RETURN_LAUNCH();
+}
+}  // namespace rb
 
 // value tower + last linear layer only (no bias on the last layer: value_head.py:46)
 namespace {

@@ -206,11 +206,33 @@ class MLPPolicy:
                                     L.ptr(work), L.stream_ptr()), "mlp_value")
         return vals
 
-    def predict_action_batch(self, env_obs, calculate_values=True, noise=None, seed=0, offset=0, **kwargs):
-        """predict_action_batch (mlp_policy.py:296-321): returns (chunk_actions [B,C,A], result dict)."""
+    def mean(self, states, calculate_logprobs=True, calculate_values=True, out=None, work_key="mean"):
+        """_generate_actions(mode="eval") (mlp_policy.py:256-293): action = mean, no sampling.  Log-probs (of the mean
+        under Normal(mean, exp(logstd))) and values are skipped when not requested.  `out` = caller-provided action
+        rows; `work_key` names the scratch buffer (eval loops keep their own, apart from the training rollout's)."""
+        lib = L.load()
+        n = states.shape[0]
+        work = self._buf(work_key, lib.rb200_mlp_fwd_scratch_floats(C.byref(self.layout), n))
+        action = out if out is not None else torch.empty((n, self.act_dim), dtype=torch.float32, device=self.device)
+        logp = torch.empty_like(action) if calculate_logprobs else None
+        vals = torch.empty((n, self.value_dim), dtype=torch.float32, device=self.device) if (
+            calculate_values and self.value_dim > 0) else None
+        L.check(lib.rb200_mlp_mean(C.byref(self.layout), L.ptr(self.flat_params), self._ws(), L.ptr(states), n,
+                                   L.ptr(action), L.ptr(logp), L.ptr(vals), L.ptr(work), L.stream_ptr()), "mlp_mean")
+        return action, logp, vals
+
+    def predict_action_batch(self, env_obs, calculate_values=True, noise=None, seed=0, offset=0, mode="train",
+                             **kwargs):
+        """predict_action_batch (mlp_policy.py:296-321): returns (chunk_actions [B,C,A], result dict).
+        mode "train" samples N(mean, exp(logstd)); mode "eval" returns the mean."""
         states = env_obs["states"]
-        action, logp, vals = self.sample(states, noise=noise, seed=seed, offset=offset,
-                                         calculate_values=calculate_values)
+        if mode == "train":
+            action, logp, vals = self.sample(states, noise=noise, seed=seed, offset=offset,
+                                             calculate_values=calculate_values)
+        elif mode == "eval":
+            action, logp, vals = self.mean(states, calculate_values=calculate_values)
+        else:
+            raise NotImplementedError(f"mode={mode!r}")
         if vals is None:
             vals = torch.zeros((states.shape[0], 1), dtype=torch.float32, device=self.device)
         result = {"prev_logprobs": logp, "prev_values": vals,

@@ -364,3 +364,103 @@ class RolloutWorker:
             self._graph = g
         self._graph.replay()
         self._calls += 1
+
+
+class EvalWorker:
+    """Deterministic evaluation rollouts of one rank: EnvWorker.evaluate / env_evaluate_step (rlinf/workers/env/
+    env_worker.py:557-620,1374-1461) against MultiStepRolloutWorker.evaluate with predict_action_batch(mode="eval").
+
+    Per chunk step: action = policy mean (rb200_mlp_mean, no value tower), one env chunk step, then the episode
+    statistics (rb200_episode_stats_step).  Nothing of the trajectory is kept: two [B,obs] state tensors used in turn
+    and one [B,C*A] / [B,C] row set.  The env is reset at the first eval epoch and, with auto_reset off, at every epoch
+    (running return / length / prev_done reset with it); with auto_reset on its state carries over between epochs.
+    The statistics stay on the device until `run()` has reduced them to [count, sum return, sum length, sum reward]."""
+
+    def __init__(self, cfg, policy, env, num_action_chunks=1):
+        ev = cfg.env.eval
+        self.policy, self.env = policy, env
+        self.num_action_chunks = Cn = int(num_action_chunks)
+        T = int(ev.max_steps_per_rollout_epoch)
+        if T % Cn != 0:
+            raise ValueError(f"env.eval.max_steps_per_rollout_epoch {T} is not a multiple of num_action_chunks {Cn}")
+        self.n_chunk_steps = T // Cn
+        self.rollout_epoch = int(ev.get("rollout_epoch", 1))
+        self.auto_reset = bool(ev.auto_reset)
+        self._use_graph = bool(cfg.rollout.get("enable_cuda_graph", True))
+        B, obs, dev = env.num_envs, env.obs_dim, policy.device
+        f32, u8 = torch.float32, torch.uint8
+        self.B = B
+        self.states = torch.zeros(2, B, obs, dtype=f32, device=dev)
+        self.final_obs = torch.zeros(B, obs, dtype=f32, device=dev)
+        self.actions = torch.zeros(B, policy.act_dim, dtype=f32, device=dev)
+        self.rewards = torch.zeros(B, Cn, dtype=f32, device=dev)
+        self.terminations = torch.zeros(B, Cn, dtype=u8, device=dev)
+        self.truncations = torch.zeros(B, Cn, dtype=u8, device=dev)
+        self.dones = torch.zeros(B, Cn, dtype=u8, device=dev)
+        self.ret = torch.zeros(B, dtype=f32, device=dev)
+        self.len = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.prev_done = torch.zeros(B, dtype=u8, device=dev)
+        self.acc = torch.zeros(B, 4, dtype=torch.float64, device=dev)  # count, sum return, sum length, sum reward
+        self.sums = torch.zeros(4, dtype=torch.float64, device=dev)
+        self._graph = None
+        self._calls = 0
+        self.graph_kernel_count = 0
+
+    def _reset(self, initial_states=None):
+        obs, _ = self.env.reset()
+        self.states[0].copy_(obs["states"] if initial_states is None else initial_states)
+        self.ret.zero_()
+        self.len.zero_()
+        self.prev_done.zero_()
+
+    def _epoch(self, env_noise=None, episodes=None):
+        """One eval epoch of n_chunk_steps chunk steps from states[0]; leaves the last observation in states[0].
+        env_noise [n, B, ...] (layout of the env's step); episodes [n, B, 3] receives the per-step episode records."""
+        lib = L.load()
+        pol, env, B, Cn = self.policy, self.env, self.B, self.num_action_chunks
+        st = L.stream_ptr()
+        pol.mark_params_changed()  # the weight split refresh is part of the (captured) epoch
+        for n in range(self.n_chunk_steps):
+            s, s_next = self.states[n & 1], self.states[(n + 1) & 1]
+            noise = None if env_noise is None else env_noise[n]
+            pol.mean(s, calculate_logprobs=False, calculate_values=False, out=self.actions, work_key="eval")
+            if Cn == 1:
+                env.step_into(s, self.actions, s_next, self.final_obs, self.rewards.view(B),
+                              self.terminations.view(B), self.truncations.view(B), self.dones.view(B), noise=noise)
+            else:
+                env.chunk_step_into(s, self.actions, s_next, self.final_obs, self.rewards, self.terminations,
+                                    self.truncations, self.dones, noise=noise)
+            L.check(lib.rb200_episode_stats_step(
+                L.ptr(self.rewards), L.ptr(self.dones), B, Cn, int(self.auto_reset), L.ptr(self.ret), L.ptr(self.len),
+                L.ptr(self.prev_done), L.ptr(self.acc), None if episodes is None else L.ptr(episodes[n]), st),
+                "episode_stats_step")
+        if self.n_chunk_steps % 2:
+            self.states[0].copy_(self.states[1])
+
+    def run(self, env_noise=None, initial_states=None, episodes=None) -> torch.Tensor:
+        """All eval epochs; returns the device tensor [count, sum return, sum length, sum reward] (fp64).
+        env_noise [rollout_epoch, n, B, ...] / initial_states [number of resets, B, obs]: pre-drawn draws (parity
+        tests; they run eagerly); episodes [rollout_epoch, n, B, 3]: optional per-step episode records."""
+        self.acc.zero_()
+        resets = 0
+        for e in range(self.rollout_epoch):
+            if e == 0 or not self.auto_reset:  # EnvWorker.evaluate: reset at the first epoch / every epoch
+                self._reset(None if initial_states is None else initial_states[resets])
+                resets += 1
+            eager = (env_noise is not None or episodes is not None or not self._use_graph or self._calls == 0)
+            if eager:
+                self._epoch(None if env_noise is None else env_noise[e], None if episodes is None else episodes[e])
+                continue
+            if self._graph is None:
+                torch.cuda.synchronize()
+                g = torch.cuda.CUDAGraph()
+                n0 = L.load().rb200_launch_count()
+                with torch.cuda.graph(g):
+                    self._epoch()
+                self.graph_kernel_count = int(L.load().rb200_launch_count() - n0)
+                self._graph = g
+            self._graph.replay()
+        L.check(L.load().rb200_episode_stats_reduce(L.ptr(self.acc), self.B, L.ptr(self.sums), L.stream_ptr()),
+                "episode_stats_reduce")
+        self._calls += 1
+        return self.sums
