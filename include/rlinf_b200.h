@@ -387,6 +387,46 @@ int rb200_rollout_tc_chunked(const rb200_mlp_layout* L, const float* params, con
                              double gamma, double p_term, double noise_std, double reward_noise_std,
                              rb200_stream_t stream);
 
+/* Training-rollout episode statistics (env/* metrics) inside the persistent rollouts: the same kernels and arguments
+ * as rb200_rollout_tc / rb200_rollout_tc_chunked / rb200_rollout_fused, with the buffers, flags and random streams
+ * unchanged, plus episode_return [B] fp32 (running return, carried across rollouts; the caller zeroes it with every
+ * env reset) and episode_acc [B,4] fp64 (count, sum return, sum length, sum reward; zeroed by the caller per rollout).
+ * Per env step the raw reward (before the truncation bootstrap) is added to the return; at a chunk's last sub-step
+ *   auto_reset:  where the chunk is done, acc += {1, ret, elapsed, ret / (float)elapsed} with the pre-reset elapsed
+ *                count, then ret = 0;
+ *   otherwise:   at the rollout's last chunk step every env records its running episode the same way.
+ * Replaces ManiskillEnv._record_metrics / _reset_metrics / _handle_auto_reset (rlinf/envs/maniskill/maniskill_env.py:
+ * 243-272,377-391) with EnvWorker.env_interact_step's env_info and the should_record rule of
+ * EnvWorker._run_interact_once (rlinf/workers/env/env_worker.py:507-522,1229-1235).  Reduce acc with
+ * rb200_episode_stats_reduce. */
+int rb200_rollout_tc_stats(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
+                           float* states, float* actions, float* logprobs, float* values, float* rewards,
+                           uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
+                           float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
+                           const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
+                           uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps,
+                           int auto_reset, int bootstrap_on_done, double gamma, double p_term, double noise_std,
+                           double reward_noise_std, float* episode_return, double* episode_acc, rb200_stream_t stream);
+int rb200_rollout_tc_chunked_stats(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
+                                   float* states, float* actions, float* logprobs, float* values, float* rewards,
+                                   uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
+                                   float* final_values, int32_t* elapsed, const float* policy_noise,
+                                   const float* env_noise, const uint64_t* counter_policy,
+                                   const uint64_t* counter_env, uint64_t seed_policy, uint64_t seed_env,
+                                   uint64_t offset_policy, int T, int B, int num_action_chunks, int max_episode_steps,
+                                   int auto_reset, int bootstrap_on_done, double gamma, double p_term,
+                                   double noise_std, double reward_noise_std, float* episode_return,
+                                   double* episode_acc, rb200_stream_t stream);
+int rb200_rollout_fused_stats(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
+                              const float* w_a, float* states, float* actions, float* logprobs, float* values,
+                              float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
+                              float* final_obs, float* final_values, int32_t* elapsed, const float* policy_noise,
+                              const float* env_noise, const uint64_t* counter_policy, const uint64_t* counter_env,
+                              uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
+                              int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma,
+                              double p_term, double noise_std, double reward_noise_std, float* episode_return,
+                              double* episode_acc, rb200_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * SURVEY 8(f)3: token log-probabilities and entropies straight from the logits (csrc/logits.cu).
  * Replaces compute_logprobs_from_logits (rlinf/utils/utils.py:454-492, = -cross_entropy) and
@@ -475,6 +515,13 @@ int rb200_episode_stats_step(const float* rewards, const uint8_t* done, int B, i
 /* out[4] = {count, sum return, sum length, sum reward} over the B rows of acc [B,4], summed in a fixed order by one
  * CTA (no atomics): repeated runs give bit-identical results. */
 int rb200_episode_stats_reduce(const double* acc, int B, double* out, rb200_stream_t stream);
+/* Training-rollout episode statistics of one chunk step of the per-kernel loop (run after the env step, before the
+ * truncation bootstrap adds to rewards): the rb200_episode_stats_step update with the training record rule of
+ * rb200_rollout_tc_stats - auto_reset: every env whose chunk is done records and restarts ret / len; otherwise every
+ * env records at the rollout's last chunk step (last_step != 0) and none before.  len [B] int32 is the env's elapsed
+ * count, zeroed with ret at every env reset.  Replaces the same reference lines as rb200_rollout_tc_stats. */
+int rb200_train_episode_stats_step(const float* rewards, const uint8_t* done, int B, int C, int auto_reset,
+                                   int last_step, float* ret, int32_t* len, double* acc, rb200_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * a10 reward filter: replaces the filter_rewards block of EmbodiedFSDPActor._process_received_rollout_batch,

@@ -129,6 +129,12 @@ SIGNATURES = {
     "rb200_rollout_tc_chunked_supported": (c_int, [C.POINTER(MlpLayout), c_int, c_int]),
     "rb200_rollout_tc_chunked": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 6 +
                                  [c_double] * 4 + [c_void_p]),
+    "rb200_rollout_fused_stats": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 19 + [c_uint64] * 3 + [c_int] * 5 +
+                                  [c_double] * 4 + [c_void_p] * 3),
+    "rb200_rollout_tc_stats": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 5 +
+                               [c_double] * 4 + [c_void_p] * 3),
+    "rb200_rollout_tc_chunked_stats": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 +
+                                       [c_int] * 6 + [c_double] * 4 + [c_void_p] * 3),
     "rb200_logits_logprob_entropy_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                                  c_int, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "rb200_logits_logprob_entropy_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
@@ -152,6 +158,7 @@ SIGNATURES = {
     "rb200_mlp_mean": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_int64] + [c_void_p] * 5),
     "rb200_episode_stats_step": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int] + [c_void_p] * 6),
     "rb200_episode_stats_reduce": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "rb200_train_episode_stats_step": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p] * 4),
 }
 
 _LIB: Optional[C.CDLL] = None

@@ -10,6 +10,7 @@
 // fixed-order reduction produces [count, sum return, sum length, sum reward] - no float atomics, so two runs of the
 // same evaluation give bit-identical metrics.
 #include "common.cuh"
+#include "episode_stats.cuh"
 
 namespace rb {
 int mlp_mean_forward(const rb200_mlp_layout* L, const float* params, const float* wsplit, const float* states,
@@ -25,11 +26,17 @@ struct StatsArgs {
   const uint8_t* done;    // [B,C]; column C-1 is the chunk's done flag
   float* ret;             // [B]
   int32_t* len;           // [B]
-  uint8_t* prev_done;     // [B]
+  uint8_t* prev_done;     // [B]; read and written by kNewlyDone only
   double* acc;            // [B,4]: count, sum return, sum length, sum reward
   float* episode;         // [B,3] or null: (return, length, reward) of the episode finished this step, else NaN
   int B, C, auto_reset;
+  int rule;               // which envs record an episode this step (Record)
 };
+
+// Record rules.  Evaluation (EnvWorker.env_evaluate_step): kDone with auto-reset, else kNewlyDone.  Training
+// (EnvWorker._run_interact_once with should_record / env_interact_step): kDone with auto-reset; without it every env
+// records its running episode at the rollout's last chunk step (kAll) and none before (kNone).
+enum Record { kDone = 0, kNewlyDone = 1, kNone = 2, kAll = 3 };
 
 __global__ void __launch_bounds__(256) episode_stats_step_kernel(StatsArgs p) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -39,17 +46,15 @@ __global__ void __launch_bounds__(256) episode_stats_step_kernel(StatsArgs p) {
   // ManiSkill's elapsed_steps keeps counting through a termination inside a chunk
   const int32_t l = p.len[b] + p.C;
   const bool done = p.done[(size_t)b * p.C + p.C - 1] != 0;
-  const bool prev = p.prev_done[b] != 0;
-  const bool newly = p.auto_reset ? done : (done && !prev);
-  p.prev_done[b] = prev || done;
+  bool newly = p.rule == kAll || (p.rule == kDone && done);
+  if (p.rule == kNewlyDone) {
+    const bool prev = p.prev_done[b] != 0;
+    newly = done && !prev;
+    p.prev_done[b] = prev || done;
+  }
   float* ep = p.episode ? p.episode + (size_t)b * 3 : nullptr;
   if (newly) {
-    const float rew = __fdiv_rn(r, (float)l);
-    double* a = p.acc + (size_t)b * 4;
-    a[0] += 1.0;
-    a[1] += (double)r;
-    a[2] += (double)l;
-    a[3] += (double)rew;
+    const float rew = rb::episode_finish(p.acc + (size_t)b * 4, r, l);
     if (ep) {
       ep[0] = r;
       ep[1] = (float)l;
@@ -98,7 +103,20 @@ extern "C" int rb200_episode_stats_step(const float* rewards, const uint8_t* don
   if (B <= 0 || C <= 0) return RB200_E_SHAPE;
   StatsArgs p{};
   p.rewards = rewards; p.done = done; p.ret = ret; p.len = len; p.prev_done = prev_done; p.acc = acc;
-  p.episode = episode; p.B = B; p.C = C; p.auto_reset = auto_reset;
+  p.episode = episode; p.B = B; p.C = C; p.auto_reset = auto_reset; p.rule = auto_reset ? kDone : kNewlyDone;
+  episode_stats_step_kernel<<<(B + 255) / 256, 256, 0, rb::as_stream(stream)>>>(p);
+  rb::count_launch();
+  RB_RETURN_LAUNCH();
+}
+
+extern "C" int rb200_train_episode_stats_step(const float* rewards, const uint8_t* done, int B, int C, int auto_reset,
+                                              int last_step, float* ret, int32_t* len, double* acc,
+                                              rb200_stream_t stream) {
+  if (!rewards || !done || !ret || !len || !acc) return RB200_E_NULL;
+  if (B <= 0 || C <= 0) return RB200_E_SHAPE;
+  StatsArgs p{};
+  p.rewards = rewards; p.done = done; p.ret = ret; p.len = len; p.acc = acc; p.B = B; p.C = C;
+  p.auto_reset = auto_reset; p.rule = auto_reset ? kDone : (last_step ? kAll : kNone);
   episode_stats_step_kernel<<<(B + 255) / 256, 256, 0, rb::as_stream(stream)>>>(p);
   rb::count_launch();
   RB_RETURN_LAUNCH();

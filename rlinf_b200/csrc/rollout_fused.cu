@@ -20,6 +20,7 @@
 #include <curand_kernel.h>
 
 #include "common.cuh"
+#include "episode_stats.cuh"
 #include "tc_gemm.cuh"  // rb::tc::g_debug_flags (experiment switches)
 
 namespace {
@@ -54,6 +55,12 @@ struct FusedArgs {
   int T, B, E, obs, act, vdim;
   int max_episode_steps, auto_reset, bootstrap_on_done;
   float gamma, p_term, noise_std, reward_noise_std;
+};
+
+// episode statistics of the rollout (kStats): running fp32 return [B], carried across rollouts, and fp64 sums [B,4]
+struct EpStats {
+  float* ret;
+  double* acc;
 };
 
 __device__ __forceinline__ float tanh_fast(float x) {  // same formula as the tensor-core epilogue (tc_gemm.cu)
@@ -264,8 +271,12 @@ __device__ __forceinline__ float value_dot(const float* g3_row, const float* s_v
   return rb::warp_sum(s);
 }
 
-template <int EMAX, int PF>
-__global__ void __launch_bounds__(kThreads, 1) rollout_fused_kernel(FusedArgs p) {
+// kStats: the raw reward of every step goes into the running return (before the bootstrap adds gamma * V); an episode
+// is recorded (ManiskillEnv._record_metrics) where the step is done with auto-reset, and for every environment at the
+// last step without it (should_record in EnvWorker._run_interact_once); a recorded episode restarts the return on
+// auto-reset.
+template <int EMAX, int PF, bool kStats>
+__global__ void __launch_bounds__(kThreads, 1) rollout_fused_kernel(FusedArgs p, EpStats es) {
   extern __shared__ __align__(16) float sm[];
   const int obs = p.obs, act = p.act;
   float* x = sm;                        // [EMAX][obs]  current observation
@@ -279,6 +290,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_fused_kernel(FusedArgs p)
   float* rew_s = act_s + EMAX * kMaxAct;               // [EMAX]
   int* el_s = reinterpret_cast<int*>(rew_s + EMAX);    // [EMAX]
   int* flag_s = el_s + EMAX;                           // [EMAX] bootstrap flag of this step
+  float* ret_s = reinterpret_cast<float*>(flag_s + EMAX);  // [EMAX] running return (kStats)
 
   const int j = threadIdx.x, lane = j & 31, warp = j >> 5;
   const int e0 = blockIdx.x * p.E;
@@ -302,6 +314,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_fused_kernel(FusedArgs p)
   if (j < EMAX) {
     el_s[j] = j < nE ? p.elapsed[e0 + j] : 0;
     flag_s[j] = 0;
+    if constexpr (kStats) ret_s[j] = j < nE ? es.ret[e0 + j] : 0.f;
   }
   __syncthreads();
 
@@ -410,6 +423,12 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_fused_kernel(FusedArgs p)
       __syncwarp();
       if (lane == 0) {
         rew_s[e] = -sq / (float)obs + p.reward_noise_std * eps_r;
+        if constexpr (kStats) {
+          const float r = __fadd_rn(ret_s[e], rew_s[e]);
+          const bool rec = p.auto_reset ? done : t == T - 1;
+          if (rec) rb::episode_finish(es.acc + (size_t)row * 4, r, el);
+          ret_s[e] = (rec && p.auto_reset) ? 0.f : r;
+        }
         const size_t o = (size_t)(t + 1) * B + row;
         p.term[o] = term;
         p.trunc[o] = trunc;
@@ -458,6 +477,8 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_fused_kernel(FusedArgs p)
     }
   }
   if (j < nE) p.elapsed[e0 + j] = el_s[j];
+  if constexpr (kStats)
+    if (j < nE) es.ret[e0 + j] = ret_s[j];
 }
 
 __global__ void __launch_bounds__(256) transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int R,
@@ -484,25 +505,25 @@ size_t fused_smem(int obs) {
          sizeof(int) * 2 * EMAX;
 }
 
-template <int EMAX, int PF>
-int launch_fused_pf(const FusedArgs& a, int grid, cudaStream_t st) {
-  const size_t smem = fused_smem<EMAX>(a.obs);
+template <int EMAX, int PF, bool kStats>
+int launch_fused_pf(const FusedArgs& a, const EpStats& es, int grid, cudaStream_t st) {
+  const size_t smem = fused_smem<EMAX>(a.obs) + (kStats ? sizeof(float) * EMAX : 0);
   if (smem > 227 * 1024) return RB200_E_UNSUPPORTED;
-  cudaError_t ce = cudaFuncSetAttribute(rollout_fused_kernel<EMAX, PF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)smem);
+  cudaError_t ce = cudaFuncSetAttribute(rollout_fused_kernel<EMAX, PF, kStats>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (ce != cudaSuccess) return (int)ce;
-  rollout_fused_kernel<EMAX, PF><<<grid, kThreads, smem, st>>>(a);
+  rollout_fused_kernel<EMAX, PF, kStats><<<grid, kThreads, smem, st>>>(a, es);
   rb::count_launch();
   ce = cudaPeekAtLastError();
   return ce == cudaSuccess ? 0 : (int)ce;
 }
 
-template <int EMAX>
-int launch_fused(const FusedArgs& a, int grid, cudaStream_t st) {
+template <int EMAX, bool kStats>
+int launch_fused(const FusedArgs& a, const EpStats& es, int grid, cudaStream_t st) {
   // default: weight rows of the next 4 k-steps in flight (bit-identical buffers, tests/test_gpu_runner.py); debug bit 1
   // selects the one-k-step prefetch
-  if (rb::tc::g_debug_flags & 2) return launch_fused_pf<EMAX, 0>(a, grid, st);
-  return launch_fused_pf<EMAX, 4>(a, grid, st);
+  if (rb::tc::g_debug_flags & 2) return launch_fused_pf<EMAX, 0, kStats>(a, es, grid, st);
+  return launch_fused_pf<EMAX, 4, kStats>(a, es, grid, st);
 }
 
 }  // namespace
@@ -545,17 +566,19 @@ extern "C" int rb200_rollout_fused_prepare(const rb200_mlp_layout* L, const floa
   return ce == cudaSuccess ? 0 : (int)ce;
 }
 
-extern "C" int rb200_rollout_fused(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
-                                   const float* w_a, float* states, float* actions, float* logprobs, float* values,
-                                   float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
-                                   float* final_obs, float* final_values, int32_t* elapsed,
-                                   const float* policy_noise, const float* env_noise, const uint64_t* counter_policy,
-                                   const uint64_t* counter_env, uint64_t seed_policy, uint64_t seed_env,
-                                   uint64_t offset_policy, int T, int B, int max_episode_steps, int auto_reset,
-                                   int bootstrap_on_done, double gamma, double p_term, double noise_std,
-                                   double reward_noise_std, rb200_stream_t stream) {
+namespace {
+template <bool kStats>
+int rollout_fused_impl(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
+                       const float* w_a, float* states, float* actions, float* logprobs, float* values, float* rewards,
+                       uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
+                       float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
+                       const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
+                       uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps, int auto_reset,
+                       int bootstrap_on_done, double gamma, double p_term, double noise_std, double reward_noise_std,
+                       const EpStats& es, rb200_stream_t stream) {
   int e = rb200_rollout_fused_supported(L, B);
   if (e) return e;
+  if (kStats && (!es.ret || !es.acc)) return RB200_E_NULL;
   if (!params || !wt || !w_s || !w_a || !states || !actions || !logprobs || !rewards || !terminations ||
       !truncations || !dones || !final_obs || !elapsed)
     return RB200_E_NULL;
@@ -576,8 +599,42 @@ extern "C" int rb200_rollout_fused(const rb200_mlp_layout* L, const float* param
   a.E = E;
   const int grid = (B + E - 1) / E;
   cudaStream_t st = rb::as_stream(stream);
-  if (E <= 4) return launch_fused<4>(a, grid, st);
-  if (E <= 8) return launch_fused<8>(a, grid, st);
-  if (E <= 16) return launch_fused<16>(a, grid, st);
-  return launch_fused<32>(a, grid, st);
+  if (E <= 4) return launch_fused<4, kStats>(a, es, grid, st);
+  if (E <= 8) return launch_fused<8, kStats>(a, es, grid, st);
+  if (E <= 16) return launch_fused<16, kStats>(a, es, grid, st);
+  return launch_fused<32, kStats>(a, es, grid, st);
+}
+}  // namespace
+
+extern "C" int rb200_rollout_fused(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
+                                   const float* w_a, float* states, float* actions, float* logprobs, float* values,
+                                   float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
+                                   float* final_obs, float* final_values, int32_t* elapsed,
+                                   const float* policy_noise, const float* env_noise, const uint64_t* counter_policy,
+                                   const uint64_t* counter_env, uint64_t seed_policy, uint64_t seed_env,
+                                   uint64_t offset_policy, int T, int B, int max_episode_steps, int auto_reset,
+                                   int bootstrap_on_done, double gamma, double p_term, double noise_std,
+                                   double reward_noise_std, rb200_stream_t stream) {
+  return rollout_fused_impl<false>(L, params, wt, w_s, w_a, states, actions, logprobs, values, rewards, terminations,
+                                   truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
+                                   counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B,
+                                   max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term, noise_std,
+                                   reward_noise_std, EpStats{}, stream);
+}
+
+extern "C" int rb200_rollout_fused_stats(const rb200_mlp_layout* L, const float* params, const float* wt,
+                                         const float* w_s, const float* w_a, float* states, float* actions,
+                                         float* logprobs, float* values, float* rewards, uint8_t* terminations,
+                                         uint8_t* truncations, uint8_t* dones, float* final_obs, float* final_values,
+                                         int32_t* elapsed, const float* policy_noise, const float* env_noise,
+                                         const uint64_t* counter_policy, const uint64_t* counter_env,
+                                         uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
+                                         int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma,
+                                         double p_term, double noise_std, double reward_noise_std,
+                                         float* episode_return, double* episode_acc, rb200_stream_t stream) {
+  return rollout_fused_impl<true>(L, params, wt, w_s, w_a, states, actions, logprobs, values, rewards, terminations,
+                                  truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
+                                  counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B,
+                                  max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term, noise_std,
+                                  reward_noise_std, EpStats{episode_return, episode_acc}, stream);
 }

@@ -12,6 +12,7 @@
 #include <curand_kernel.h>
 
 #include "common.cuh"
+#include "episode_stats.cuh"
 #include "tma.cuh"
 #include "wgmma.cuh"
 
@@ -78,6 +79,29 @@ static_assert(kSmemBytesChunk <= 232448, "rollout_tc chunked shared memory");
 static_assert(kMaxChunks * kH <= kMaxActTc * kH, "chunked value head in Misc::mw");
 __device__ __forceinline__ ChunkSmem* chunk_smem(Misc* ms) {
   return reinterpret_cast<ChunkSmem*>(reinterpret_cast<uint8_t*>(ms) + (kOffChunk - kOffMisc));
+}
+
+// Episode statistics of the training rollout (kStats): the running fp32 return of the CTA's environments (loaded from
+// and stored back to the caller's ret [B], so episodes span rollouts) and the caller's fp64 sums acc [B,4].  They sit
+// behind the C = 1 / chunked maps above, so the kernels without statistics keep their shared-memory layout.
+struct StatsSmem {
+  float ret[kNE];
+  double* acc;
+};
+struct EpStats {
+  float* ret;   // [B]
+  double* acc;  // [B,4]: count, sum return, sum length, sum reward
+};
+template <bool kChunk>
+constexpr int kOffStats = kOffChunk + (kChunk ? (int)sizeof(ChunkSmem) : 0);
+template <bool kChunk, bool kStats>
+constexpr int kSmemTotal =
+    kStats ? kOffStats<kChunk> + (int)sizeof(StatsSmem) + 1024 : (kChunk ? kSmemBytesChunk : kSmemBytes);
+static_assert(kOffStats<true> % 8 == 0 && kOffStats<false> % 8 == 0, "StatsSmem alignment");
+static_assert(kSmemTotal<true, true> <= 232448 && kSmemTotal<false, true> <= 232448, "rollout_tc statistics shared memory");
+template <bool kChunk>
+__device__ __forceinline__ StatsSmem* stats_smem(Misc* ms) {
+  return reinterpret_cast<StatsSmem*>(reinterpret_cast<uint8_t*>(ms) + (kOffStats<kChunk> - kOffMisc));
 }
 
 struct TcArgs {
@@ -215,7 +239,10 @@ __device__ __noinline__ float policy_draw(unsigned long long seed, unsigned long
 // kChunk: t counts env sub-steps, chunk step n = t / C, sub-step c = t % C, with the semantics of
 // env_substep_kernel + chunk_finish_kernel: sub-step c uses action columns [cA, (c+1)A), no reset inside the chunk,
 // flags OR-ed over the chunk and written to column C-1 only, one auto-reset after the last sub-step.
-template <bool kChunk>
+// kStats: the raw reward goes into the running return; an episode is recorded (ManiskillEnv._record_metrics) at the
+// chunk's last sub-step where the chunk is done with auto-reset, and for every environment at the rollout's last chunk
+// step without it (should_record in EnvWorker._run_interact_once); a recorded episode restarts the return on auto-reset.
+template <bool kChunk, bool kStats>
 __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obuf, uint32_t ob_half, const float* zs,
                                             const float* eps_s, int w8, int lane, int t, int e0, int nE, int nk,
                                             uint64_t c_e, bool boot) {
@@ -302,6 +329,13 @@ __device__ __noinline__ void env_finish4(const TcArgs& p, Misc* ms, uint8_t* obu
         p.trunc[o] = (fl >> 1) & 1;
         p.done[o] = (fl >> 2) & 1;
         if (kChunk) cs->orf[e] = bits[i] & 3;
+        if constexpr (kStats) {
+          StatsSmem* ss = stats_smem<kChunk>(ms);
+          const float r = __fadd_rn(ss->ret[e], rw[i]);
+          const bool rec = last && (p.auto_reset ? (bits[i] & 4) != 0 : n == T - 1);
+          if (rec) rb::episode_finish(ss->acc + (size_t)row * 4, r, ms->el[e] + 1);  // el before the reset
+          ss->ret[e] = (rec && p.auto_reset) ? 0.f : r;
+        }
         ms->el[e] = bits[i] >> 4;
         ms->flag[e] = (bits[i] >> 3) & 1;
         ms->rew[e] = rw[i];
@@ -438,8 +472,9 @@ __device__ __noinline__ void tower_layer(Misc* ms, uint32_t ring_a, int slot0, u
 
 // kChunk: num_action_chunks = p.C > 1.  Per chunk step the towers run once; the env warpgroup runs C x.W_s products and
 // the env and actor warpgroups C dynamics finishes, the first one after the value tower has read the observation tile.
-template <bool kChunk>
-__global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p) {
+// kStats: episode statistics of the rollout into es (env_finish4).
+template <bool kChunk, bool kStats>
+__global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p, const EpStats es) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* ring = smem + kOffRing;
@@ -496,6 +531,11 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
     ms->el[tid] = tid < nE ? p.elapsed[e0 + tid] : 0;
     ms->flag[tid] = 0;
     ms->rew[tid] = 0.f;
+  }
+  if constexpr (kStats) {
+    StatsSmem* ss = stats_smem<kChunk>(ms);
+    if (tid < kNE) ss->ret[tid] = tid < nE ? es.ret[e0 + tid] : 0.f;
+    if (tid == 0) ss->acc = es.acc;
   }
   rb::tma::fence_proxy_async();
   __syncthreads();
@@ -623,7 +663,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
       named_sync(4, 256);
       for (int c = 0; c < Cn; ++c) {
         named_sync(4, 256);
-        env_finish4<kChunk>(*pa, ms, obuf, ob_half, reinterpret_cast<const float*>(abuf),
+        env_finish4<kChunk, kStats>(*pa, ms, obuf, ob_half, reinterpret_cast<const float*>(abuf),
                             reinterpret_cast<const float*>(abuf + kAbufHalf), w, lane, t * Cn + c, e0, nE, sg.nkb0, c_e,
                             boot);
         rb::tma::fence_proxy_async();
@@ -763,7 +803,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
         }
       named_sync(4, 256);
       // ---- 4. finish 4 environments per warp (the actor group takes environments 0..15) ----
-      env_finish4<kChunk>(*pa, ms, obuf, ob_half, zs, eps_s, 4 + ew, lane, t, e0, nE, nk, c_e, boot);
+      env_finish4<kChunk, kStats>(*pa, ms, obuf, ob_half, zs, eps_s, 4 + ew, lane, t, e0, nE, nk, c_e, boot);
       rb::tma::fence_proxy_async();
       named_sync(4, 256);
       if (sub == Cn - 1 && gt == 0) {
@@ -775,6 +815,8 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p)
       }
     }
     if (gt < nE) p.elapsed[e0 + gt] = ms->el[gt];  // written by this group, ordered by the last named barrier
+    if constexpr (kStats)
+      if (gt < nE) es.ret[e0 + gt] = stats_smem<kChunk>(ms)->ret[gt];
   }
 }
 
@@ -880,7 +922,7 @@ extern "C" int rb200_rollout_tc_prepare(const rb200_mlp_layout* L, const float* 
 }
 
 namespace {
-template <bool kChunk>
+template <bool kChunk, bool kStats>
 int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
                       float* states, float* actions, float* logprobs, float* values, float* rewards,
                       uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs, float* final_values,
@@ -888,7 +930,8 @@ int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void
                       const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
                       uint64_t seed_env, uint64_t offset_policy, int T, int B, int num_action_chunks,
                       int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma, double p_term,
-                      double noise_std, double reward_noise_std, rb200_stream_t stream) {
+                      double noise_std, double reward_noise_std, const EpStats& es, rb200_stream_t stream) {
+  if (kStats && (!es.ret || !es.acc)) return RB200_E_NULL;
   if (!params || !pack || !w_a || !states || !actions || !logprobs || !values || !rewards || !terminations ||
       !truncations || !dones || !final_obs || !final_values || !elapsed)
     return RB200_E_NULL;
@@ -903,14 +946,15 @@ int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void
   a.act = L->act_dim; a.max_episode_steps = max_episode_steps; a.auto_reset = auto_reset;
   a.bootstrap_on_done = bootstrap_on_done; a.gamma = (float)gamma; a.p_term = (float)p_term;
   a.noise_std = (float)noise_std; a.reward_noise_std = (float)reward_noise_std; a.C = num_action_chunks;
-  const int smem = kChunk ? kSmemBytesChunk : kSmemBytes;
+  const int smem = kSmemTotal<kChunk, kStats>;
   static bool attr_done = false;
   if (!attr_done) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc_kernel<kChunk>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc_kernel<kChunk, kStats>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       smem));
     attr_done = true;
   }
   const int grid = (B + kNE - 1) / kNE;
-  rollout_tc_kernel<kChunk><<<grid, kThreads, smem, rb::as_stream(stream)>>>(a);
+  rollout_tc_kernel<kChunk, kStats><<<grid, kThreads, smem, rb::as_stream(stream)>>>(a, es);
   rb::count_launch();
   RB_RETURN_LAUNCH();
 }
@@ -926,11 +970,11 @@ extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, 
                                 double reward_noise_std, rb200_stream_t stream) {
   int e = rb200_rollout_tc_supported(L, B);
   if (e) return e;
-  return launch_rollout_tc<false>(L, params, pack, w_a, states, actions, logprobs, values, rewards, terminations,
-                                  truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
-                                  counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B, 1,
-                                  max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term, noise_std,
-                                  reward_noise_std, stream);
+  return launch_rollout_tc<false, false>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
+                                         terminations, truncations, dones, final_obs, final_values, elapsed,
+                                         policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
+                                         offset_policy, T, B, 1, max_episode_steps, auto_reset, bootstrap_on_done,
+                                         gamma, p_term, noise_std, reward_noise_std, EpStats{}, stream);
 }
 
 extern "C" int rb200_rollout_tc_chunked(const rb200_mlp_layout* L, const float* params, const void* pack,
@@ -945,9 +989,51 @@ extern "C" int rb200_rollout_tc_chunked(const rb200_mlp_layout* L, const float* 
                                         double reward_noise_std, rb200_stream_t stream) {
   int e = rb200_rollout_tc_chunked_supported(L, num_action_chunks, B);
   if (e) return e;
-  return launch_rollout_tc<true>(L, params, pack, w_a, states, actions, logprobs, values, rewards, terminations,
-                                 truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
-                                 counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B,
-                                 num_action_chunks, max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term,
-                                 noise_std, reward_noise_std, stream);
+  return launch_rollout_tc<true, false>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
+                                        terminations, truncations, dones, final_obs, final_values, elapsed,
+                                        policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
+                                        offset_policy, T, B, num_action_chunks, max_episode_steps, auto_reset,
+                                        bootstrap_on_done, gamma, p_term, noise_std, reward_noise_std, EpStats{},
+                                        stream);
+}
+
+extern "C" int rb200_rollout_tc_stats(const rb200_mlp_layout* L, const float* params, const void* pack,
+                                      const float* w_a, float* states, float* actions, float* logprobs, float* values,
+                                      float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
+                                      float* final_obs, float* final_values, int32_t* elapsed,
+                                      const float* policy_noise, const float* env_noise,
+                                      const uint64_t* counter_policy, const uint64_t* counter_env,
+                                      uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
+                                      int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma,
+                                      double p_term, double noise_std, double reward_noise_std, float* episode_return,
+                                      double* episode_acc, rb200_stream_t stream) {
+  int e = rb200_rollout_tc_supported(L, B);
+  if (e) return e;
+  return launch_rollout_tc<false, true>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
+                                        terminations, truncations, dones, final_obs, final_values, elapsed,
+                                        policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
+                                        offset_policy, T, B, 1, max_episode_steps, auto_reset, bootstrap_on_done,
+                                        gamma, p_term, noise_std, reward_noise_std,
+                                        EpStats{episode_return, episode_acc}, stream);
+}
+
+extern "C" int rb200_rollout_tc_chunked_stats(const rb200_mlp_layout* L, const float* params, const void* pack,
+                                              const float* w_a, float* states, float* actions, float* logprobs,
+                                              float* values, float* rewards, uint8_t* terminations,
+                                              uint8_t* truncations, uint8_t* dones, float* final_obs,
+                                              float* final_values, int32_t* elapsed, const float* policy_noise,
+                                              const float* env_noise, const uint64_t* counter_policy,
+                                              const uint64_t* counter_env, uint64_t seed_policy, uint64_t seed_env,
+                                              uint64_t offset_policy, int T, int B, int num_action_chunks,
+                                              int max_episode_steps, int auto_reset, int bootstrap_on_done,
+                                              double gamma, double p_term, double noise_std, double reward_noise_std,
+                                              float* episode_return, double* episode_acc, rb200_stream_t stream) {
+  int e = rb200_rollout_tc_chunked_supported(L, num_action_chunks, B);
+  if (e) return e;
+  return launch_rollout_tc<true, true>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
+                                       terminations, truncations, dones, final_obs, final_values, elapsed,
+                                       policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
+                                       offset_policy, T, B, num_action_chunks, max_episode_steps, auto_reset,
+                                       bootstrap_on_done, gamma, p_term, noise_std, reward_noise_std,
+                                       EpStats{episode_return, episode_acc}, stream);
 }

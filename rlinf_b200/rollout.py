@@ -16,6 +16,7 @@ Three implementations of the same loop: the persistent tensor-core kernel (`rb20
 the default whenever it supports the problem), the persistent fp32 SIMT kernel (`rb200_rollout_fused`,
 `rollout.fused_kernel: true`) and the per-kernel loop (`rollout.fused_kernel: false`)
 captured once in a CUDA graph (rollout.enable_cuda_graph) and replayed - any env exposing `step_into` works there.
+Each of the three also keeps the episode statistics of the rollout (the reference's `env/*` metrics) on the device.
 """
 from __future__ import annotations
 
@@ -164,13 +165,23 @@ class RolloutBuffer:
 
 
 class RolloutWorker:
-    """One rank's env + policy replica."""
+    """One rank's env + policy replica.
+
+    Episode statistics of the training rollouts (ManiskillEnv._record_metrics / _reset_metrics / _handle_auto_reset
+    with the should_record rule of EnvWorker._run_interact_once, rlinf/envs/maniskill/maniskill_env.py:243-272,377-391,
+    rlinf/workers/env/env_worker.py:507-522,1229-1235): every env step adds its raw reward (before the truncation
+    bootstrap) to a per-env fp32 running return `ep_ret`.  With auto_reset an env whose chunk is done records
+    (return, episode length, return / length) and restarts its return; return and length carry over between rollouts.
+    Without auto_reset every env records its running episode at the rollout's last chunk step.  The records are summed
+    per env into `ep_acc` [B,4] fp64 inside whichever rollout implementation runs, and `episode_sums` [4] fp64 =
+    [count, sum return, sum length, sum reward] is reduced from it in a fixed order after every rollout.
+    `episode_stats=False` selects the rollout entries without statistics (for comparisons)."""
 
     # thresholds of rollout.fused_kernel: auto, carried over from an earlier GPU; not re-measured on the H100
     FUSED_AUTO_MAX_ENVS_PER_CTA = 16
     TC_AUTO_MIN_ENVS = 640
 
-    def __init__(self, cfg, policy, env, buffer: RolloutBuffer):
+    def __init__(self, cfg, policy, env, buffer: RolloutBuffer, episode_stats: bool = True):
         self.cfg, self.policy, self.env, self.buf = cfg, policy, env, buffer
         self.gamma = float(cfg.algorithm.get("gamma", 1))
         self.bootstrap_type = cfg.algorithm.get("bootstrap_type", "standard")
@@ -220,6 +231,22 @@ class RolloutWorker:
             sms = torch.cuda.get_device_properties(policy.device).multi_processor_count
             mode = -(-int(buffer.B) // sms) <= self.FUSED_AUTO_MAX_ENVS_PER_CTA
         self._fused = bool(mode) and supported
+        self.episode_stats = bool(episode_stats)
+        dev = policy.device
+        self.ep_ret = torch.zeros(buffer.B, dtype=torch.float32, device=dev)  # running return, carried across rollouts
+        self.ep_len = torch.zeros(buffer.B, dtype=torch.int32, device=dev)    # elapsed steps (per-kernel loop only)
+        self.ep_acc = torch.zeros(buffer.B, 4, dtype=torch.float64, device=dev)
+        self.episode_sums = torch.zeros(4, dtype=torch.float64, device=dev)
+
+    def _stats_args(self):
+        return (L.ptr(self.ep_ret), L.ptr(self.ep_acc)) if self.episode_stats else ()
+
+    def _stats_step(self, rewards, dones, C, last):
+        """Episode statistics of one chunk step of the per-kernel loop: after the env step, before the bootstrap."""
+        if self.episode_stats:
+            L.check(L.load().rb200_train_episode_stats_step(
+                L.ptr(rewards), L.ptr(dones), self.buf.B, C, int(self.auto_reset), int(last), L.ptr(self.ep_ret),
+                L.ptr(self.ep_len), L.ptr(self.ep_acc), L.stream_ptr()), "train_episode_stats_step")
 
     def _fused_rollout(self, policy_noise=None, env_noise=None):
         """The whole T-step loop in one persistent kernel (csrc/rollout_fused.cu)."""
@@ -229,14 +256,15 @@ class RolloutWorker:
         lay = C.byref(pol.layout)
         wt = pol._buf("rollout_wt", lib.rb200_rollout_fused_wt_floats(lay))
         L.check(lib.rb200_rollout_fused_prepare(lay, L.ptr(pol.flat_params), L.ptr(wt), st), "rollout_fused_prepare")
-        L.check(lib.rb200_rollout_fused(
+        entry = lib.rb200_rollout_fused_stats if self.episode_stats else lib.rb200_rollout_fused
+        L.check(entry(
             lay, L.ptr(pol.flat_params), L.ptr(wt), L.ptr(env.w_s), L.ptr(env.w_a), L.ptr(buf.states),
             L.ptr(buf.actions), L.ptr(buf.prev_logprobs), L.ptr(buf.prev_values) if pol.value_dim > 0 else None,
             L.ptr(buf.rewards), L.ptr(buf.terminations), L.ptr(buf.truncations), L.ptr(buf.dones),
             L.ptr(buf.final_obs), L.ptr(buf.final_values) if pol.value_dim > 0 else None, L.ptr(env.elapsed),
             L.ptr(policy_noise), L.ptr(env_noise), L.ptr(self.counter), L.ptr(env.counter), self.seed, env.seed, 0,
             buf.T, buf.B, env.max_episode_steps, int(self.auto_reset), int(self.bootstrap_type != "standard"),
-            self.gamma, env.p_term, env.noise_std, env.reward_noise_std, st), "rollout_fused")
+            self.gamma, env.p_term, env.noise_std, env.reward_noise_std, *self._stats_args(), st), "rollout_fused")
         L.check(lib.rb200_counter_add(L.ptr(self.counter), buf.T, st), "counter_add")
         L.check(lib.rb200_counter_add(L.ptr(env.counter), buf.T, st), "counter_add")
 
@@ -257,11 +285,13 @@ class RolloutWorker:
                 L.ptr(env.elapsed), L.ptr(policy_noise), L.ptr(env_noise), L.ptr(self.counter), L.ptr(env.counter),
                 self.seed, env.seed, 0, buf.T, buf.B)
         tail = (env.max_episode_steps, int(self.auto_reset), int(self.bootstrap_type != "standard"), self.gamma,
-                env.p_term, env.noise_std, env.reward_noise_std, st)
+                env.p_term, env.noise_std, env.reward_noise_std, *self._stats_args(), st)
         if self.num_action_chunks > 1:
-            L.check(lib.rb200_rollout_tc_chunked(*args, self.num_action_chunks, *tail), "rollout_tc_chunked")
+            entry = lib.rb200_rollout_tc_chunked_stats if self.episode_stats else lib.rb200_rollout_tc_chunked
+            L.check(entry(*args, self.num_action_chunks, *tail), "rollout_tc_chunked")
         else:
-            L.check(lib.rb200_rollout_tc(*args, *tail), "rollout_tc")
+            entry = lib.rb200_rollout_tc_stats if self.episode_stats else lib.rb200_rollout_tc
+            L.check(entry(*args, *tail), "rollout_tc")
         L.check(lib.rb200_counter_add(L.ptr(self.counter), buf.T, st), "counter_add")
         L.check(lib.rb200_counter_add(L.ptr(env.counter), buf.T, st), "counter_add")
 
@@ -298,6 +328,7 @@ class RolloutWorker:
             env.step_into(buf.states[t], buf.actions[t], buf.states[t + 1], buf.final_obs,
                           buf.rewards[t].view(B), buf.terminations[t + 1].view(B), buf.truncations[t + 1].view(B),
                           buf.dones[t + 1].view(B), noise=None if env_noise is None else env_noise[t])
+            self._stats_step(buf.rewards[t], buf.dones[t + 1], 1, t == T - 1)
             # compute_bootstrap_rewards (env_worker.py:719-758): r += gamma * V(final_obs) where truncated/done
             if self.auto_reset and pol.value_dim > 0:
                 flag = buf.truncations[t + 1] if self.bootstrap_type == "standard" else buf.dones[t + 1]
@@ -329,6 +360,7 @@ class RolloutWorker:
             env.chunk_step_into(buf.states[n], buf.actions[n], buf.states[n + 1], buf.final_obs, buf.rewards[n],
                                 buf.terminations[n + 1], buf.truncations[n + 1], buf.dones[n + 1],
                                 noise=None if env_noise is None else env_noise[n])
+            self._stats_step(buf.rewards[n], buf.dones[n + 1], Cn, n == nc - 1)
             if self.auto_reset and pol.value_dim > 0:
                 flag = buf.truncations[n + 1] if self.bootstrap_type == "standard" else buf.dones[n + 1]
                 pol.value(buf.final_obs, out=buf.final_values)
@@ -346,14 +378,23 @@ class RolloutWorker:
             # (elapsed back to 0, fresh initial states); with auto_reset on only once, at the very beginning
             obs, _ = self.env.reset()
             buf.states[0].copy_(obs["states"])
+            self.ep_ret.zero_()  # ManiskillEnv.reset -> _reset_metrics
+            self.ep_len.zero_()
             self.started = True
         else:
             buf.states[0].copy_(buf.states[buf.T])  # last obs of the previous rollout (bootstrap_step)
+        self.ep_acc.zero_()
         # dones row 0 = zeros (env_worker.py:899-945): never written by the loop, stays zero
         if self._tc or self._fused or not self._use_graph or self._calls == 0:
             self._one_rollout()  # first call runs eagerly (also allocates every scratch buffer)
-            self._calls += 1
-            return
+        else:
+            self._replay()
+        self._calls += 1
+        if self.episode_stats:
+            L.check(L.load().rb200_episode_stats_reduce(L.ptr(self.ep_acc), buf.B, L.ptr(self.episode_sums),
+                                                        L.stream_ptr()), "episode_stats_reduce")
+
+    def _replay(self):
         if self._graph is None:
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
@@ -363,7 +404,6 @@ class RolloutWorker:
             self.graph_kernel_count = int(L.load().rb200_launch_count() - n0)
             self._graph = g
         self._graph.replay()
-        self._calls += 1
 
 
 class EvalWorker:

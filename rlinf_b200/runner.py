@@ -49,16 +49,23 @@ def check_eval_config(cfg) -> int:
     return interval
 
 
-def eval_metrics_from_sums(sums) -> dict:
+def eval_metrics_from_sums(sums, prefix: str = "eval") -> dict:
     """compute_evaluate_metrics (rlinf/utils/metric_utils.py:372-419) for an env without `success`, from the reduced
-    [count, sum return, sum length, sum reward]: means over finished episodes and their number; only the count when
-    no episode finished (there is no per-episode entry to average then)."""
+    [count, sum return, sum length, sum reward]: means over recorded episodes and their number; only the count when
+    no episode was recorded (there is no per-episode entry to average then).  Keys are `{prefix}/...`: `eval` for
+    evaluation, `env` for the training rollouts (EmbodiedRunner._log_step_metrics)."""
     count, s_ret, s_len, s_rew = (float(x) for x in sums)
     n = int(count)
     if n == 0:
-        return {"eval/num_trajectories": 0}
-    return {"eval/return": s_ret / n, "eval/episode_len": s_len / n, "eval/reward": s_rew / n,
-            "eval/num_trajectories": n}
+        return {f"{prefix}/num_trajectories": 0}
+    return {f"{prefix}/return": s_ret / n, f"{prefix}/episode_len": s_len / n, f"{prefix}/reward": s_rew / n,
+            f"{prefix}/num_trajectories": n}
+
+
+def records_train_episodes(env_train_cfg) -> bool:
+    """Whether the training rollouts report env/* metrics: always, except with auto_reset off and
+    ignore_terminations on, which the synthetic training env does not implement."""
+    return bool(env_train_cfg.auto_reset) or not env_train_cfg.get("ignore_terminations", False)
 
 
 class EmbodiedRunner:
@@ -92,7 +99,7 @@ class EmbodiedRunner:
         self.env.w_a.copy_(torch.randn(m.action_dim, m.obs_dim, generator=g) / math.sqrt(m.action_dim))
         self.buffer = RolloutBuffer(self.n_chunk_steps, self.B, m.obs_dim, pol.act_dim, max(pol.value_dim, 1),
                                     num_action_chunks=Cn)
-        self.rollout = RolloutWorker(cfg, pol, self.env, self.buffer)
+        self.rollout = RolloutWorker(cfg, pol, self.env, self.buffer, episode_stats=records_train_episodes(et))
         ev = cfg.env.get("eval")
         self.eval_env, self.evaluator = None, None
         if ev is not None:
@@ -133,6 +140,17 @@ class EmbodiedRunner:
             dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self._pg)
         return eval_metrics_from_sums(sums.cpu().tolist())
 
+    def env_metrics(self) -> dict:
+        """env/return, env/episode_len, env/reward, env/num_trajectories of the last training rollout on all ranks
+        (one all-reduce of 4 doubles, one device-to-host copy); {} when the config records no training episodes."""
+        if not self.rollout.episode_stats:
+            return {}
+        sums = self.rollout.episode_sums
+        if self.world_size > 1:
+            sums = sums.clone()
+            dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self._pg)
+        return eval_metrics_from_sums(sums.cpu().tolist(), "env")
+
     def update_rollout_weights(self):
         self.actor.sync_model_to_rollout(self.rollout.policy.flat_params)
 
@@ -152,6 +170,7 @@ class EmbodiedRunner:
             self.update_rollout_weights()
         self.rollout_phase()
         metrics = self.update_phase()
+        metrics.update(self.env_metrics())
         self.global_step += 1
         # _maybe_eval_and_checkpoint (embodied_runner.py:308-329), on the incremented step count
         if should_evaluate(self.global_step, self.max_steps, self.val_check_interval):
