@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define RB200_ABI_VERSION 1
+#define RB200_ABI_VERSION 2
 
 /* error codes (<0); >0 is a cudaError_t */
 #define RB200_OK 0
@@ -322,110 +322,88 @@ int rb200_tc_wgrad_h(const float* Z, const float* H, float* dW, int64_t n, int I
  * (one-k-step weight prefetch). */
 int rb200_debug_set_flags(int flags);
 
-/* Persistent fused rollout (csrc/rollout_fused.cu): the whole T-step loop of one rank - MLP actor/critic inference,
- * Normal sampling, synthetic-env dynamics with auto-reset and the truncation bootstrap of rewards - in ONE kernel;
- * CTA c owns environments [c*E, c*E+E) for all T steps.  Replaces EnvWorker.interact / MultiStepRolloutWorker.generate
- * (rlinf/workers/env/env_worker.py:1059-1349, rlinf/workers/rollout/hf/huggingface_worker.py:678-781) for the
- * MLP-policy + device-resident env case; same buffers, row alignment and random streams as the per-kernel path
- * (rb200_mlp_sample + rb200_synth_env_step + rb200_mlp_value + rb200_bootstrap_rewards per step).
+/* Persistent rollouts: the whole T-step loop of one rank - MLP actor/critic inference, Normal sampling, synthetic-env
+ * dynamics with auto-reset and the truncation bootstrap of rewards - in ONE kernel.  Replaces EnvWorker.interact /
+ * MultiStepRolloutWorker.generate (rlinf/workers/env/env_worker.py:1059-1349,
+ * rlinf/workers/rollout/hf/huggingface_worker.py:678-781) for the MLP-policy + device-resident env case, with the same
+ * buffers, row alignment and random streams as the per-kernel path (rb200_mlp_sample + rb200_synth_env_step or
+ * rb200_synth_env_chunk_step + rb200_mlp_value + rb200_bootstrap_rewards[_ld] per step).  Both kernels take everything
+ * but the weights in one rb200_rollout_args (pointers, then 64-bit, then 32-bit integers, then doubles: no padding). */
+typedef struct rb200_rollout_args {
+  /* buffers; T = chunk steps, C = num_action_chunks, act = act_dim = C*A, obs = obs_dim */
+  float* states;         /* [T+1,B,obs]: row 0 = the current observation (input), rows 1..T written */
+  float* actions;        /* [T,B,act] */
+  float* logprobs;       /* [T,B,act] */
+  float* values;         /* [T+1,B,value_dim]; may be NULL in rb200_rollout_fused when value_dim == 0 */
+  float* rewards;        /* [T,B,C], the truncation bootstrap gamma * V(final_obs) folded in */
+  uint8_t* terminations; /* [T+1,B,C]: rows 1..T written; with C > 1 all-zero except the chunk's last column = any */
+  uint8_t* truncations;  /* [T+1,B,C] */
+  uint8_t* dones;        /* [T+1,B,C] */
+  float* final_obs;      /* [B,obs]: observation before the auto-reset */
+  float* final_values;   /* [B,value_dim]: V(final_obs); may be NULL as `values` */
+  /* synthetic env dynamics, as rb200_synth_env_step */
+  const float* w_s;      /* [obs,obs]; read by rb200_rollout_fused only (the tensor-core pack holds its own copy) */
+  const float* w_a;      /* [A,obs] */
+  int32_t* elapsed;      /* [B] env step counters, in/out */
+  /* random streams: pre-drawn draws (parity mode) or NULL = Philox on the device */
+  const float* policy_noise;      /* [T,B,act] or NULL */
+  const float* env_noise;         /* [T,B,2*obs+2]; C > 1: [T,B,C*(obs+2)+obs] = per sub-step eps[obs] | eps_r | u,
+                                     then the reset state; or NULL */
+  /* device step counters, read once (chunk step t uses counter + t): the caller adds T to both afterwards
+   * (rb200_counter_add) */
+  const uint64_t* counter_policy;
+  const uint64_t* counter_env;
+  /* Training-rollout episode statistics: both NULL = off; exactly one NULL = RB200_E_NULL.  Buffers, flags and random
+   * streams are the same with statistics on and off.  Per env step the raw reward (before the truncation bootstrap)
+   * is added to the return; at a chunk's last sub-step
+   *   auto_reset:  where the chunk is done, acc += {1, ret, elapsed, ret / (float)elapsed} with the pre-reset elapsed
+   *                count, then ret = 0;
+   *   otherwise:   at the rollout's last chunk step every env records its running episode the same way.
+   * Replaces ManiskillEnv._record_metrics / _reset_metrics / _handle_auto_reset (rlinf/envs/maniskill/maniskill_env.py:
+   * 243-272,377-391) with EnvWorker.env_interact_step's env_info and the should_record rule of
+   * EnvWorker._run_interact_once (rlinf/workers/env/env_worker.py:507-522,1229-1235).  Reduce acc with
+   * rb200_episode_stats_reduce. */
+  float* episode_return; /* [B] fp32 running return, carried across rollouts; the caller zeroes it with every env reset */
+  double* episode_acc;   /* [B,4] fp64 count, sum return, sum length, sum reward; zeroed by the caller per rollout */
+  uint64_t seed_policy, seed_env, offset_policy;
+  int32_t T, B;
+  int32_t num_action_chunks; /* C: 1, or 2..8 in the tensor-core kernel */
+  int32_t max_episode_steps, auto_reset;
+  int32_t bootstrap_on_done; /* 1: bootstrap where done ("always"), 0: where truncated ("standard") */
+  double gamma, p_term, noise_std, reward_noise_std;
+} rb200_rollout_args;
+
+/* fp32 SIMT kernel (csrc/rollout_fused.cu): CTA c owns environments [c*E, c*E+E) for all T steps.
  * rb200_rollout_fused_supported() == 0 iff hidden == 256, obs_dim % 4 == 0, obs_dim <= 256, value_dim <= 1 and
- * B <= 32 * #SM.  `wt` (rb200_rollout_fused_wt_floats floats) holds the transposed hidden weights; refresh it with
- * rb200_rollout_fused_prepare() after every parameter update.  states row 0 is the current observation (input);
- * the device counters are read once (step t uses counter + t): add T to both afterwards (rb200_counter_add). */
+ * B <= 32 * #SM; rb200_rollout_fused() also needs num_action_chunks == 1 (else RB200_E_UNSUPPORTED).  `wt`
+ * (rb200_rollout_fused_wt_floats floats) holds the transposed hidden weights; refresh it with
+ * rb200_rollout_fused_prepare() after every parameter update. */
 int64_t rb200_rollout_fused_wt_floats(const rb200_mlp_layout* L);
 int rb200_rollout_fused_supported(const rb200_mlp_layout* L, int B);
 int rb200_rollout_fused_prepare(const rb200_mlp_layout* L, const float* params, float* wt, rb200_stream_t stream);
-int rb200_rollout_fused(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
-                        const float* w_a, float* states, float* actions, float* logprobs, float* values,
-                        float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
-                        float* final_obs, float* final_values, int32_t* elapsed, const float* policy_noise,
-                        const float* env_noise, const uint64_t* counter_policy, const uint64_t* counter_env,
-                        uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
-                        int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma, double p_term,
-                        double noise_std, double reward_noise_std, rb200_stream_t stream);
+int rb200_rollout_fused(const rb200_mlp_layout* L, const float* params, const float* wt, const rb200_rollout_args* a,
+                        rb200_stream_t stream);
 
-/* Persistent TENSOR-CORE rollout (csrc/rollout_tc.cu): same loop, buffers, row alignment and random streams as
- * rb200_rollout_fused, but every hidden layer of both towers and the env's s.W_s product run on wgmma (fp16 in,
- * 2-way fp16 split with fp32 accumulation, computed transposed: D[hidden unit, env] = W . X^T, 32 environments per CTA,
- * activations handed from the accumulator registers to the next layer's operand tile in shared memory); the truncation bootstrap
- * V(final_obs) rides in 32 extra MMA columns of the next step's value tower.  The weights are streamed from a packed,
- * pre-split, pre-swizzled copy (rb200_rollout_tc_pack_bytes bytes, 16-byte aligned) that rb200_rollout_tc_prepare()
- * rebuilds from the flat parameters and the env's w_s [obs,obs] after every parameter update.
- * rb200_rollout_tc_supported() == 0 iff hidden == 256, value_dim == 1, act_dim <= 8, obs_dim % 32 == 0, obs_dim <= 128.
- * Replaces the same reference loop as rb200_rollout_fused (env_worker.py:1059-1349, huggingface_worker.py:678-781). */
-int rb200_rollout_tc_supported(const rb200_mlp_layout* L, int B);
+/* TENSOR-CORE kernel (csrc/rollout_tc.cu): every hidden layer of both towers and the env's s.W_s product run on wgmma
+ * (fp16 in, 2-way fp16 split with fp32 accumulation, computed transposed: D[hidden unit, env] = W . X^T, 32 environments
+ * per CTA, activations handed from the accumulator registers to the next layer's operand tile in shared memory); the
+ * truncation bootstrap V(final_obs) rides in 32 extra MMA columns of the next step's value tower.  The weights are
+ * streamed from a packed, pre-split, pre-swizzled copy (rb200_rollout_tc_pack_bytes bytes, 16-byte aligned) that
+ * rb200_rollout_tc_prepare() rebuilds from the flat parameters and the env's w_s [obs,obs] after every parameter update.
+ * Chunked policies (C = num_action_chunks > 1, act_dim = C*A): per chunk step one actor / value inference on obs_n,
+ * then C synthetic-env sub-steps without reset (sub-step c uses action columns [cA, (c+1)A)), flags OR-ed over the
+ * chunk, one auto-reset after the chunk and the truncation bootstrap on the last column - the semantics and random
+ * streams of rb200_synth_env_chunk_step plus rb200_bootstrap_rewards_ld.
+ * rb200_rollout_tc_supported(L, C, B) == 0 iff hidden == 256, obs_dim % 32 == 0, obs_dim <= 128, B > 0 and
+ *   C == 1:  value_dim == 1, act_dim <= 8;
+ *   C > 1:   2 <= C <= 8, act_dim = C*A with 1 <= A <= 8 and C*A <= 32, value_dim == C.
+ * rb200_rollout_tc() checks it for (a->num_action_chunks, a->B) first. */
+int rb200_rollout_tc_supported(const rb200_mlp_layout* L, int num_action_chunks, int B);
 int64_t rb200_rollout_tc_pack_bytes(const rb200_mlp_layout* L);
 int rb200_rollout_tc_prepare(const rb200_mlp_layout* L, const float* params, const float* w_s, void* pack,
                              rb200_stream_t stream);
-int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
-                     float* states, float* actions, float* logprobs, float* values, float* rewards,
-                     uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
-                     float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
-                     const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
-                     uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps, int auto_reset,
-                     int bootstrap_on_done, double gamma, double p_term, double noise_std, double reward_noise_std,
+int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const rb200_rollout_args* a,
                      rb200_stream_t stream);
-
-/* Chunked variant of the persistent tensor-core rollout (num_action_chunks = C > 1, act_dim = C*A): per chunk step
- * one actor / value inference on obs_n, then C synthetic-env sub-steps without reset (sub-step c uses action columns
- * [cA, (c+1)A)), flags OR-ed over the chunk and written to the chunk's last column, one auto-reset after the chunk and
- * the truncation bootstrap on the last column - the semantics and random streams of rb200_synth_env_chunk_step plus
- * rb200_bootstrap_rewards_ld.  T = chunk steps; buffers: states [T+1,B,obs], actions / logprobs [T,B,C*A],
- * values [T+1,B,C], rewards [T,B,C], terminations / truncations / dones [T+1,B,C], final_values [B,C];
- * policy_noise [T,B,C*A], env_noise [T,B,C*(obs+2)+obs] (per sub-step eps[obs] | eps_r | u, then reset[obs]).
- * The pack comes from rb200_rollout_tc_prepare(), which accepts these layouts too.
- * rb200_rollout_tc_chunked_supported() == 0 iff hidden == 256, obs_dim % 32 == 0, obs_dim <= 128,
- * 2 <= C <= 8, act_dim = C*A with 1 <= A <= 8 and C*A <= 32, value_dim == C. */
-int rb200_rollout_tc_chunked_supported(const rb200_mlp_layout* L, int num_action_chunks, int B);
-int rb200_rollout_tc_chunked(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
-                             float* states, float* actions, float* logprobs, float* values, float* rewards,
-                             uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
-                             float* final_values, int32_t* elapsed, const float* policy_noise,
-                             const float* env_noise, const uint64_t* counter_policy, const uint64_t* counter_env,
-                             uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
-                             int num_action_chunks, int max_episode_steps, int auto_reset, int bootstrap_on_done,
-                             double gamma, double p_term, double noise_std, double reward_noise_std,
-                             rb200_stream_t stream);
-
-/* Training-rollout episode statistics (env/* metrics) inside the persistent rollouts: the same kernels and arguments
- * as rb200_rollout_tc / rb200_rollout_tc_chunked / rb200_rollout_fused, with the buffers, flags and random streams
- * unchanged, plus episode_return [B] fp32 (running return, carried across rollouts; the caller zeroes it with every
- * env reset) and episode_acc [B,4] fp64 (count, sum return, sum length, sum reward; zeroed by the caller per rollout).
- * Per env step the raw reward (before the truncation bootstrap) is added to the return; at a chunk's last sub-step
- *   auto_reset:  where the chunk is done, acc += {1, ret, elapsed, ret / (float)elapsed} with the pre-reset elapsed
- *                count, then ret = 0;
- *   otherwise:   at the rollout's last chunk step every env records its running episode the same way.
- * Replaces ManiskillEnv._record_metrics / _reset_metrics / _handle_auto_reset (rlinf/envs/maniskill/maniskill_env.py:
- * 243-272,377-391) with EnvWorker.env_interact_step's env_info and the should_record rule of
- * EnvWorker._run_interact_once (rlinf/workers/env/env_worker.py:507-522,1229-1235).  Reduce acc with
- * rb200_episode_stats_reduce. */
-int rb200_rollout_tc_stats(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
-                           float* states, float* actions, float* logprobs, float* values, float* rewards,
-                           uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
-                           float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
-                           const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
-                           uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps,
-                           int auto_reset, int bootstrap_on_done, double gamma, double p_term, double noise_std,
-                           double reward_noise_std, float* episode_return, double* episode_acc, rb200_stream_t stream);
-int rb200_rollout_tc_chunked_stats(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
-                                   float* states, float* actions, float* logprobs, float* values, float* rewards,
-                                   uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
-                                   float* final_values, int32_t* elapsed, const float* policy_noise,
-                                   const float* env_noise, const uint64_t* counter_policy,
-                                   const uint64_t* counter_env, uint64_t seed_policy, uint64_t seed_env,
-                                   uint64_t offset_policy, int T, int B, int num_action_chunks, int max_episode_steps,
-                                   int auto_reset, int bootstrap_on_done, double gamma, double p_term,
-                                   double noise_std, double reward_noise_std, float* episode_return,
-                                   double* episode_acc, rb200_stream_t stream);
-int rb200_rollout_fused_stats(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
-                              const float* w_a, float* states, float* actions, float* logprobs, float* values,
-                              float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
-                              float* final_obs, float* final_values, int32_t* elapsed, const float* policy_noise,
-                              const float* env_noise, const uint64_t* counter_policy, const uint64_t* counter_env,
-                              uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
-                              int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma,
-                              double p_term, double noise_std, double reward_noise_std, float* episode_return,
-                              double* episode_acc, rb200_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY 8(f)3: token log-probabilities and entropies straight from the logits (csrc/logits.cu).
@@ -516,10 +494,10 @@ int rb200_episode_stats_step(const float* rewards, const uint8_t* done, int B, i
  * CTA (no atomics): repeated runs give bit-identical results. */
 int rb200_episode_stats_reduce(const double* acc, int B, double* out, rb200_stream_t stream);
 /* Training-rollout episode statistics of one chunk step of the per-kernel loop (run after the env step, before the
- * truncation bootstrap adds to rewards): the rb200_episode_stats_step update with the training record rule of
- * rb200_rollout_tc_stats - auto_reset: every env whose chunk is done records and restarts ret / len; otherwise every
- * env records at the rollout's last chunk step (last_step != 0) and none before.  len [B] int32 is the env's elapsed
- * count, zeroed with ret at every env reset.  Replaces the same reference lines as rb200_rollout_tc_stats. */
+ * truncation bootstrap adds to rewards): the rb200_episode_stats_step update with the training record rule of the
+ * persistent rollouts (rb200_rollout_args.episode_return) - auto_reset: every env whose chunk is done records and
+ * restarts ret / len; otherwise every env records at the rollout's last chunk step (last_step != 0) and none before.
+ * len [B] int32 is the env's elapsed count, zeroed with ret at every env reset.  Replaces the same reference lines. */
 int rb200_train_episode_stats_step(const float* rewards, const uint8_t* done, int B, int C, int auto_reset,
                                    int last_step, float* ret, int32_t* len, double* acc, rb200_stream_t stream);
 

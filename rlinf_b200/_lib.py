@@ -61,6 +61,18 @@ class DppoArgs(C.Structure):
                 ("has_behave_weight_threshold", C.c_int32), ("behave_weight_threshold", c_double)]
 
 
+class RolloutArgs(C.Structure):
+    _fields_ = [(n, c_void_p) for n in (
+        "states", "actions", "logprobs", "values", "rewards", "terminations", "truncations", "dones", "final_obs",
+        "final_values", "w_s", "w_a", "elapsed", "policy_noise", "env_noise", "counter_policy", "counter_env",
+        "episode_return", "episode_acc")] + [
+        ("seed_policy", c_uint64), ("seed_env", c_uint64), ("offset_policy", c_uint64),
+        ("T", C.c_int32), ("B", C.c_int32), ("num_action_chunks", C.c_int32), ("max_episode_steps", C.c_int32),
+        ("auto_reset", C.c_int32), ("bootstrap_on_done", C.c_int32),
+        ("gamma", c_double), ("p_term", c_double), ("noise_std", c_double), ("reward_noise_std", c_double),
+    ]
+
+
 DM_KEYS = {
     0: "actor/policy_loss", 1: "actor/proximal_ratio", 2: "actor/clipped_proximal_ratio", 3: "actor/clip_fraction",
     4: "actor/dual_clip_fraction", 5: "actor/behav_clip_fraction", 6: "actor/proximal_approx_kl",
@@ -119,22 +131,11 @@ SIGNATURES = {
     "rb200_rollout_fused_wt_floats": (c_int64, [C.POINTER(MlpLayout)]),
     "rb200_rollout_fused_supported": (c_int, [C.POINTER(MlpLayout), c_int]),
     "rb200_rollout_fused_prepare": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p]),
-    "rb200_rollout_fused": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 19 + [c_uint64] * 3 + [c_int] * 5 +
-                            [c_double] * 4 + [c_void_p]),
-    "rb200_rollout_tc_supported": (c_int, [C.POINTER(MlpLayout), c_int]),
+    "rb200_rollout_fused": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, C.POINTER(RolloutArgs), c_void_p]),
+    "rb200_rollout_tc_supported": (c_int, [C.POINTER(MlpLayout), c_int, c_int]),
     "rb200_rollout_tc_pack_bytes": (c_int64, [C.POINTER(MlpLayout)]),
     "rb200_rollout_tc_prepare": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_void_p]),
-    "rb200_rollout_tc": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 5 +
-                         [c_double] * 4 + [c_void_p]),
-    "rb200_rollout_tc_chunked_supported": (c_int, [C.POINTER(MlpLayout), c_int, c_int]),
-    "rb200_rollout_tc_chunked": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 6 +
-                                 [c_double] * 4 + [c_void_p]),
-    "rb200_rollout_fused_stats": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 19 + [c_uint64] * 3 + [c_int] * 5 +
-                                  [c_double] * 4 + [c_void_p] * 3),
-    "rb200_rollout_tc_stats": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 + [c_int] * 5 +
-                               [c_double] * 4 + [c_void_p] * 3),
-    "rb200_rollout_tc_chunked_stats": (c_int, [C.POINTER(MlpLayout)] + [c_void_p] * 18 + [c_uint64] * 3 +
-                                       [c_int] * 6 + [c_double] * 4 + [c_void_p] * 3),
+    "rb200_rollout_tc": (c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, C.POINTER(RolloutArgs), c_void_p]),
     "rb200_logits_logprob_entropy_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                                  c_int, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "rb200_logits_logprob_entropy_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,

@@ -568,36 +568,29 @@ extern "C" int rb200_rollout_fused_prepare(const rb200_mlp_layout* L, const floa
 
 namespace {
 template <bool kStats>
-int rollout_fused_impl(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
-                       const float* w_a, float* states, float* actions, float* logprobs, float* values, float* rewards,
-                       uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
-                       float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
-                       const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
-                       uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps, int auto_reset,
-                       int bootstrap_on_done, double gamma, double p_term, double noise_std, double reward_noise_std,
-                       const EpStats& es, rb200_stream_t stream) {
-  int e = rb200_rollout_fused_supported(L, B);
-  if (e) return e;
-  if (kStats && (!es.ret || !es.acc)) return RB200_E_NULL;
-  if (!params || !wt || !w_s || !w_a || !states || !actions || !logprobs || !rewards || !terminations ||
-      !truncations || !dones || !final_obs || !elapsed)
+int rollout_fused_impl(const rb200_mlp_layout* L, const float* params, const float* wt, const rb200_rollout_args& r,
+                       rb200_stream_t stream) {
+  if (!params || !wt || !r.w_s || !r.w_a || !r.states || !r.actions || !r.logprobs || !r.rewards || !r.terminations ||
+      !r.truncations || !r.dones || !r.final_obs || !r.elapsed)
     return RB200_E_NULL;
-  if (L->value_dim > 0 && (!values || !final_values)) return RB200_E_NULL;
-  if (T <= 0) return RB200_E_SHAPE;
+  if (L->value_dim > 0 && (!r.values || !r.final_values)) return RB200_E_NULL;
+  if (r.T <= 0) return RB200_E_SHAPE;
   FusedArgs a{};
-  a.L = *L; a.params = params; a.wt = wt; a.w_s = w_s; a.w_a = w_a; a.states = states; a.actions = actions;
-  a.logp = logprobs; a.values = values; a.rewards = rewards; a.term = terminations; a.trunc = truncations;
-  a.done = dones; a.final_obs = final_obs; a.final_values = final_values; a.elapsed = elapsed;
-  a.policy_noise = policy_noise; a.env_noise = env_noise; a.counter_p = counter_policy; a.counter_e = counter_env;
-  a.seed_p = seed_policy; a.seed_e = seed_env; a.offset_p = offset_policy; a.T = T; a.B = B; a.obs = L->obs_dim;
-  a.act = L->act_dim; a.vdim = L->value_dim; a.max_episode_steps = max_episode_steps; a.auto_reset = auto_reset;
-  a.bootstrap_on_done = bootstrap_on_done; a.gamma = (float)gamma; a.p_term = (float)p_term;
-  a.noise_std = (float)noise_std; a.reward_noise_std = (float)reward_noise_std;
+  a.L = *L; a.params = params; a.wt = wt; a.w_s = r.w_s; a.w_a = r.w_a; a.states = r.states; a.actions = r.actions;
+  a.logp = r.logprobs; a.values = r.values; a.rewards = r.rewards; a.term = r.terminations; a.trunc = r.truncations;
+  a.done = r.dones; a.final_obs = r.final_obs; a.final_values = r.final_values; a.elapsed = r.elapsed;
+  a.policy_noise = r.policy_noise; a.env_noise = r.env_noise; a.counter_p = r.counter_policy;
+  a.counter_e = r.counter_env; a.seed_p = r.seed_policy; a.seed_e = r.seed_env; a.offset_p = r.offset_policy;
+  a.T = r.T; a.B = r.B; a.obs = L->obs_dim; a.act = L->act_dim; a.vdim = L->value_dim;
+  a.max_episode_steps = r.max_episode_steps; a.auto_reset = r.auto_reset; a.bootstrap_on_done = r.bootstrap_on_done;
+  a.gamma = (float)r.gamma; a.p_term = (float)r.p_term; a.noise_std = (float)r.noise_std;
+  a.reward_noise_std = (float)r.reward_noise_std;
+  const EpStats es{r.episode_return, r.episode_acc};
   const int sms = rb::sm_count();
-  int E = (B + sms - 1) / sms;
+  int E = (r.B + sms - 1) / sms;
   if (E < 1) E = 1;
   a.E = E;
-  const int grid = (B + E - 1) / E;
+  const int grid = (r.B + E - 1) / E;
   cudaStream_t st = rb::as_stream(stream);
   if (E <= 4) return launch_fused<4, kStats>(a, es, grid, st);
   if (E <= 8) return launch_fused<8, kStats>(a, es, grid, st);
@@ -606,35 +599,13 @@ int rollout_fused_impl(const rb200_mlp_layout* L, const float* params, const flo
 }
 }  // namespace
 
-extern "C" int rb200_rollout_fused(const rb200_mlp_layout* L, const float* params, const float* wt, const float* w_s,
-                                   const float* w_a, float* states, float* actions, float* logprobs, float* values,
-                                   float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
-                                   float* final_obs, float* final_values, int32_t* elapsed,
-                                   const float* policy_noise, const float* env_noise, const uint64_t* counter_policy,
-                                   const uint64_t* counter_env, uint64_t seed_policy, uint64_t seed_env,
-                                   uint64_t offset_policy, int T, int B, int max_episode_steps, int auto_reset,
-                                   int bootstrap_on_done, double gamma, double p_term, double noise_std,
-                                   double reward_noise_std, rb200_stream_t stream) {
-  return rollout_fused_impl<false>(L, params, wt, w_s, w_a, states, actions, logprobs, values, rewards, terminations,
-                                   truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
-                                   counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B,
-                                   max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term, noise_std,
-                                   reward_noise_std, EpStats{}, stream);
-}
-
-extern "C" int rb200_rollout_fused_stats(const rb200_mlp_layout* L, const float* params, const float* wt,
-                                         const float* w_s, const float* w_a, float* states, float* actions,
-                                         float* logprobs, float* values, float* rewards, uint8_t* terminations,
-                                         uint8_t* truncations, uint8_t* dones, float* final_obs, float* final_values,
-                                         int32_t* elapsed, const float* policy_noise, const float* env_noise,
-                                         const uint64_t* counter_policy, const uint64_t* counter_env,
-                                         uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
-                                         int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma,
-                                         double p_term, double noise_std, double reward_noise_std,
-                                         float* episode_return, double* episode_acc, rb200_stream_t stream) {
-  return rollout_fused_impl<true>(L, params, wt, w_s, w_a, states, actions, logprobs, values, rewards, terminations,
-                                  truncations, dones, final_obs, final_values, elapsed, policy_noise, env_noise,
-                                  counter_policy, counter_env, seed_policy, seed_env, offset_policy, T, B,
-                                  max_episode_steps, auto_reset, bootstrap_on_done, gamma, p_term, noise_std,
-                                  reward_noise_std, EpStats{episode_return, episode_acc}, stream);
+extern "C" int rb200_rollout_fused(const rb200_mlp_layout* L, const float* params, const float* wt,
+                                   const rb200_rollout_args* a, rb200_stream_t stream) {
+  if (!a) return RB200_E_NULL;
+  int e = rb200_rollout_fused_supported(L, a->B);
+  if (e) return e;
+  if (a->num_action_chunks != 1) return RB200_E_UNSUPPORTED;
+  if (!a->episode_return != !a->episode_acc) return RB200_E_NULL;
+  if (!a->episode_return) return rollout_fused_impl<false>(L, params, wt, *a, stream);
+  return rollout_fused_impl<true>(L, params, wt, *a, stream);
 }

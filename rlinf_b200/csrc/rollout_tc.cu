@@ -874,31 +874,25 @@ __global__ void __launch_bounds__(256) pack_kernel(PackArgs a) {
 
 }  // namespace
 
-extern "C" int rb200_rollout_tc_supported(const rb200_mlp_layout* L, int B) {
-  if (!L) return RB200_E_NULL;
-  if (L->hidden != kH || L->act_dim <= 0 || L->act_dim > kMaxActTc || L->value_dim != 1) return RB200_E_UNSUPPORTED;
-  if (L->obs_dim < 32 || L->obs_dim > kMaxObsTc || (L->obs_dim % 32) != 0) return RB200_E_UNSUPPORTED;
-  if (B <= 0) return RB200_E_UNSUPPORTED;
-  return RB200_OK;
-}
-
-extern "C" int rb200_rollout_tc_chunked_supported(const rb200_mlp_layout* L, int num_action_chunks, int B) {
+extern "C" int rb200_rollout_tc_supported(const rb200_mlp_layout* L, int num_action_chunks, int B) {
   if (!L) return RB200_E_NULL;
   const int Cn = num_action_chunks;
-  if (L->hidden != kH || Cn < 2 || Cn > kMaxChunks || L->value_dim != Cn) return RB200_E_UNSUPPORTED;
-  if (L->act_dim <= 0 || L->act_dim > kMaxActChunk || L->act_dim % Cn != 0 || L->act_dim / Cn > kMaxActTc)
-    return RB200_E_UNSUPPORTED;
+  if (L->hidden != kH) return RB200_E_UNSUPPORTED;
+  if (Cn == 1) {
+    if (L->act_dim <= 0 || L->act_dim > kMaxActTc || L->value_dim != 1) return RB200_E_UNSUPPORTED;
+  } else {
+    if (Cn < 2 || Cn > kMaxChunks || L->value_dim != Cn) return RB200_E_UNSUPPORTED;
+    if (L->act_dim <= 0 || L->act_dim > kMaxActChunk || L->act_dim % Cn != 0 || L->act_dim / Cn > kMaxActTc)
+      return RB200_E_UNSUPPORTED;
+  }
   if (L->obs_dim < 32 || L->obs_dim > kMaxObsTc || (L->obs_dim % 32) != 0) return RB200_E_UNSUPPORTED;
   if (B <= 0) return RB200_E_UNSUPPORTED;
   return RB200_OK;
 }
 
 namespace {
-// the pack holds the hidden layers and W_s only: any layout one of the two kernels runs
-int pack_supported(const rb200_mlp_layout* L) {
-  if (rb200_rollout_tc_supported(L, 1) == RB200_OK) return RB200_OK;
-  return rb200_rollout_tc_chunked_supported(L, L->value_dim, 1);
-}
+// the pack holds the hidden layers and W_s only: any layout one of the kernels runs (value_dim == C in both)
+int pack_supported(const rb200_mlp_layout* L) { return rb200_rollout_tc_supported(L, L->value_dim, 1); }
 }  // namespace
 
 extern "C" int64_t rb200_rollout_tc_pack_bytes(const rb200_mlp_layout* L) {
@@ -923,29 +917,23 @@ extern "C" int rb200_rollout_tc_prepare(const rb200_mlp_layout* L, const float* 
 
 namespace {
 template <bool kChunk, bool kStats>
-int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
-                      float* states, float* actions, float* logprobs, float* values, float* rewards,
-                      uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs, float* final_values,
-                      int32_t* elapsed, const float* policy_noise, const float* env_noise,
-                      const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
-                      uint64_t seed_env, uint64_t offset_policy, int T, int B, int num_action_chunks,
-                      int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma, double p_term,
-                      double noise_std, double reward_noise_std, const EpStats& es, rb200_stream_t stream) {
-  if (kStats && (!es.ret || !es.acc)) return RB200_E_NULL;
-  if (!params || !pack || !w_a || !states || !actions || !logprobs || !values || !rewards || !terminations ||
-      !truncations || !dones || !final_obs || !final_values || !elapsed)
+int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const rb200_rollout_args& r,
+                      rb200_stream_t stream) {
+  if (!params || !pack || !r.w_a || !r.states || !r.actions || !r.logprobs || !r.values || !r.rewards ||
+      !r.terminations || !r.truncations || !r.dones || !r.final_obs || !r.final_values || !r.elapsed)
     return RB200_E_NULL;
-  if (T <= 0) return RB200_E_SHAPE;
+  if (r.T <= 0) return RB200_E_SHAPE;
   if (reinterpret_cast<uintptr_t>(pack) & 15) return RB200_E_ALIGN;
   TcArgs a{};
-  a.L = *L; a.params = params; a.pack = static_cast<const uint8_t*>(pack); a.w_a = w_a; a.states = states;
-  a.actions = actions; a.logp = logprobs; a.values = values; a.rewards = rewards; a.term = terminations;
-  a.trunc = truncations; a.done = dones; a.final_obs = final_obs; a.final_values = final_values; a.elapsed = elapsed;
-  a.policy_noise = policy_noise; a.env_noise = env_noise; a.counter_p = counter_policy; a.counter_e = counter_env;
-  a.seed_p = seed_policy; a.seed_e = seed_env; a.offset_p = offset_policy; a.T = T; a.B = B; a.obs = L->obs_dim;
-  a.act = L->act_dim; a.max_episode_steps = max_episode_steps; a.auto_reset = auto_reset;
-  a.bootstrap_on_done = bootstrap_on_done; a.gamma = (float)gamma; a.p_term = (float)p_term;
-  a.noise_std = (float)noise_std; a.reward_noise_std = (float)reward_noise_std; a.C = num_action_chunks;
+  a.L = *L; a.params = params; a.pack = static_cast<const uint8_t*>(pack); a.w_a = r.w_a; a.states = r.states;
+  a.actions = r.actions; a.logp = r.logprobs; a.values = r.values; a.rewards = r.rewards; a.term = r.terminations;
+  a.trunc = r.truncations; a.done = r.dones; a.final_obs = r.final_obs; a.final_values = r.final_values;
+  a.elapsed = r.elapsed; a.policy_noise = r.policy_noise; a.env_noise = r.env_noise; a.counter_p = r.counter_policy;
+  a.counter_e = r.counter_env; a.seed_p = r.seed_policy; a.seed_e = r.seed_env; a.offset_p = r.offset_policy;
+  a.T = r.T; a.B = r.B; a.obs = L->obs_dim; a.act = L->act_dim; a.max_episode_steps = r.max_episode_steps;
+  a.auto_reset = r.auto_reset; a.bootstrap_on_done = r.bootstrap_on_done; a.gamma = (float)r.gamma;
+  a.p_term = (float)r.p_term; a.noise_std = (float)r.noise_std; a.reward_noise_std = (float)r.reward_noise_std;
+  a.C = r.num_action_chunks;
   const int smem = kSmemTotal<kChunk, kStats>;
   static bool attr_done = false;
   if (!attr_done) {
@@ -953,87 +941,23 @@ int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void
                                        smem));
     attr_done = true;
   }
-  const int grid = (B + kNE - 1) / kNE;
-  rollout_tc_kernel<kChunk, kStats><<<grid, kThreads, smem, rb::as_stream(stream)>>>(a, es);
+  const int grid = (r.B + kNE - 1) / kNE;
+  rollout_tc_kernel<kChunk, kStats><<<grid, kThreads, smem, rb::as_stream(stream)>>>(
+      a, EpStats{r.episode_return, r.episode_acc});
   rb::count_launch();
   RB_RETURN_LAUNCH();
 }
 }  // namespace
 
-extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack, const float* w_a,
-                                float* states, float* actions, float* logprobs, float* values, float* rewards,
-                                uint8_t* terminations, uint8_t* truncations, uint8_t* dones, float* final_obs,
-                                float* final_values, int32_t* elapsed, const float* policy_noise, const float* env_noise,
-                                const uint64_t* counter_policy, const uint64_t* counter_env, uint64_t seed_policy,
-                                uint64_t seed_env, uint64_t offset_policy, int T, int B, int max_episode_steps,
-                                int auto_reset, int bootstrap_on_done, double gamma, double p_term, double noise_std,
-                                double reward_noise_std, rb200_stream_t stream) {
-  int e = rb200_rollout_tc_supported(L, B);
+extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack,
+                                const rb200_rollout_args* a, rb200_stream_t stream) {
+  if (!a) return RB200_E_NULL;
+  int e = rb200_rollout_tc_supported(L, a->num_action_chunks, a->B);
   if (e) return e;
-  return launch_rollout_tc<false, false>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
-                                         terminations, truncations, dones, final_obs, final_values, elapsed,
-                                         policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
-                                         offset_policy, T, B, 1, max_episode_steps, auto_reset, bootstrap_on_done,
-                                         gamma, p_term, noise_std, reward_noise_std, EpStats{}, stream);
-}
-
-extern "C" int rb200_rollout_tc_chunked(const rb200_mlp_layout* L, const float* params, const void* pack,
-                                        const float* w_a, float* states, float* actions, float* logprobs, float* values,
-                                        float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
-                                        float* final_obs, float* final_values, int32_t* elapsed,
-                                        const float* policy_noise, const float* env_noise,
-                                        const uint64_t* counter_policy, const uint64_t* counter_env,
-                                        uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
-                                        int num_action_chunks, int max_episode_steps, int auto_reset,
-                                        int bootstrap_on_done, double gamma, double p_term, double noise_std,
-                                        double reward_noise_std, rb200_stream_t stream) {
-  int e = rb200_rollout_tc_chunked_supported(L, num_action_chunks, B);
-  if (e) return e;
-  return launch_rollout_tc<true, false>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
-                                        terminations, truncations, dones, final_obs, final_values, elapsed,
-                                        policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
-                                        offset_policy, T, B, num_action_chunks, max_episode_steps, auto_reset,
-                                        bootstrap_on_done, gamma, p_term, noise_std, reward_noise_std, EpStats{},
-                                        stream);
-}
-
-extern "C" int rb200_rollout_tc_stats(const rb200_mlp_layout* L, const float* params, const void* pack,
-                                      const float* w_a, float* states, float* actions, float* logprobs, float* values,
-                                      float* rewards, uint8_t* terminations, uint8_t* truncations, uint8_t* dones,
-                                      float* final_obs, float* final_values, int32_t* elapsed,
-                                      const float* policy_noise, const float* env_noise,
-                                      const uint64_t* counter_policy, const uint64_t* counter_env,
-                                      uint64_t seed_policy, uint64_t seed_env, uint64_t offset_policy, int T, int B,
-                                      int max_episode_steps, int auto_reset, int bootstrap_on_done, double gamma,
-                                      double p_term, double noise_std, double reward_noise_std, float* episode_return,
-                                      double* episode_acc, rb200_stream_t stream) {
-  int e = rb200_rollout_tc_supported(L, B);
-  if (e) return e;
-  return launch_rollout_tc<false, true>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
-                                        terminations, truncations, dones, final_obs, final_values, elapsed,
-                                        policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
-                                        offset_policy, T, B, 1, max_episode_steps, auto_reset, bootstrap_on_done,
-                                        gamma, p_term, noise_std, reward_noise_std,
-                                        EpStats{episode_return, episode_acc}, stream);
-}
-
-extern "C" int rb200_rollout_tc_chunked_stats(const rb200_mlp_layout* L, const float* params, const void* pack,
-                                              const float* w_a, float* states, float* actions, float* logprobs,
-                                              float* values, float* rewards, uint8_t* terminations,
-                                              uint8_t* truncations, uint8_t* dones, float* final_obs,
-                                              float* final_values, int32_t* elapsed, const float* policy_noise,
-                                              const float* env_noise, const uint64_t* counter_policy,
-                                              const uint64_t* counter_env, uint64_t seed_policy, uint64_t seed_env,
-                                              uint64_t offset_policy, int T, int B, int num_action_chunks,
-                                              int max_episode_steps, int auto_reset, int bootstrap_on_done,
-                                              double gamma, double p_term, double noise_std, double reward_noise_std,
-                                              float* episode_return, double* episode_acc, rb200_stream_t stream) {
-  int e = rb200_rollout_tc_chunked_supported(L, num_action_chunks, B);
-  if (e) return e;
-  return launch_rollout_tc<true, true>(L, params, pack, w_a, states, actions, logprobs, values, rewards,
-                                       terminations, truncations, dones, final_obs, final_values, elapsed,
-                                       policy_noise, env_noise, counter_policy, counter_env, seed_policy, seed_env,
-                                       offset_policy, T, B, num_action_chunks, max_episode_steps, auto_reset,
-                                       bootstrap_on_done, gamma, p_term, noise_std, reward_noise_std,
-                                       EpStats{episode_return, episode_acc}, stream);
+  if (!a->episode_return != !a->episode_acc) return RB200_E_NULL;
+  const bool chunk = a->num_action_chunks > 1, stats = a->episode_return != nullptr;
+  if (!chunk && !stats) return launch_rollout_tc<false, false>(L, params, pack, *a, stream);
+  if (chunk && !stats) return launch_rollout_tc<true, false>(L, params, pack, *a, stream);
+  if (!chunk) return launch_rollout_tc<false, true>(L, params, pack, *a, stream);
+  return launch_rollout_tc<true, true>(L, params, pack, *a, stream);
 }

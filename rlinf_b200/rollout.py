@@ -164,6 +164,51 @@ class RolloutBuffer:
             self.terminations, self.truncations))
 
 
+# thresholds of rollout.fused_kernel: auto, carried over from an earlier GPU; not re-measured on the H100
+FUSED_AUTO_MAX_ENVS_PER_CTA = 16
+TC_AUTO_MIN_ENVS = 640
+
+
+def select_rollout_impl(fused_kernel, num_action_chunks: int, B: int, sm_count: int, tc_supported: bool,
+                        simt_supported: bool) -> str:
+    """The rollout implementation for rollout.fused_kernel = "auto" | "tc" | True / "simt" | False: "tc" (persistent
+    tensor-core kernel), "simt" (persistent fp32 SIMT kernel) or "graph" (per-kernel loop).  tc_supported /
+    simt_supported: the env dynamics are on the device and rb200_rollout_tc_supported / rb200_rollout_fused_supported
+    accept the problem."""
+    Cn = num_action_chunks
+    if Cn > 1 and fused_kernel in ("simt", True):
+        raise ValueError("the persistent fp32 SIMT rollout kernel implements num_action_chunks == 1; chunked "
+                         "policies use the tensor-core kernel (rollout.fused_kernel: tc / auto) or the per-kernel "
+                         "loop (rollout.fused_kernel: false)")
+    if fused_kernel == "tc" and not tc_supported:
+        if Cn > 1:
+            raise ValueError("rollout.fused_kernel='tc' with num_action_chunks > 1 needs hidden 256, obs_dim % 32 "
+                             "== 0, obs_dim <= 128, 2 <= num_action_chunks <= 8, 1 <= action_dim <= 8, "
+                             "num_action_chunks * action_dim <= 32 and one value per sub-step "
+                             "(rb200_rollout_tc_supported)")
+        raise ValueError("rollout.fused_kernel='tc' needs hidden 256, a value head, act_dim <= 8, obs_dim % 32 "
+                         "== 0 and obs_dim <= 128 (rb200_rollout_tc_supported)")
+    if tc_supported and (fused_kernel == "tc" or (fused_kernel == "auto" and Cn == 1 and B >= TC_AUTO_MIN_ENVS)):
+        return "tc"
+    # chunked: `auto` keeps the per-kernel loop, measured faster than the kernel at 256-4096 environments on an
+    # H100 80GB HBM3 at 700 W (DESIGN.md §6)
+    if Cn > 1 or not simt_supported:
+        return "graph"
+    if fused_kernel == "auto":
+        return "simt" if -(-B // sm_count) <= FUSED_AUTO_MAX_ENVS_PER_CTA else "graph"
+    return "simt" if fused_kernel else "graph"
+
+
+def _capture_graph(fn):
+    """(CUDA graph of fn(), kernels this library launched while capturing it = kernels replayed per replay)."""
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    n0 = L.load().rb200_launch_count()
+    with torch.cuda.graph(g):
+        fn()
+    return g, int(L.load().rb200_launch_count() - n0)
+
+
 class RolloutWorker:
     """One rank's env + policy replica.
 
@@ -175,11 +220,8 @@ class RolloutWorker:
     Without auto_reset every env records its running episode at the rollout's last chunk step.  The records are summed
     per env into `ep_acc` [B,4] fp64 inside whichever rollout implementation runs, and `episode_sums` [4] fp64 =
     [count, sum return, sum length, sum reward] is reduced from it in a fixed order after every rollout.
-    `episode_stats=False` selects the rollout entries without statistics (for comparisons)."""
-
-    # thresholds of rollout.fused_kernel: auto, carried over from an earlier GPU; not re-measured on the H100
-    FUSED_AUTO_MAX_ENVS_PER_CTA = 16
-    TC_AUTO_MIN_ENVS = 640
+    `episode_stats=False` runs the rollouts without statistics (for comparisons).
+    `impl` is the implementation every rollout runs (select_rollout_impl)."""
 
     def __init__(self, cfg, policy, env, buffer: RolloutBuffer, episode_stats: bool = True):
         self.cfg, self.policy, self.env, self.buf = cfg, policy, env, buffer
@@ -196,41 +238,14 @@ class RolloutWorker:
         # V(final_obs) of step t (bootstrap of truncated episodes) only feeds rewards[t]: it runs on a side stream,
         # concurrently with the policy inference of step t+1 (both are 32-CTA GEMM chains on a 132-SM device)
         self._side = torch.cuda.Stream(device=policy.device) if policy.device.type == "cuda" else None
-        # persistent fused kernel: needs the synthetic env's dynamics (w_s, w_a) and a supported MLP shape
-        # "auto" | "tc" (tensor-core persistent kernel) | True / "simt" (fp32 SIMT persistent kernel) | False (per-kernel graph)
-        mode = cfg.rollout.get("fused_kernel", "auto")
+        # the persistent kernels need the synthetic env's dynamics (w_s, w_a) on the device and a supported MLP shape
         self.num_action_chunks = Cn = int(getattr(buffer, "num_action_chunks", 1))
-        if Cn > 1 and mode in ("simt", True):
-            raise ValueError("the persistent fp32 SIMT rollout kernel implements num_action_chunks == 1; chunked "
-                             "policies use the tensor-core kernel (rollout.fused_kernel: tc / auto) or the per-kernel "
-                             "loop (rollout.fused_kernel: false)")
+        B, lay = int(buffer.B), C.byref(policy.layout)
         on_dev_env = policy.device.type == "cuda" and hasattr(env, "w_s") and hasattr(env, "w_a")
-        supported = (on_dev_env and Cn == 1
-                     and L.load().rb200_rollout_fused_supported(C.byref(policy.layout), int(buffer.B)) == 0)
-        if Cn > 1:
-            tc_ok = (on_dev_env and L.load().rb200_rollout_tc_chunked_supported(C.byref(policy.layout), Cn,
-                                                                               int(buffer.B)) == 0)
-            if mode == "tc" and not tc_ok:
-                raise ValueError("rollout.fused_kernel='tc' with num_action_chunks > 1 needs hidden 256, obs_dim % 32 "
-                                 "== 0, obs_dim <= 128, 2 <= num_action_chunks <= 8, 1 <= action_dim <= 8, "
-                                 "num_action_chunks * action_dim <= 32 and one value per sub-step "
-                                 "(rb200_rollout_tc_chunked_supported)")
-        else:
-            tc_ok = (on_dev_env and L.load().rb200_rollout_tc_supported(C.byref(policy.layout), int(buffer.B)) == 0)
-            if mode == "tc" and not tc_ok:
-                raise ValueError("rollout.fused_kernel='tc' needs hidden 256, a value head, act_dim <= 8, obs_dim % 32 "
-                                 "== 0 and obs_dim <= 128 (rb200_rollout_tc_supported)")
-        # chunked: `auto` keeps the per-kernel loop, measured faster than the kernel at 256-4096 environments on an
-        # H100 80GB HBM3 at 700 W (DESIGN.md §6)
-        self._tc = tc_ok and (mode == "tc" or (mode == "auto" and Cn == 1 and int(buffer.B) >= self.TC_AUTO_MIN_ENVS))
-        if mode == "simt":
-            mode = True
-        if self._tc or Cn > 1:  # chunked policies below the threshold: the per-kernel loop
-            mode = False
-        if mode == "auto":
-            sms = torch.cuda.get_device_properties(policy.device).multi_processor_count
-            mode = -(-int(buffer.B) // sms) <= self.FUSED_AUTO_MAX_ENVS_PER_CTA
-        self._fused = bool(mode) and supported
+        tc_ok = on_dev_env and L.load().rb200_rollout_tc_supported(lay, Cn, B) == 0
+        simt_ok = on_dev_env and Cn == 1 and L.load().rb200_rollout_fused_supported(lay, B) == 0
+        sms = torch.cuda.get_device_properties(policy.device).multi_processor_count if on_dev_env else 0
+        self.impl = select_rollout_impl(cfg.rollout.get("fused_kernel", "auto"), Cn, B, sms, tc_ok, simt_ok)
         self.episode_stats = bool(episode_stats)
         dev = policy.device
         self.ep_ret = torch.zeros(buffer.B, dtype=torch.float32, device=dev)  # running return, carried across rollouts
@@ -238,8 +253,15 @@ class RolloutWorker:
         self.ep_acc = torch.zeros(buffer.B, 4, dtype=torch.float64, device=dev)
         self.episode_sums = torch.zeros(4, dtype=torch.float64, device=dev)
 
-    def _stats_args(self):
-        return (L.ptr(self.ep_ret), L.ptr(self.ep_acc)) if self.episode_stats else ()
+    @property
+    def _tc(self) -> bool:
+        """The persistent tensor-core kernel runs the rollouts."""
+        return self.impl == "tc"
+
+    @property
+    def _fused(self) -> bool:
+        """The persistent fp32 SIMT kernel runs the rollouts."""
+        return self.impl == "simt"
 
     def _stats_step(self, rewards, dones, C, last):
         """Episode statistics of one chunk step of the per-kernel loop: after the env step, before the bootstrap."""
@@ -248,65 +270,47 @@ class RolloutWorker:
                 L.ptr(rewards), L.ptr(dones), self.buf.B, C, int(self.auto_reset), int(last), L.ptr(self.ep_ret),
                 L.ptr(self.ep_len), L.ptr(self.ep_acc), L.stream_ptr()), "train_episode_stats_step")
 
-    def _fused_rollout(self, policy_noise=None, env_noise=None):
-        """The whole T-step loop in one persistent kernel (csrc/rollout_fused.cu)."""
+    def _kernel_rollout(self, policy_noise, env_noise):
+        """The whole T-step loop in one persistent kernel: tensor-core (csrc/rollout_tc.cu; T = chunk steps when
+        num_action_chunks > 1) or fp32 SIMT (csrc/rollout_fused.cu)."""
         lib = L.load()
         buf, pol, env = self.buf, self.policy, self.env
         st = L.stream_ptr()
         lay = C.byref(pol.layout)
-        wt = pol._buf("rollout_wt", lib.rb200_rollout_fused_wt_floats(lay))
-        L.check(lib.rb200_rollout_fused_prepare(lay, L.ptr(pol.flat_params), L.ptr(wt), st), "rollout_fused_prepare")
-        entry = lib.rb200_rollout_fused_stats if self.episode_stats else lib.rb200_rollout_fused
-        L.check(entry(
-            lay, L.ptr(pol.flat_params), L.ptr(wt), L.ptr(env.w_s), L.ptr(env.w_a), L.ptr(buf.states),
-            L.ptr(buf.actions), L.ptr(buf.prev_logprobs), L.ptr(buf.prev_values) if pol.value_dim > 0 else None,
-            L.ptr(buf.rewards), L.ptr(buf.terminations), L.ptr(buf.truncations), L.ptr(buf.dones),
-            L.ptr(buf.final_obs), L.ptr(buf.final_values) if pol.value_dim > 0 else None, L.ptr(env.elapsed),
-            L.ptr(policy_noise), L.ptr(env_noise), L.ptr(self.counter), L.ptr(env.counter), self.seed, env.seed, 0,
-            buf.T, buf.B, env.max_episode_steps, int(self.auto_reset), int(self.bootstrap_type != "standard"),
-            self.gamma, env.p_term, env.noise_std, env.reward_noise_std, *self._stats_args(), st), "rollout_fused")
-        L.check(lib.rb200_counter_add(L.ptr(self.counter), buf.T, st), "counter_add")
-        L.check(lib.rb200_counter_add(L.ptr(env.counter), buf.T, st), "counter_add")
-
-    def _tc_rollout(self, policy_noise=None, env_noise=None):
-        """The whole T-step loop in one persistent tensor-core kernel (csrc/rollout_tc.cu); T = chunk steps when
-        num_action_chunks > 1."""
-        lib = L.load()
-        buf, pol, env = self.buf, self.policy, self.env
-        st = L.stream_ptr()
-        lay = C.byref(pol.layout)
-        nbytes = int(lib.rb200_rollout_tc_pack_bytes(lay))
-        pack = pol._buf("rollout_tc_pack", (nbytes + 3) // 4)
-        L.check(lib.rb200_rollout_tc_prepare(lay, L.ptr(pol.flat_params), L.ptr(env.w_s), L.ptr(pack), st),
-                "rollout_tc_prepare")
-        args = (lay, L.ptr(pol.flat_params), L.ptr(pack), L.ptr(env.w_a), L.ptr(buf.states), L.ptr(buf.actions),
-                L.ptr(buf.prev_logprobs), L.ptr(buf.prev_values), L.ptr(buf.rewards), L.ptr(buf.terminations),
-                L.ptr(buf.truncations), L.ptr(buf.dones), L.ptr(buf.final_obs), L.ptr(buf.final_values),
-                L.ptr(env.elapsed), L.ptr(policy_noise), L.ptr(env_noise), L.ptr(self.counter), L.ptr(env.counter),
-                self.seed, env.seed, 0, buf.T, buf.B)
-        tail = (env.max_episode_steps, int(self.auto_reset), int(self.bootstrap_type != "standard"), self.gamma,
-                env.p_term, env.noise_std, env.reward_noise_std, *self._stats_args(), st)
-        if self.num_action_chunks > 1:
-            entry = lib.rb200_rollout_tc_chunked_stats if self.episode_stats else lib.rb200_rollout_tc_chunked
-            L.check(entry(*args, self.num_action_chunks, *tail), "rollout_tc_chunked")
+        if self.impl == "tc":
+            nbytes = int(lib.rb200_rollout_tc_pack_bytes(lay))
+            weights = pol._buf("rollout_tc_pack", (nbytes + 3) // 4)
+            L.check(lib.rb200_rollout_tc_prepare(lay, L.ptr(pol.flat_params), L.ptr(env.w_s), L.ptr(weights), st),
+                    "rollout_tc_prepare")
+            entry, what = lib.rb200_rollout_tc, "rollout_tc"
         else:
-            entry = lib.rb200_rollout_tc_stats if self.episode_stats else lib.rb200_rollout_tc
-            L.check(entry(*args, *tail), "rollout_tc")
+            weights = pol._buf("rollout_wt", lib.rb200_rollout_fused_wt_floats(lay))
+            L.check(lib.rb200_rollout_fused_prepare(lay, L.ptr(pol.flat_params), L.ptr(weights), st),
+                    "rollout_fused_prepare")
+            entry, what = lib.rb200_rollout_fused, "rollout_fused"
+        has_v, stats = pol.value_dim > 0, self.episode_stats
+        a = L.RolloutArgs(
+            states=L.ptr(buf.states), actions=L.ptr(buf.actions), logprobs=L.ptr(buf.prev_logprobs),
+            values=L.ptr(buf.prev_values) if has_v else None, rewards=L.ptr(buf.rewards),
+            terminations=L.ptr(buf.terminations), truncations=L.ptr(buf.truncations), dones=L.ptr(buf.dones),
+            final_obs=L.ptr(buf.final_obs), final_values=L.ptr(buf.final_values) if has_v else None,
+            w_s=L.ptr(env.w_s), w_a=L.ptr(env.w_a), elapsed=L.ptr(env.elapsed), policy_noise=L.ptr(policy_noise),
+            env_noise=L.ptr(env_noise), counter_policy=L.ptr(self.counter), counter_env=L.ptr(env.counter),
+            episode_return=L.ptr(self.ep_ret) if stats else None, episode_acc=L.ptr(self.ep_acc) if stats else None,
+            seed_policy=self.seed, seed_env=env.seed, offset_policy=0, T=buf.T, B=buf.B,
+            num_action_chunks=self.num_action_chunks, max_episode_steps=env.max_episode_steps,
+            auto_reset=int(self.auto_reset), bootstrap_on_done=int(self.bootstrap_type != "standard"), gamma=self.gamma,
+            p_term=env.p_term, noise_std=env.noise_std, reward_noise_std=env.reward_noise_std)
+        L.check(entry(lay, L.ptr(pol.flat_params), L.ptr(weights), C.byref(a), st), what)
         L.check(lib.rb200_counter_add(L.ptr(self.counter), buf.T, st), "counter_add")
         L.check(lib.rb200_counter_add(L.ptr(env.counter), buf.T, st), "counter_add")
 
     def _one_rollout(self, policy_noise=None, env_noise=None):
         """policy_noise [T,B,act] / env_noise [T,B,2*obs+2]: pre-drawn N(0,1)/U(0,1) draws (parity tests);
         None -> Philox on the device."""
-        if self._tc:
-            return self._tc_rollout(None if policy_noise is None else policy_noise.contiguous(),
-                                    None if env_noise is None else env_noise.contiguous())
-        if self._fused:
-            if policy_noise is not None:
-                policy_noise = policy_noise.contiguous()
-            if env_noise is not None:
-                env_noise = env_noise.contiguous()
-            return self._fused_rollout(policy_noise, env_noise)
+        if self.impl != "graph":
+            return self._kernel_rollout(None if policy_noise is None else policy_noise.contiguous(),
+                                        None if env_noise is None else env_noise.contiguous())
         lib = L.load()
         buf, pol, env = self.buf, self.policy, self.env
         T, B = buf.T, buf.B
@@ -385,7 +389,7 @@ class RolloutWorker:
             buf.states[0].copy_(buf.states[buf.T])  # last obs of the previous rollout (bootstrap_step)
         self.ep_acc.zero_()
         # dones row 0 = zeros (env_worker.py:899-945): never written by the loop, stays zero
-        if self._tc or self._fused or not self._use_graph or self._calls == 0:
+        if self.impl != "graph" or not self._use_graph or self._calls == 0:
             self._one_rollout()  # first call runs eagerly (also allocates every scratch buffer)
         else:
             self._replay()
@@ -396,13 +400,7 @@ class RolloutWorker:
 
     def _replay(self):
         if self._graph is None:
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            n0 = L.load().rb200_launch_count()
-            with torch.cuda.graph(g):
-                self._one_rollout()
-            self.graph_kernel_count = int(L.load().rb200_launch_count() - n0)
-            self._graph = g
+            self._graph, self.graph_kernel_count = _capture_graph(self._one_rollout)
         self._graph.replay()
 
 
@@ -492,13 +490,7 @@ class EvalWorker:
                 self._epoch(None if env_noise is None else env_noise[e], None if episodes is None else episodes[e])
                 continue
             if self._graph is None:
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                n0 = L.load().rb200_launch_count()
-                with torch.cuda.graph(g):
-                    self._epoch()
-                self.graph_kernel_count = int(L.load().rb200_launch_count() - n0)
-                self._graph = g
+                self._graph, self.graph_kernel_count = _capture_graph(self._epoch)
             self._graph.replay()
         L.check(L.load().rb200_episode_stats_reduce(L.ptr(self.acc), self.B, L.ptr(self.sums), L.stream_ptr()),
                 "episode_stats_reduce")

@@ -1,4 +1,4 @@
-"""The persistent tensor-core rollout kernel with num_action_chunks = C > 1 (rb200_rollout_tc_chunked): env.chunk_step
+"""The persistent tensor-core rollout kernel with num_action_chunks = C > 1 (rb200_rollout_tc, C > 1): env.chunk_step
 semantics (maniskill_env.py:327-375 - C sub-steps without reset, flags OR-ed over the chunk on its last column, one
 auto-reset per chunk) and the bootstrap on the chunk's last sub-step (env_worker.py:719-758), against the oracle with
 injected noise, against the per-kernel chunked loop on the device Philox streams, the `auto` selection, and a full
@@ -170,7 +170,7 @@ def test_rollout_tc_chunked_full_iteration():
     torch.testing.assert_close(b["rewards"], expect, rtol=1e-4, atol=2e-5)
 
 
-def test_rollout_tc_chunked_envelope():
+def test_rollout_tc_supported_envelope():
     from rlinf_b200 import _lib as L
 
     lib = L.load()
@@ -179,8 +179,10 @@ def test_rollout_tc_chunked_envelope():
         lay = L.MlpLayout()
         L.check(lib.rb200_mlp_layout_init(C.byref(lay), obs, A * Cn, Cn if value_dim is None else value_dim, 256),
                 "mlp_layout_init")
-        return lib.rb200_rollout_tc_chunked_supported(C.byref(lay), Cn, 1024) == 0
+        return lib.rb200_rollout_tc_supported(C.byref(lay), Cn, 1024) == 0
 
     assert ok(128, 8, 4) and ok(32, 4, 8)
     assert not ok(40, 4, 2) and not ok(160, 4, 2) and not ok(128, 9, 2)
-    assert not ok(128, 4, 4, value_dim=1) and not ok(128, 4, 1)
+    assert not ok(128, 4, 4, value_dim=1) and not ok(32, 2, 9, value_dim=8)
+    # C = 1: the unchunked kernel's envelope
+    assert ok(128, 4, 1) and not ok(128, 9, 1) and not ok(128, 4, 1, value_dim=0)
