@@ -344,6 +344,26 @@ class EmbodiedActor:
             return lr_list
         return self.optimizer.lr_list()
 
+    # ---- checkpoint ------------------------------------------------------------------------------
+    def state_dict(self) -> dict:
+        """Learner state besides the parameters: the optimiser, its step count, the critic warm-up steps still to go
+        and the LR schedule's position (`last_epoch` of the schedule in force, which is the one rebuilt at the end of
+        critic warm-up if that happened) with the multiplier in use.  Gradients are not part of it: they are zero
+        between run_training calls.  The shuffle permutations are rebuilt from the seed."""
+        return {"optimizer": self.optimizer.state_dict(), "optimizer_steps": int(self.optimizer_steps),
+                "critic_warmup_steps": int(self.critic_warmup_steps),
+                "lr_last_epoch": int(self.lr_schedule.last_epoch), "lr_scale": float(self.optimizer.lr_scale)}
+
+    def load_state_dict(self, sd: dict) -> None:
+        """In place (captured optimiser-step graphs keep their pointers); load the parameters first."""
+        self.optimizer.load_state_dict(sd["optimizer"])
+        self.optimizer_steps = int(sd["optimizer_steps"])
+        self.critic_warmup_steps = int(sd["critic_warmup_steps"])
+        self._set_frozen_groups()
+        self.lr_schedule.last_epoch = int(sd["lr_last_epoch"])  # a rebuilt schedule differs only in its position
+        self.optimizer.lr_scale = float(sd["lr_scale"])
+        self.model.mark_params_changed()
+
     def optimizer_step(self):
         """all-reduce(SUM) of the flat gradient buffer over the data-parallel ranks, then one fused
         norm / clip / AdamW pass that also applies the 1/world_size average."""

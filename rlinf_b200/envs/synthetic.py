@@ -41,6 +41,19 @@ class SyntheticVectorEnv:
         self.elapsed.zero_()
         return {"states": self.state}, {}
 
+    def state_dict(self) -> dict:
+        """What the env carries between steps: the state written by the last reset, the elapsed step counts, the
+        device random-stream counter and the reset generator.  The dynamics (w_s, w_a) come from the config."""
+        return {"state": self.state, "elapsed": self.elapsed, "counter": self.counter,
+                "reset_generator": self._reset_gen.get_state()}
+
+    def load_state_dict(self, sd: dict) -> None:
+        """In place: captured rollout graphs keep pointing at these tensors."""
+        self.state.copy_(sd["state"])
+        self.elapsed.copy_(sd["elapsed"])
+        self.counter.copy_(sd["counter"])
+        self._reset_gen.set_state(sd["reset_generator"])
+
     def step_into(self, state, action, next_state, final_obs, reward, term, trunc, done, noise=None):
         """One env step written straight into caller-provided (rollout-buffer) rows."""
         lib = L.load()

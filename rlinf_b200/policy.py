@@ -91,8 +91,18 @@ class MLPPolicy:
             self._wsplit_fresh = True
         return L.ptr(self.wsplit)
 
-    def load_state_dict(self, sd: dict):
+    def load_state_dict(self, sd: dict, strict: bool = False):
+        """Copy a `{name: tensor}` dict into the flat buffer in place.  `strict`: the keys and shapes must be exactly
+        this policy's (torch's load_state_dict(strict=True)); otherwise extra keys are ignored and a tensor only needs
+        the right number of elements."""
         views = dict(self.named_parameters())
+        if strict:
+            unexpected = [k for k in sd if k not in views]
+            shapes = [f"{k}: {tuple(sd[k].shape)} vs {tuple(v.shape)}" for k, v in views.items()
+                      if k in sd and tuple(sd[k].shape) != tuple(v.shape)]
+            if unexpected or shapes:
+                raise ValueError(f"state dict does not match the policy: unexpected keys {unexpected}, "
+                                 f"shape mismatches {shapes}")
         missing = [k for k in views if k not in sd]
         if missing:
             raise KeyError(f"missing parameters: {missing}")
@@ -299,6 +309,19 @@ class FlatAdamW:
                                          float(grad_scale), L.ptr(self.grad_sq), L.ptr(self.state), st), "adamw_step")
         self._last_grad_scale = float(grad_scale)
         p.mark_params_changed()
+
+    def state_dict(self) -> dict:
+        """Both moments, the device state [step, last norm, last coef, skipped] and the gradient scale of the last step
+        (the rebuild at the end of critic warm-up reads it).  Device tensors, not copies."""
+        return {"exp_avg": self.exp_avg, "exp_avg_sq": self.exp_avg_sq, "state": self.state,
+                "last_grad_scale": float(getattr(self, "_last_grad_scale", 1.0))}
+
+    def load_state_dict(self, sd: dict):
+        """In place: captured optimiser graphs keep pointing at these tensors."""
+        self.exp_avg.copy_(sd["exp_avg"])
+        self.exp_avg_sq.copy_(sd["exp_avg_sq"])
+        self.state.copy_(sd["state"])
+        self._last_grad_scale = float(sd["last_grad_scale"])
 
     def reset_state(self, carry_grads: bool = False):
         """Fresh moments and step count: the reference REBUILDS its optimiser when critic warm-up ends

@@ -263,6 +263,21 @@ class RolloutWorker:
         """The persistent fp32 SIMT kernel runs the rollouts."""
         return self.impl == "simt"
 
+    def state_dict(self) -> dict:
+        """What carries from one rollout to the next: the policy-sampling counter, whether the envs were reset, the
+        last observation (row T, the next rollout's row 0 with auto_reset) and the running episode return / length.
+        Device tensors, not copies; the env saves its own state."""
+        return {"counter": self.counter, "started": bool(self.started), "last_obs": self.buf.states[self.buf.T],
+                "ep_ret": self.ep_ret, "ep_len": self.ep_len}
+
+    def load_state_dict(self, sd: dict) -> None:
+        """In place: a captured rollout graph keeps pointing at these tensors."""
+        self.counter.copy_(sd["counter"])
+        self.started = bool(sd["started"])
+        self.buf.states[self.buf.T].copy_(sd["last_obs"])
+        self.ep_ret.copy_(sd["ep_ret"])
+        self.ep_len.copy_(sd["ep_len"])
+
     def _stats_step(self, rewards, dones, C, last):
         """Episode statistics of one chunk step of the per-kernel loop: after the env step, before the bootstrap."""
         if self.episode_stats:

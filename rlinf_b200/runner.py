@@ -13,6 +13,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib as L
+from . import checkpoint as ckpt
 from .actor import EmbodiedActor
 from .config import wrap
 from .envs import SyntheticVectorEnv
@@ -49,6 +50,28 @@ def check_eval_config(cfg) -> int:
     return interval
 
 
+def should_save(step: int, max_steps: int, val_check_interval: int, save_interval: int) -> bool:
+    """The save half of check_progress (rlinf/utils/runner_utils.py:31-61): save when save_interval > 0 and either step
+    is a positive multiple of it or step == max_steps (the last step).  With evaluation on, save_interval must be
+    negative or a multiple of val_check_interval (ValueError otherwise, the reference's assertion)."""
+    if val_check_interval > 0 and not (save_interval < 0 or save_interval % val_check_interval == 0):
+        raise ValueError(f"runner.save_interval={save_interval} must be divisible by "
+                         f"runner.val_check_interval={val_check_interval}")
+    if save_interval <= 0:
+        return False
+    return (step != 0 and step % save_interval == 0) or step == max_steps
+
+
+def check_save_config(cfg, val_check_interval: int) -> int:
+    """runner.save_interval (0 / absent / negative = no checkpoints); saving needs runner.logger.log_path and
+    runner.logger.experiment_name.  Returns the interval."""
+    interval = int(cfg.runner.get("save_interval", 0) or 0)
+    should_save(0, 0, val_check_interval, interval)  # the interval check only
+    if interval > 0:
+        ckpt.checkpoint_dir(cfg.runner, 0)
+    return interval
+
+
 def eval_metrics_from_sums(sums, prefix: str = "eval") -> dict:
     """compute_evaluate_metrics (rlinf/utils/metric_utils.py:372-419) for an env without `success`, from the reduced
     [count, sum return, sum length, sum reward]: means over recorded episodes and their number; only the count when
@@ -72,6 +95,7 @@ class EmbodiedRunner:
     def __init__(self, cfg, rank=None, world_size=None, process_group=None):
         self.cfg = cfg = wrap(cfg)
         self.val_check_interval = check_eval_config(cfg)
+        self.save_interval = check_save_config(cfg, self.val_check_interval)
         self.max_steps = max_steps(cfg.runner)
         self._dist = dist.is_available() and dist.is_initialized()
         self.rank = rank if rank is not None else (dist.get_rank() if self._dist else 0)
@@ -106,9 +130,13 @@ class EmbodiedRunner:
             self.eval_env = self._build_eval_env(ev, et, m)
             self.evaluator = EvalWorker(cfg, pol, self.eval_env, Cn)
         self.global_step = 0
+        if cfg.runner.get("ckpt_path"):  # policy weights only (embodied_fsdp_actor_worker.py:122-124)
+            pol.load_state_dict(ckpt.load_weights(cfg.runner.ckpt_path), strict=True)
         if self.world_size > 1:  # same initial weights everywhere (rank 0's)
             dist.broadcast(pol.flat_params, src=0, group=process_group)
         self._pg = process_group
+        if cfg.runner.get("resume_dir"):  # the end of init_workers (embodied_runner.py:175-185)
+            self.load_checkpoint(cfg.runner.resume_dir)
 
     def _build_eval_env(self, ev, et, m):
         """The eval env set (cfg.env.eval): same task as the train env (its W_s / W_a), own state, step counter and
@@ -175,10 +203,65 @@ class EmbodiedRunner:
         # _maybe_eval_and_checkpoint (embodied_runner.py:308-329), on the incremented step count
         if should_evaluate(self.global_step, self.max_steps, self.val_check_interval):
             metrics.update(self.evaluate())
+        if should_save(self.global_step, self.max_steps, self.val_check_interval, self.save_interval):
+            self.save_checkpoint()
         return metrics
 
     def run(self, max_epochs=None):
+        """`max_epochs` iterations; by default the iterations left until runner.max_epochs, so a resumed run stops
+        where an uninterrupted one would."""
         out = []
-        for _ in range(max_epochs or self.cfg.runner.max_epochs):
+        for _ in range(max_epochs or max(0, int(self.cfg.runner.max_epochs) - self.global_step)):
             out.append(self.run_iteration())
         return out
+
+    # ---- checkpoint --------------------------------------------------------------------------------
+    def fingerprint(self) -> dict:
+        """The shapes and the sharding a checkpoint must agree with (checkpoint.FINGERPRINT_FIELDS)."""
+        et, ev, pol = self.cfg.env.train, self.cfg.env.get("eval"), self.actor.model
+        return {"obs_dim": pol.obs_dim, "action_dim": pol.action_dim, "num_action_chunks": pol.num_action_chunks,
+                "value_dim": pol.value_dim, "world_size": self.world_size, "total_num_envs": int(et.total_num_envs),
+                "max_steps_per_rollout_epoch": int(self.T), "rollout_epoch": int(et.get("rollout_epoch", 1)),
+                "eval_total_num_envs": int(ev.total_num_envs) if ev is not None else 0}
+
+    def _barrier(self):
+        if self.world_size > 1:
+            dist.barrier(group=self._pg)
+
+    def save_checkpoint(self, path=None) -> str:
+        """Save everything an exact resume needs (checkpoint.py has the layout) to `path`, by default
+        checkpoints/global_step_{global_step} under runner.logger; returns the directory.  Call it on every rank.
+        One device synchronisation: all device tensors are copied to pinned host memory, then the stream is waited on."""
+        path = path or ckpt.checkpoint_dir(self.cfg.runner, self.global_step)
+        pol = self.actor.model
+        rank_state = {"global_step": int(self.global_step), "env": self.env.state_dict(),
+                      "rollout": self.rollout.state_dict()}
+        if self.eval_env is not None:
+            rank_state["eval_env"] = self.eval_env.state_dict()
+        tree = {"rank": rank_state, "grads_nonzero": torch.count_nonzero(pol.flat_grads)}
+        if self.rank == 0:
+            tree["weights"] = dict(pol.named_parameters())
+            tree["trainer"] = {"actor": self.actor.state_dict(), "fingerprint": self.fingerprint()}
+        host = ckpt.to_host(tree)
+        torch.cuda.current_stream().synchronize()
+        # run_training ends with zero_grad: no gradient is carried between iterations
+        assert int(host["grads_nonzero"]) == 0, "save_checkpoint() between iterations only: gradients are not zero"
+        return ckpt.write(path, self.rank, host["rank"], host.get("weights"), host.get("trainer"), self._barrier)
+
+    def load_checkpoint(self, path) -> None:
+        """Restore a checkpoint written by save_checkpoint() at the same world size, env count and shapes; the next
+        iteration continues exactly where the saved run left off.  Everything is copied into the existing tensors, so
+        captured rollout, evaluation and optimiser-step graphs stay valid."""
+        path = str(path)
+        step = ckpt.step_from_path(path)
+        weights, trainer, rank_state = ckpt.read(path, self.rank)
+        ckpt.check_fingerprint(trainer["fingerprint"], self.fingerprint())
+        if int(rank_state["global_step"]) != step:
+            raise ValueError(f"{path} names step {step} but holds the state of step {rank_state['global_step']}")
+        self.actor.model.load_state_dict(weights, strict=True)
+        self.actor.load_state_dict(trainer["actor"])  # also refreshes the weight split and the frozen groups
+        self.env.load_state_dict(rank_state["env"])
+        self.rollout.load_state_dict(rank_state["rollout"])
+        if self.eval_env is not None:
+            self.eval_env.load_state_dict(rank_state["eval_env"])
+        self.global_step = step
