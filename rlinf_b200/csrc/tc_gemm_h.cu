@@ -31,8 +31,13 @@ constexpr int kB16 = BN * BK * 2;              // 16 KB per fp16 half of the wei
 constexpr int kWBytes = 2 * kB16;              // 32 KB: W hi | W lo
 constexpr int kStageBytes = kA32 + kWBytes;    // 48 KB
 constexpr int kRingBytes = kStages * kStageBytes;  // 192 KB
-constexpr int kThreads = 288;  // the block is resourced as three whole warpgroups: 168 registers per thread (a larger
-                               // register count fails to launch), so ptxas serialises the six wgmmas of a k-block
+// Three warpgroups: consumers 0 / 1 and the producer warpgroup 2.  A launch gives every thread 65536 / 384 -> 168
+// registers, too few for a 128-float accumulator plus two k-blocks of A fragments (ptxas would serialise the
+// wgmmas), so the producer warpgroup drops to kProducerRegs and the consumers take kConsumerRegs
+// (128 * P + 256 * C <= 65536).
+constexpr int kThreads = 384;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file");
 constexpr int kWeightScaleLog2 = 10;  // weights are stored as fp16 (hi, lo) of w * 2^10 (|w| <~ 1: both halves normal)
 
 // 1-D bulk copy global -> shared, completion counted on an mbarrier
@@ -42,8 +47,11 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(tma::smem_u32(bar))
                : "memory");
 }
-// barrier over the 256 consumer threads only (the producer warp runs ahead)
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// one warp's share of freeing a ring slot (the barrier counts one arrival per reading warp)
+__device__ __forceinline__ void warp_arrive(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) tma::mbar_arrive(bar);
+}
 
 // Operand layouts: K-major SWIZZLE_64B (forward pack: 64-B rows, SBO 512), MN-major SWIZZLE_128B (dgrad pack: SBO 1024 B
 // between 8 K-rows, LBO 4096 B between 64-wide N groups), MN-major SWIZZLE_64B (wgrad H: SBO 512, LBO 2048).
@@ -166,6 +174,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_gemm_kernel(const __grid_con
 
   if (wg == 2) {
     // ================= producer =================
+    wg::setmaxnreg_dec<kProducerRegs>();
     if (threadIdx.x == 256) {
       tma::prefetch_desc(&P.a[grp]);
       uint32_t s = 0, ph = 0;
@@ -182,6 +191,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_gemm_kernel(const __grid_con
     }
   } else {
     // ================= consumers: 64 rows each =================
+    wg::setmaxnreg_inc<kConsumerRegs>();
     const int cw = wg;
     const int g = lane >> 2, t = lane & 3;
     const int r_lo = cw * 64 + (warp & 3) * 16 + g;  // this thread's tile rows r_lo and r_lo + 8
@@ -190,18 +200,24 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_gemm_kernel(const __grid_con
     const float a_scale = pow2i(sa);
     const float out_scale = pow2i(-(sa + kWeightScaleLog2));
     float vmax = 0.f;
-    uint32_t s = 0, ph = 0;
+    // The CTA's k-block q (counted over all its tiles) sits in ring stage q % kStages, filled in phase q / kStages.
+    // Pipeline: the wgmmas of k-block q are one group; while it runs, the group of q - 1 is retired (wait<1>), its
+    // stage freed, and the A rows of q + 1 are split into the fragment registers q - 1 read.
+    auto load_a = [&](uint32_t q, uint32_t(&ah)[BK / 16][4], uint32_t(&al)[BK / 16][4]) {
+      tma::mbar_wait_brk(&bars->full[q % kStages], (q / kStages) & 1u);
+      const uint8_t* st = smem + (q % kStages) * kStageBytes;
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) a_frag_rows(st, r_lo, k * 16 + 2 * t, a_scale, ah[k], al[k]);
+    };
+    uint32_t q0 = 0;
     for (int64_t tile = cta; tile < n_tiles; tile += n_cta) {
       float acc[128];
 #pragma unroll
       for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < n_kb; ++kb) {
-        tma::mbar_wait(&bars->full[s], ph);
-        const uint8_t* st = smem + s * kStageBytes;
-        const uint32_t wbase = tma::smem_u32(st + kA32);
-        uint32_t ah[BK / 16][4], al[BK / 16][4];
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) a_frag_rows(st, r_lo, k * 16 + 2 * t, a_scale, ah[k], al[k]);
+      auto step = [&](int kb, const uint32_t(&ah)[BK / 16][4], const uint32_t(&al)[BK / 16][4],
+                      uint32_t(&nh)[BK / 16][4], uint32_t(&nl)[BK / 16][4]) {
+        const uint32_t q = q0 + kb;
+        const uint32_t wbase = tma::smem_u32(smem + (q % kStages) * kStageBytes + kA32);
         wg::fence();  // the A fragments were written by ordinary instructions
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
@@ -214,11 +230,19 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_gemm_kernel(const __grid_con
           wg::Mma<256, B_MN>::run(acc, ah[k], b_hi, 1u);
         }
         wg::commit();
-        wg::wait<0>();
-        __syncwarp();
-        if (lane == 0) tma::mbar_arrive(&bars->empty[s]);
-        if (++s == kStages) { s = 0; ph ^= 1u; }
+        wg::wait<1>();
+        if (kb > 0) warp_arrive(&bars->empty[(q - 1) % kStages]);
+        if (kb + 1 < n_kb) load_a(q + 1, nh, nl);
+      };
+      uint32_t ah0[BK / 16][4], al0[BK / 16][4], ah1[BK / 16][4], al1[BK / 16][4];
+      load_a(q0, ah0, al0);
+      for (int kb = 0; kb < n_kb; kb += 2) {
+        step(kb, ah0, al0, ah1, al1);
+        if (kb + 1 < n_kb) step(kb + 1, ah1, al1, ah0, al0);
       }
+      wg::wait<0>();
+      q0 += n_kb;
+      warp_arrive(&bars->empty[(q0 - 1) % kStages]);
       // ---- epilogue straight from the accumulator registers: 8-byte stores, each quad of lanes writes 32 B of a row ----
       const int64_t row0 = tile * BM + r_lo, row1 = row0 + 8;
       const bool ok0 = row0 < P.M, ok1 = row1 < P.M;
@@ -273,7 +297,8 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_gemm_kernel(const __grid_con
 // Weight-gradient GEMM:  dW[256, IN] += sum_m dZ[m, :]^T . H[m, :]     (IN % 32 == 0, <= 256); the reduction index m
 // (sample) is the strided one for both operands.  Grid = ngroups x 2 output tiles (128 rows of dW) x sample chunks;
 // each CTA writes its chunk's partial to a slot, the slots are summed in chunk order.  dZ^T fragments go straight into
-// registers, H is split into fp16 MN-major tiles (two operand slots).
+// registers; warps 9-11 of the producer warpgroup split H into fp16 MN-major tiles (two operand slots) while warp 8
+// issues the TMA loads.  The producer warpgroup keeps more registers than the forward kernel's for the split.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kWgLand = 3;
 constexpr int kWgA32 = 128 * BK * 4;                          // 16 KB of dZ
@@ -281,9 +306,15 @@ constexpr int kWgB32 = 256 * BK * 4, kWgB16 = 256 * BK * 2;   // 32 KB / 16 KB o
 constexpr int kWgLandBytes = kWgA32 + kWgB32;                 // 48 KB
 constexpr int kWgOpBytes = 2 * kWgB16;                        // 32 KB: H hi | H lo
 constexpr int kWgRingBytes = kWgLand * kWgLandBytes + 2 * kWgOpBytes;  // 144 + 64 KB
+constexpr int kWgSplitThreads = 96;                           // warps 9-11
+constexpr int kWgProducerRegs = 56, kWgConsumerRegs = 224;
+static_assert(128 * kWgProducerRegs + 256 * kWgConsumerRegs <= 65536, "register file");
 
 struct WgBarriers {
-  uint64_t full[kWgLand], empty[kWgLand];  // landing ring: TMA tx bytes / consumers done reading (one arrival per warp)
+  uint64_t full[kWgLand];   // landing ring: TMA tx bytes
+  uint64_t empty[kWgLand];  // landing stage read: dZ by the 8 consumer warps, H by the 3 split warps (one per warp)
+  uint64_t op_full[2];      // operand slot written by the split threads (one arrival per thread, after its proxy fence)
+  uint64_t op_empty[2];     // wgmmas reading the operand slot retired (one arrival per consumer warp)
 };
 
 struct WgradParams {
@@ -315,7 +346,11 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
   if (threadIdx.x == 0) {
     for (int s = 0; s < kWgLand; ++s) {
       tma::mbar_init(&bars->full[s], 1);
-      tma::mbar_init(&bars->empty[s], 8);
+      tma::mbar_init(&bars->empty[s], 8 + kWgSplitThreads / 32);
+    }
+    for (int o = 0; o < 2; ++o) {
+      tma::mbar_init(&bars->op_full[o], kWgSplitThreads);
+      tma::mbar_init(&bars->op_empty[o], 8);
     }
     tma::fence_barrier_init();
   }
@@ -323,7 +358,20 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
   if (n_kb <= 0) return;
 
   if (wg == 2) {
-    {  // producer warp
+    wg::setmaxnreg_dec<kWgProducerRegs>();
+    if (warp > 8) {  // H split: landing stage it % kWgLand -> operand slot it & 1
+      for (int it = 0; it < n_kb; ++it) {
+        const int s = it % kWgLand, o = it & 1;
+        tma::mbar_wait(&bars->full[s], (it / kWgLand) & 1u);
+        tma::mbar_wait(&bars->op_empty[o], ((it >> 1) & 1u) ^ 1u);  // wgmmas of k-block it - 2 retired
+        uint8_t* hop = op + o * kWgOpBytes;
+        // H groups of [32 samples x 32 floats] (4 KB) -> [32 samples x 32 halfs] (2 KB), contiguous on both sides
+        split_tile<kWgSplitThreads>(smem + s * kWgLandBytes + kWgA32, hop, hop + kWgB16, IN, threadIdx.x - 288, 1.0f);
+        tma::fence_proxy_async();  // generic-proxy stores -> the wgmmas' async-proxy reads
+        tma::mbar_arrive(&bars->op_full[o]);
+        warp_arrive(&bars->empty[s]);
+      }
+    } else {  // TMA warp
       const int n_box = 4 + IN / 32;
       for (int it = 0; it < n_kb; ++it) {
         const int s = it % kWgLand;
@@ -342,6 +390,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
       }
     }
   } else {
+    wg::setmaxnreg_inc<kWgConsumerRegs>();
     const int cw = wg;
     const int g = lane >> 2, t = lane & 3;
     const int f_lo = cw * 64 + (warp & 3) * 16 + g;  // this thread's rows of the dW tile: f_lo and f_lo + 8
@@ -350,20 +399,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
     float acc[NW / 2];
 #pragma unroll
     for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
-    for (int it = 0; it < n_kb; ++it) {
+    // dZ^T fragments of k-block it: A(m = feature f, k = sample) = dZ box f / 32 at (sample, f % 32); the landing
+    // stage is freed as soon as they are in registers
+    auto load_z = [&](int it, uint32_t(&ah)[BK / 16][4], uint32_t(&al)[BK / 16][4]) {
       const int s = it % kWgLand;
-      const uint32_t ph = (it / kWgLand) & 1u;
-      tma::mbar_wait(&bars->full[s], ph);
+      tma::mbar_wait_brk(&bars->full[s], (it / kWgLand) & 1u);
       const uint8_t* st = smem + s * kWgLandBytes;
-      uint8_t* hop = op + (it & 1) * kWgOpBytes;
-      // H groups of [32 samples x 32 floats] (4 KB) -> [32 samples x 32 halfs] (2 KB), contiguous on both sides.  The slot
-      // was last read by the wgmmas of k-block it - 2, which every consumer thread waited for before the barrier of it - 1.
-      split_tile<256>(st + kWgA32, hop, hop + kWgB16, (IN / 32) * 32, threadIdx.x, 1.0f);
-      tma::fence_proxy_async();
-      consumer_sync();
-      const uint32_t hb = tma::smem_u32(hop);
-      // dZ^T fragments: A(m = feature f, k = sample) = dZ box f / 32 at (sample, f % 32)
-      uint32_t ah[BK / 16][4], al[BK / 16][4];
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
 #pragma unroll
@@ -377,6 +418,14 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
           split2(x0 * z_scale, x1 * z_scale, ah[k][i], al[k][i]);
         }
       }
+      warp_arrive(&bars->empty[s]);
+    };
+    // one k-block: its wgmmas are one group; while it runs, the group of it - 1 is retired (wait<1>), its operand
+    // slot freed, and the dZ^T of it + 1 is split into the fragment registers it - 1 read
+    auto step = [&](int it, const uint32_t(&ah)[BK / 16][4], const uint32_t(&al)[BK / 16][4], uint32_t(&nh)[BK / 16][4],
+                    uint32_t(&nl)[BK / 16][4]) {
+      tma::mbar_wait_brk(&bars->op_full[it & 1], (it >> 1) & 1u);
+      const uint32_t hb = tma::smem_u32(op + (it & 1) * kWgOpBytes);
       wg::fence();
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
@@ -387,10 +436,17 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
         wg::Mma<NW, 1>::run(acc, ah[k], b_hi, 1u);
       }
       wg::commit();
-      wg::wait<0>();
-      __syncwarp();
-      if (lane == 0) tma::mbar_arrive(&bars->empty[s]);
+      wg::wait<1>();
+      if (it > 0) warp_arrive(&bars->op_empty[(it - 1) & 1]);
+      if (it + 1 < n_kb) load_z(it + 1, nh, nl);
+    };
+    uint32_t ah0[BK / 16][4], al0[BK / 16][4], ah1[BK / 16][4], al1[BK / 16][4];
+    load_z(0, ah0, al0);
+    for (int it = 0; it < n_kb; it += 2) {
+      step(it, ah0, al0, ah1, al1);
+      if (it + 1 < n_kb) step(it + 1, ah1, al1, ah0, al0);
     }
+    wg::wait<0>();
     float* slot = P.part + (size_t)(chunk * P.ngroups + grp) * 256 * IN;
     const int row0 = out_tile * 128 + f_lo;
 #pragma unroll

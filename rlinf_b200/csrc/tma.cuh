@@ -42,6 +42,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > (1u << 28)) __trap();
   }
 }
+// The same bound for warps that raised their registers with setmaxnreg.inc.  On sm_90a __brkpt() assembles to the
+// same BPT.TRAP instruction as __trap(), but a __trap() on the path makes ptxas (CUDA 12.9) ignore the raised count:
+// the wgmmas are then serialised and registers spill.
+__device__ __forceinline__ void mbar_wait_brk(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 28)) __brkpt();
+  }
+}
 
 // 2-D tiled load: box lands in smem, completion counted on `bar` (complete_tx::bytes).
 __device__ __forceinline__ void load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {

@@ -13,6 +13,13 @@ __device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync
 template <int N>
 __device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
+// warpgroup register reallocation (every warp of the warpgroup executes the same one): a producer warpgroup gives
+// registers back to the pool, the consumer warpgroups take them (R: multiple of 8 in [24, 256])
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // shared-memory matrix descriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout [62,64): 1 = SWIZZLE_128B,
 // 2 = SWIZZLE_64B (operand tiles 1024-byte aligned, base offset 0)
 __device__ __forceinline__ uint64_t desc(uint32_t saddr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
