@@ -181,8 +181,9 @@ typedef struct rb200_ppo_args {
 int rb200_ppo_loss(const rb200_ppo_args* args, rb200_stream_t stream);
 
 /* "decoupled_actor_critic" (losses.py:27-167 + :315-380, registered :383-394): PPO clipped around a proximal policy.
- * `base` carries everything shared with rb200_ppo_loss (entropy / log-ratio clamps / adv_stats must be unset);
- * metrics use the RB200_DM_* layout. */
+ * `base` carries everything shared with rb200_ppo_loss (log-ratio clamps / adv_stats must be unset). The entropy
+ * bonus is the worker's (async_ppo_fsdp_worker.py:443-456): base.entropy / d_entropy / entropy_bonus as in
+ * rb200_ppo_loss, with the masked-mean entropy reported in RB200_DM_ENTROPY.  Metrics use the RB200_DM_* layout. */
 enum {
   RB200_DM_POLICY_LOSS = 0,            /* actor/policy_loss            */
   RB200_DM_PROXIMAL_RATIO = 1,         /* actor/proximal_ratio         */
@@ -199,7 +200,8 @@ enum {
   RB200_DM_TOTAL_LOSS = 16,
   RB200_DM_TOKEN_NUM = 17,
   RB200_DM_CURRENT_VERSION = 18,       /* actor/current_version */
-  RB200_DM_HAS_VERSION_METRICS = 19
+  RB200_DM_HAS_VERSION_METRICS = 19,
+  RB200_DM_ENTROPY = 20                /* actor/entropy_loss (0 unless base.entropy, entropy_bonus > 0, no critic warm-up) */
 };
 typedef struct rb200_dppo_args {
   rb200_ppo_args base;
@@ -211,6 +213,19 @@ typedef struct rb200_dppo_args {
   double behave_weight_threshold;
 } rb200_dppo_args;
 int rb200_decoupled_ppo_loss(const rb200_dppo_args* args, rb200_stream_t stream);
+
+/* The same loss for a batch generated by ONE weight version (one rollout between weight refreshes): the version is a
+ * scalar, so no [rows, C*A] version tensor is built or gathered.  Identical results to rb200_decoupled_ppo_loss with
+ * `versions` filled with `version` and has_current_version = 1. */
+typedef struct rb200_dppo_scalar_version_args {
+  rb200_ppo_args base;
+  const float* proximal_logprobs; /* [rows, C*A] or NULL: the version interpolation */
+  double version;                 /* weight version that generated every token of the batch */
+  double current_version;
+  int32_t has_behave_weight_threshold;
+  double behave_weight_threshold;
+} rb200_dppo_scalar_version_args;
+int rb200_decoupled_ppo_loss_scalar_version(const rb200_dppo_scalar_version_args* args, rb200_stream_t stream);
 
 /* "opd" (losses.py:427-505): loss = agg(-logprobs * stop_grad(advantages)) with the mask / mask_sum broadcast over the
  * tokens of a unit. logprobs, advantages: [n_units, tokens_per_unit]; loss_mask (uint8), loss_mask_sum: [n_units].
@@ -527,6 +542,8 @@ int rb200_masked_stats(const float* x, const uint8_t* mask, int64_t n, int64_t m
  * ---------------------------------------------------------------------------------------- */
 /* masked_stats (distributed.py:942-954) and the three sums masked_normalization all-reduces (:903-933):
  * out3 = {count, sum x, sum x^2} over entries with mask != 0 (mask NULL = all), accumulated in fp64. */
+/* Fixed summation order (per-CTA slots in the library's per-device scratch, one ordered pass): repeated calls give the
+ * same bits. The scratch is per device, so calls on one device must be stream-ordered. */
 int rb200_masked_moments(const float* x, const uint8_t* mask, int64_t n, double* out3 /*reset by the call*/,
                          rb200_stream_t stream);
 /* Apply half, stats3 = (all-reduced) {count, sum, sumsq}:

@@ -61,6 +61,12 @@ class DppoArgs(C.Structure):
                 ("has_behave_weight_threshold", C.c_int32), ("behave_weight_threshold", c_double)]
 
 
+class DppoScalarVersionArgs(C.Structure):
+    _fields_ = [("base", PpoArgs), ("proximal_logprobs", c_void_p), ("version", c_double),
+                ("current_version", c_double), ("has_behave_weight_threshold", C.c_int32),
+                ("behave_weight_threshold", c_double)]
+
+
 class RolloutArgs(C.Structure):
     _fields_ = [(n, c_void_p) for n in (
         "states", "actions", "logprobs", "values", "rewards", "terminations", "truncations", "dones", "final_obs",
@@ -81,6 +87,7 @@ DM_KEYS = {
     12: "__sum__/_critic_explained_variance/returns_sq_sum", 13: "__sum__/_critic_explained_variance/errors_sum",
     14: "__sum__/_critic_explained_variance/errors_sq_sum",
 }
+DM_ENTROPY = 20  # RB200_DM_ENTROPY: actor/entropy_loss of the decoupled loss
 
 
 class MlpLayout(C.Structure):
@@ -108,6 +115,7 @@ SIGNATURES = {
     "rb200_gather_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
     "rb200_ppo_loss": (c_int, [C.POINTER(PpoArgs), c_void_p]),
     "rb200_decoupled_ppo_loss": (c_int, [C.POINTER(DppoArgs), c_void_p]),
+    "rb200_decoupled_ppo_loss_scalar_version": (c_int, [C.POINTER(DppoScalarVersionArgs), c_void_p]),
     "rb200_opd_loss": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_double] + [c_void_p] * 5),
     "rb200_scale": (c_int, [c_void_p, c_int64, c_float, c_void_p]),
     "rb200_scale_by": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),

@@ -221,8 +221,6 @@ def fused_embodied_policy_loss(**kwargs):
     entropy = kwargs.get("entropy")
     ent_bonus = float(kwargs.get("entropy_bonus", 0.0) or 0.0)
     if entropy is not None:
-        if decoupled:
-            raise NotImplementedError("entropy term is not fused into the decoupled loss kernel")
         ent_type = kwargs.get("entropy_type", "action_level")
         want = "chunk_level" if logprob_type == "chunk_level" else "action_level"
         if ent_type != want:
@@ -236,7 +234,7 @@ def fused_embodied_policy_loss(**kwargs):
                               cfg, with_critic, as_float=True, decoupled=decoupled)
     if entropy is not None or kwargs.get("loss_scale") is not None:
         host = raw.tolist()
-        metrics["actor/entropy_loss"] = host[15]
+        metrics["actor/entropy_loss"] = host[L.DM_ENTROPY if decoupled else 15]
         metrics["actor/total_loss"] = host[16]
     return loss, metrics
 

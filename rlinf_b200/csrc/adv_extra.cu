@@ -8,9 +8,17 @@
 namespace {
 
 // ---- {count, sum, sumsq} of x over the mask, fp64 (masked_stats; masked_normalization's factor / x_sum / x_sum_sq) --
+// Fixed order, so repeated calls agree bit for bit: each CTA writes its partial sums to its own slot; the last CTA to
+// arrive adds the slots in CTA order (thread t takes CTAs t, t + 256, ... in order, then the fixed block tree) and
+// clears the arrival counter.  `scratch` is the per-device rb::device_scratch (zero-initialised): the arrival counter in
+// its first 8 bytes, then 3 doubles per CTA.  Calls on one device are therefore stream-ordered.
 __global__ void __launch_bounds__(256) masked_moments_kernel(const float* __restrict__ x, const uint8_t* __restrict__ mask,
-                                                             int64_t n, double* __restrict__ out3) {
+                                                             int64_t n, double* __restrict__ out3,
+                                                             double* __restrict__ scratch) {
+  unsigned long long* arrived = reinterpret_cast<unsigned long long*>(scratch);
+  double* part = scratch + 1;
   __shared__ double red[3 * 32];
+  __shared__ int is_last;
   double v[3] = {0.0, 0.0, 0.0};
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
@@ -23,9 +31,28 @@ __global__ void __launch_bounds__(256) masked_moments_kernel(const float* __rest
   }
   rb::block_sum<3>(v, red);
   if (threadIdx.x == 0) {
-    atomicAdd(&out3[0], v[0]);
-    atomicAdd(&out3[1], v[1]);
-    atomicAdd(&out3[2], v[2]);
+    part[blockIdx.x * 3 + 0] = v[0];
+    part[blockIdx.x * 3 + 1] = v[1];
+    part[blockIdx.x * 3 + 2] = v[2];
+    __threadfence();
+    is_last = atomicAdd(arrived, 1ull) == (unsigned long long)gridDim.x - 1ull;
+  }
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  double w[3] = {0.0, 0.0, 0.0};
+  for (int b = threadIdx.x; b < (int)gridDim.x; b += blockDim.x) {
+    w[0] += __ldcg(&part[b * 3 + 0]);
+    w[1] += __ldcg(&part[b * 3 + 1]);
+    w[2] += __ldcg(&part[b * 3 + 2]);
+  }
+  __syncthreads();  // `red` is reused
+  rb::block_sum<3>(w, red);
+  if (threadIdx.x == 0) {
+    out3[0] = w[0];
+    out3[1] = w[1];
+    out3[2] = w[2];
+    *arrived = 0ull;
   }
 }
 
@@ -290,11 +317,15 @@ extern "C" int rb200_masked_moments(const float* x, const uint8_t* mask, int64_t
   if (!x || !out3) return RB200_E_NULL;
   if (n < 0) return RB200_E_SHAPE;
   cudaStream_t st = rb::as_stream(stream);
-  RB_CHECK_CUDA(cudaMemsetAsync(out3, 0, 3 * sizeof(double), st));
-  if (n > 0) {
-    masked_moments_kernel<<<grid_for(n, 4), 256, 0, st>>>(x, mask, n, out3);
-    rb::count_launch();
+  if (n == 0) {
+    RB_CHECK_CUDA(cudaMemsetAsync(out3, 0, 3 * sizeof(double), st));
+    return RB200_OK;
   }
+  const int blocks = grid_for(n, 4);
+  double* scratch = rb::device_scratch(1 + 3 * blocks);
+  if (!scratch) return RB200_E_UNSUPPORTED;
+  masked_moments_kernel<<<blocks, 256, 0, st>>>(x, mask, n, out3, scratch);  // writes all of out3
+  rb::count_launch();
   RB_RETURN_LAUNCH();
 }
 

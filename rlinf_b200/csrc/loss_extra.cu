@@ -4,6 +4,9 @@
 //     interpolated between behaviour and current policy from the weight versions), importance weight
 //     exp(proximal - old) towards the behaviour policy with an optional cut-off.
 //   * "opd": compute_opd_actor_loss (:427-505) - -logp * stop_grad(dense reverse-KL reward).
+// The decoupled loss also folds in the worker's entropy bonus (async_ppo_fsdp_worker.py:443-456), and its weight version
+// is either a per-token tensor (rb200_decoupled_ppo_loss) or one scalar for the whole batch
+// (rb200_decoupled_ppo_loss_scalar_version).
 // One pre-pass (mask / behaviour-mask counts: the masked-mean denominators are needed by the gradient), one main pass
 // whose last CTA forms loss + metrics and clears the workspace.
 #include "common.cuh"
@@ -22,6 +25,7 @@ enum DSlot {
   D_BKL,       // sum where(bmask, prox - old, 0)
   D_VER,       // sum versions over mask (units)
   D_VL, D_VCLIP, D_EV_N, D_EV_R, D_EV_R2, D_EV_E, D_EV_E2,
+  D_ENT,       // sum of per-unit entropy (summed over the unit's tokens) over the mask
   D_NUM
 };
 static_assert(D_NUM <= 31, "workspace is 32 doubles, slot 31 is the arrival counter");
@@ -30,7 +34,7 @@ struct DHyper {
   float clip_lo, clip_hi, dual_c;
   float value_clip, huber_delta, half_huber_delta, max_episode_steps;
   int critic_warmup;
-  float loss_scale;
+  float loss_scale, entropy_bonus;
   int has_version, has_thr;
   float cur_version, prox_version, thr;
 };
@@ -59,7 +63,9 @@ __device__ __forceinline__ float proximal(float lp, float old, const float* prox
 struct DArgs {
   rb200_ppo_args b;
   const float* prox;
-  const float* versions;
+  const float* versions;  // per-token versions, or NULL
+  int has_versions;       // versions != NULL, or the scalar `ver_scalar` stands for every token
+  float ver_scalar;
 };
 
 // reduced (lp, old, prox-sum, version) of unit u / element k
@@ -73,7 +79,7 @@ __device__ __forceinline__ void load_entry(const DArgs& a, int64_t u, int64_t so
     lp = lp_cur[k];
     old = lp_old[k];
     psum = pp ? pp[k] : 0.0f;
-    ver = a.versions ? a.versions[so * g + k] : 0.0f;
+    ver = a.versions ? a.versions[so * g + k] : a.ver_scalar;
   } else {
     lp = old = psum = 0.0f;
     for (int j = 0; j < g; ++j) {
@@ -81,7 +87,7 @@ __device__ __forceinline__ void load_entry(const DArgs& a, int64_t u, int64_t so
       old = __fadd_rn(old, lp_old[j]);
       if (pp) psum = __fadd_rn(psum, pp[j]);
     }
-    ver = a.versions ? a.versions[so * g] : 0.0f;  // versions[..., 0] / versions[:, 0, 0]
+    ver = a.versions ? a.versions[so * g] : a.ver_scalar;  // versions[..., 0] / versions[:, 0, 0]
   }
 }
 
@@ -106,7 +112,7 @@ __global__ void __launch_bounds__(256) dppo_count_kernel(DArgs a, DHyper h, int 
       for (int k = 0; k < reps; ++k) {
         float lp, old, psum, ver;
         load_entry<TOKEN>(a, u, so, g, k, lp, old, psum, ver);
-        const float px = proximal(lp, old, a.prox, psum, ver, a.versions != nullptr, h);
+        const float px = proximal(lp, old, a.prox, psum, ver, a.has_versions != 0, h);
         const float bw = expf(__fsub_rn(px, old));
         v[1] += (bw <= h.thr) ? 1.0 : 0.0;
       }
@@ -141,7 +147,7 @@ __device__ void dppo_finalize(const DArgs& a, const DHyper& h, int U, int g, int
   M[RB200_DM_PROXIMAL_APPROX_KL] = (float)(-s[D_PKL] / cnt);
   M[RB200_DM_BEHAV_APPROX_KL] = (float)(-s[D_BKL] / bcnt);
   // actor/average_version: only when versions has the (preprocessed) loss-mask shape and the mask has a True entry
-  const bool ver_shape_ok = a.versions != nullptr && h.has_version && (!token_mode || !has_mask);
+  const bool ver_shape_ok = a.has_versions && h.has_version && (!token_mode || !has_mask);
   if (ver_shape_ok && s[D_CNT] > 0.0) {
     M[RB200_DM_HAS_VERSION_METRICS] = 1.0f;
     M[RB200_DM_AVERAGE_VERSION] = (float)(s[D_VER] / s[D_CNT]);
@@ -160,6 +166,16 @@ __device__ void dppo_finalize(const DArgs& a, const DHyper& h, int U, int g, int
     M[RB200_DM_EV_COUNT + 3] = (float)s[D_EV_E];
     M[RB200_DM_EV_COUNT + 4] = (float)s[D_EV_E2];
     total += vl;
+  }
+  // the worker's entropy term: loss -= entropy_bonus * masked_mean(entropy, loss_mask), outside critic warm-up only
+  // chunk level with a mask: the reference's masked_mean broadcasts the [bsz] entropy against the [bsz, 1] mask, which
+  // gives sum(entropy) * count / count, the sum over every unit (0 when no entry is valid)
+  if (a.b.entropy && h.entropy_bonus > 0.0f && !h.critic_warmup) {
+    const bool ent_bcast = has_mask && a.b.logprob_type == RB200_LOGPROB_CHUNK;
+    const double d_ent = ent_bcast ? 1.0 : (has_mask ? (s[D_CNT] > 0.0 ? s[D_CNT] : 1.0) : n_units);
+    const double ent = (ent_bcast && !(s[D_CNT] > 0.0)) ? 0.0 : s[D_ENT] / d_ent;
+    M[RB200_DM_ENTROPY] = (float)ent;
+    total -= (double)h.entropy_bonus * ent;
   }
   total *= (double)h.loss_scale;
   M[RB200_DM_TOTAL_LOSS] = (float)total;
@@ -181,6 +197,12 @@ __global__ void __launch_bounds__(256, 2) dppo_main_kernel(DArgs a, DHyper h, in
   const float coef_actor = ratio_agg ? (float)(1.0 / n_elems) : (float)(1.0 / (bcnt > 0.0 ? bcnt : 1.0));
   const float coef_unit = ratio_agg ? (float)(1.0 / (double)n_units)
                                     : (has_mask ? (float)(1.0 / (mcnt > 0.0 ? mcnt : 1.0)) : (float)(1.0 / (double)n_units));
+  // d masked_mean(entropy, loss_mask) / d entropy: the mask count whatever the policy-loss aggregation; 1 (or 0 with no
+  // valid entry) for the chunk-level broadcast, see dppo_finalize
+  const bool ent_bcast = has_mask && a.b.logprob_type == RB200_LOGPROB_CHUNK;
+  const float coef_ent = ent_bcast ? (mcnt > 0.0 ? 1.0f : 0.0f)
+                                   : (has_mask ? (float)(1.0 / (mcnt > 0.0 ? mcnt : 1.0)) : (float)(1.0 / (double)n_units));
+  const float ent_grad = (h.entropy_bonus > 0.0f && !h.critic_warmup) ? -h.loss_scale * h.entropy_bonus * coef_ent : 0.0f;
   const float scale = h.loss_scale;
 
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -203,7 +225,7 @@ __global__ void __launch_bounds__(256, 2) dppo_main_kernel(DArgs a, DHyper h, in
     for (int k = 0; k < reps; ++k) {
       float lp, old, psum, ver;
       load_entry<TOKEN>(a, u, so, g, k, lp, old, psum, ver);
-      const float px = proximal(lp, old, a.prox, psum, ver, a.versions != nullptr, h);
+      const float px = proximal(lp, old, a.prox, psum, ver, a.has_versions != 0, h);
       const float lr = __fsub_rn(lp, px);
       const float ratio = m ? expf(lr) : 0.0f;
       const float clipped = fminf(fmaxf(ratio, h.clip_lo), h.clip_hi);
@@ -234,7 +256,7 @@ __global__ void __launch_bounds__(256, 2) dppo_main_kernel(DArgs a, DHyper h, in
       acc[D_DUAL] += (dual_hit && m) ? 1.0f : 0.0f;
       acc[D_PKL] += m ? lr : 0.0f;
       acc[D_BKL] += bm ? __fsub_rn(px, old) : 0.0f;
-      if (m && a.versions != nullptr) acc[D_VER] += ver;
+      if (m && a.has_versions) acc[D_VER] += ver;
       const float cw = ratio_agg ? coef_actor / w : coef_actor;
       const float gval = (h.critic_warmup || !bm) ? 0.0f : scale * cw * bw * dle * ratio;
       if (TOKEN) {
@@ -271,6 +293,18 @@ __global__ void __launch_bounds__(256, 2) dppo_main_kernel(DArgs a, DHyper h, in
         const float dvl = -(g1 * huber_grad(e1, h.huber_delta)) - (pass_c ? g2 * huber_grad(e2, h.huber_delta) : 0.0f);
         const float cw = has_mask ? (ratio_agg ? coef_unit / w : coef_unit) * mf : coef_unit;
         a.b.d_values[u] = scale * cw * dvl;
+      }
+    }
+
+    if (a.b.entropy) {
+      const float* en = a.b.entropy + u * g;
+      float es = 0.0f;
+      for (int k = 0; k < g; ++k) es = __fadd_rn(es, en[k]);
+      acc[D_ENT] += (has_mask && !ent_bcast) ? __fmul_rn(es, mf) : es;
+      if (a.b.d_entropy) {
+        float* de = a.b.d_entropy + u * g;
+        const float gval = (has_mask && !ent_bcast) ? ent_grad * mf : ent_grad;
+        for (int k = 0; k < g; ++k) de[k] = gval;
       }
     }
   }
@@ -372,18 +406,18 @@ inline int grid_for(int64_t n) {
   return (int)(blocks < 1 ? 1 : blocks);
 }
 
-}  // namespace
-
-extern "C" int rb200_decoupled_ppo_loss(const rb200_dppo_args* args, rb200_stream_t stream) {
-  if (!args) return RB200_E_NULL;
-  const rb200_ppo_args& b = args->base;
+// shared by both decoupled entry points: versions != NULL (per token) or has_scalar (one version for every token)
+int launch_decoupled(const rb200_ppo_args& b, const float* prox, const float* versions, int has_scalar,
+                     double ver_scalar, int has_current_version, double current_version, int has_thr, double thr,
+                     cudaStream_t st) {
   if (!b.logprobs || !b.old_logprobs || !b.advantages || !b.metrics || !b.workspace) return RB200_E_NULL;
   if (b.bsz <= 0 || b.C <= 0 || b.A <= 0) return RB200_E_SHAPE;
   if (b.logprob_type < RB200_LOGPROB_TOKEN || b.logprob_type > RB200_LOGPROB_CHUNK) return RB200_E_ARG;
   if (b.with_critic && (!b.values || !b.returns || !b.prev_values)) return RB200_E_NULL;
   if (b.clip_ratio_c > 0.0 && !(b.clip_ratio_c > 1.0)) return RB200_E_ARG;  // losses.py:106 assert
-  if (b.entropy || b.d_entropy || b.adv_stats || b.has_clip_log_ratio_min || b.has_clip_log_ratio_max)
-    return RB200_E_UNSUPPORTED;
+  if (b.d_entropy && !b.entropy) return RB200_E_NULL;
+  if (b.adv_stats || b.has_clip_log_ratio_min || b.has_clip_log_ratio_max) return RB200_E_UNSUPPORTED;
+  if (b.entropy && b.logprob_type == RB200_LOGPROB_CHUNK && b.C != 1) return RB200_E_UNSUPPORTED;
   const int U = b.logprob_type == RB200_LOGPROB_CHUNK ? 1 : b.C;
   const int g = b.logprob_type == RB200_LOGPROB_CHUNK ? b.C * b.A : b.A;
   DHyper h;
@@ -396,13 +430,13 @@ extern "C" int rb200_decoupled_ppo_loss(const rb200_dppo_args* args, rb200_strea
   h.max_episode_steps = b.max_episode_steps > 0 ? (float)b.max_episode_steps : 0.0f;
   h.critic_warmup = b.critic_warmup;
   h.loss_scale = (float)b.loss_scale;
-  h.has_version = args->has_current_version;
-  h.cur_version = (float)args->current_version;
-  h.prox_version = (float)(args->current_version - 1.0);
-  h.has_thr = args->has_behave_weight_threshold;
-  h.thr = (float)args->behave_weight_threshold;
-  DArgs a{b, args->proximal_logprobs, args->versions};
-  cudaStream_t st = rb::as_stream(stream);
+  h.entropy_bonus = (float)b.entropy_bonus;
+  h.has_version = has_current_version;
+  h.cur_version = (float)current_version;
+  h.prox_version = (float)(current_version - 1.0);
+  h.has_thr = has_thr;
+  h.thr = (float)thr;
+  DArgs a{b, prox, versions, (versions != nullptr || has_scalar) ? 1 : 0, versions ? 0.0f : (float)ver_scalar};
   const int blocks = grid_for(b.bsz * U);
   const bool token = b.logprob_type == RB200_LOGPROB_TOKEN;
   if (token) dppo_count_kernel<true><<<blocks, 256, 0, st>>>(a, h, U, g, b.workspace);
@@ -412,6 +446,22 @@ extern "C" int rb200_decoupled_ppo_loss(const rb200_dppo_args* args, rb200_strea
   else dppo_main_kernel<false><<<blocks, 256, 0, st>>>(a, h, U, g, b.workspace);
   rb::count_launch();
   RB_RETURN_LAUNCH();
+}
+
+}  // namespace
+
+extern "C" int rb200_decoupled_ppo_loss(const rb200_dppo_args* args, rb200_stream_t stream) {
+  if (!args) return RB200_E_NULL;
+  return launch_decoupled(args->base, args->proximal_logprobs, args->versions, 0, 0.0, args->has_current_version,
+                          args->current_version, args->has_behave_weight_threshold, args->behave_weight_threshold,
+                          rb::as_stream(stream));
+}
+
+extern "C" int rb200_decoupled_ppo_loss_scalar_version(const rb200_dppo_scalar_version_args* args,
+                                                       rb200_stream_t stream) {
+  if (!args) return RB200_E_NULL;
+  return launch_decoupled(args->base, args->proximal_logprobs, nullptr, 1, args->version, 1, args->current_version,
+                          args->has_behave_weight_threshold, args->behave_weight_threshold, rb::as_stream(stream));
 }
 
 extern "C" int rb200_opd_loss(const float* logprobs, const float* advantages, const uint8_t* loss_mask,

@@ -101,7 +101,8 @@ def ppo_loss(*, logprobs, old_logprobs, advantages, C_chunks, A_dim, logprob_typ
              _decoupled=None):
     """One fused launch group. Returns (loss[1], metrics[24], d_logprobs|None, d_values|None, d_entropy|None).
     `_decoupled` (internal): dict(proximal_logprobs, versions, current_version, behave_weight_threshold) selects
-    rb200_decoupled_ppo_loss (metrics in the RB200_DM_* layout)."""
+    rb200_decoupled_ppo_loss (metrics in the RB200_DM_* layout); with a `version` number instead of the `versions`
+    tensor (one weight version for the whole batch), rb200_decoupled_ppo_loss_scalar_version."""
     lib = L.load()
     dev = logprobs.device
     bsz = logprobs.shape[0]
@@ -155,6 +156,17 @@ def ppo_loss(*, logprobs, old_logprobs, advantages, C_chunks, A_dim, logprob_typ
     d_e = torch.empty_like(keep[0]) if (want_grads and entropy is not None) else None
     a.workspace, a.loss, a.metrics = L.ptr(ws), L.ptr(loss), L.ptr(metrics)
     a.d_logprobs, a.d_values, a.d_entropy = L.ptr(d_lp), L.ptr(d_v), L.ptr(d_e)
+    if _decoupled is not None and _decoupled.get("version") is not None:
+        if _decoupled.get("versions") is not None or _decoupled.get("current_version") is None:
+            raise ValueError("a scalar `version` needs `current_version` and excludes the `versions` tensor")
+        d = L.DppoScalarVersionArgs()
+        d.base = a
+        d.proximal_logprobs = P(_decoupled.get("proximal_logprobs"), torch.float32)
+        d.version, d.current_version = float(_decoupled["version"]), float(_decoupled["current_version"])
+        thr = _decoupled.get("behave_weight_threshold")
+        d.has_behave_weight_threshold, d.behave_weight_threshold = int(thr is not None), float(thr or 0.0)
+        L.check(lib.rb200_decoupled_ppo_loss_scalar_version(C.byref(d), L.stream_ptr()), "decoupled_ppo_loss")
+        return loss, metrics, d_lp, d_v, d_e
     if _decoupled is not None:
         d = L.DppoArgs()
         d.base = a
