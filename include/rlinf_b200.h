@@ -332,9 +332,18 @@ int rb200_tc_gemm_h(const float* A, const float* B, float* C, int64_t M, int K, 
                     float* work, rb200_stream_t stream);
 int rb200_tc_wgrad_h(const float* Z, const float* H, float* dW, int64_t n, int IN, const float* amax,
                      rb200_stream_t stream);
+/* Backward through a square hidden layer (csrc/tc_backward_h.cu) for ngroups (1 or 2) towers stacked along the first
+ * dimension: dW[g] += Z[g]^T . H[g];  dZprev[g] = (Z[g] . W[g]) * (1 - H[g]^2), colsum[g] += its column sums,
+ * atomicMax(amax_out[g], max|dZprev[g]|).  Z, H, dZprev: [ngroups, n, 256]; W, dW: [ngroups, 256, 256]; colsum
+ * [ngroups, 256], amax_in (max|Z[g]|) and amax_out [ngroups] are nullable.
+ * work: >= ngroups * (131072 + 256 * ceil(n / 16)) floats. */
+int rb200_tc_dgrad_wgrad_h(const float* Z, const float* W, const float* H, float* dZprev, float* dW, float* colsum,
+                           const float* amax_in, float* amax_out, int64_t n, int ngroups, float* work,
+                           rb200_stream_t stream);
 
 /* Experiment switches (tests only; default 0 = the shipped kernels): 2 = round-1 layers in the fp32 SIMT fused rollout
- * (one-k-step weight prefetch). */
+ * (one-k-step weight prefetch); 4 = the hidden-layer backward of the MLP update as separate wgrad and dgrad kernels
+ * instead of the fused one. */
 int rb200_debug_set_flags(int flags);
 
 /* Persistent rollouts: the whole T-step loop of one rank - MLP actor/critic inference, Normal sampling, synthetic-env

@@ -494,19 +494,17 @@ int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, 
 int towers_backward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, TowerIO* t, int nt, cudaStream_t st) {
   int e;
   rb::tch::WgradLaunch w[2];
-  rb::tch::GemmLaunch g[2];
+  rb::tch::BackwardLaunch b[2];
   // layer 2: dW2 += dZ3^T . H2 ; dZ2 = (dZ3 . W2) * (1 - H2^2)  (+ column sums -> g_b1, max|dZ2| -> amax[1])
-  for (int i = 0; i < nt; ++i) w[i] = rb::tch::WgradLaunch{t[i].dZ3, t[i].H2, t[i].g_w2, t[i].amax};
-  if ((e = rb::tch::wgrad(w, nt, n, kH, st))) return e;
   for (int i = 0; i < nt; ++i)
-    g[i] = rb::tch::GemmLaunch{t[i].dZ3, t[i].wh.w2d, nullptr, t[i].tA, nullptr, t[i].H2, t[i].g_b1, t[i].amax, t[i].amax + 1};
-  if ((e = rb::tch::launch(g, nt, n, kH, rb::tc::EPI_TANHGRAD, 1, st))) return e;
-  // layer 1
-  for (int i = 0; i < nt; ++i) w[i] = rb::tch::WgradLaunch{t[i].tA, t[i].H1, t[i].g_w1, t[i].amax + 1};
-  if ((e = rb::tch::wgrad(w, nt, n, kH, st))) return e;
+    b[i] = rb::tch::BackwardLaunch{t[i].dZ3, t[i].wh.w2d, t[i].H2, t[i].tA, t[i].g_w2, t[i].g_b1, t[i].amax, t[i].amax + 1,
+                                   t[i].tB};  // dZ1's buffer is free until layer 1
+  if ((e = rb::tch::dgrad_wgrad(b, nt, n, st))) return e;
+  // layer 1 (dZ3 is consumed: its buffer, part of the backward's own work area, takes the column-sum scratch)
   for (int i = 0; i < nt; ++i)
-    g[i] = rb::tch::GemmLaunch{t[i].tA, t[i].wh.w1d, nullptr, t[i].tB, nullptr, t[i].H1, t[i].g_b0, t[i].amax + 1, t[i].amax + 2};
-  if ((e = rb::tch::launch(g, nt, n, kH, rb::tc::EPI_TANHGRAD, 1, st))) return e;
+    b[i] = rb::tch::BackwardLaunch{t[i].tA, t[i].wh.w1d, t[i].H1, t[i].tB, t[i].g_w1, t[i].g_b0, t[i].amax + 1, t[i].amax + 2,
+                                   const_cast<float*>(t[i].dZ3)};
+  if ((e = rb::tch::dgrad_wgrad(b, nt, n, st))) return e;
   // layer 0: dW0 += dZ1^T . X
   if (idx == nullptr && (in_dim % rb::tc::BK == 0) && in_dim <= 256) {
     for (int i = 0; i < nt; ++i) w[i] = rb::tch::WgradLaunch{t[i].tB, X, t[i].g_w0, t[i].amax + 2};
@@ -547,9 +545,10 @@ extern "C" int rb200_mlp_layout_init(rb200_mlp_layout* L, int obs_dim, int act_d
   L->mw = take((int64_t)act_dim * hidden); L->mb = take(act_dim);
   L->total = (o + 3) & ~int64_t(3);
   // size the per-CTA partial-sum scratch of the backward for this layout now, outside any CUDA-graph capture (largest
-  // of: head_bwd <= 4 blocks per SM, wgrad <= SMs / 2 chunk slots of 256 x 256, dgrad column sums); no device: no-op
+  // of: head_bwd <= 4 blocks per SM, wgrad <= SMs / 2 chunk slots of 256 x 256 (+ <= SMs dgrad column-sum slots
+  // of 256 in the fused dgrad_wgrad), dgrad column sums); no device: no-op
   const int64_t sms = rb::sm_count(), head = 4 * sms * ((act_dim + value_dim) * hidden + 64 + 2 * hidden);
-  const int64_t wg = sms / 2 * hidden * hidden;
+  const int64_t wg = sms / 2 * hidden * hidden + sms * hidden;
   if (!rb::partials_scratch(head > wg ? head : wg)) (void)cudaGetLastError();
   return RB200_OK;
 }

@@ -10,7 +10,8 @@ constexpr int BM = 128, BN = 256, BK = 32;  // BK fp32 = 128 bytes = one swizzle
 
 enum Epi { EPI_STORE = 0, EPI_BIAS_TANH = 1, EPI_TANHGRAD = 2 };
 
-// debug/experiment switches (rb200_debug_set_flags): bit 1 (2) = round-1 fused-rollout layers (one-k-step weight prefetch)
+// debug/experiment switches (rb200_debug_set_flags): bit 1 (2) = round-1 fused-rollout layers (one-k-step weight prefetch);
+// bit 2 (4) = hidden-layer backward as separate wgrad + dgrad launches instead of the fused dgrad_wgrad kernel
 extern int g_debug_flags;
 
 }  // namespace tc
@@ -46,6 +47,19 @@ struct SplitSpec {
 // epi: rb::tc::Epi.  b_mn = 0: C = epi(A . W^T) (forward, W [256,K]);  b_mn = 1: C = epi(A . W) (dgrad, W [256,256]).
 int launch(const GemmLaunch* groups, int ngroups, int64_t M, int K, int epi, int b_mn, cudaStream_t st);
 int wgrad(const WgradLaunch* groups, int ngroups, int64_t n, int IN, cudaStream_t st);
+struct BackwardLaunch {    // one group of the backward through a square hidden layer (tc_backward_h.cu)
+  const float* z;          // [n,256] dZ_L
+  const float* wpack;      // dgrad pack of W_L (split_weights)
+  const float* h;          // [n,256] H_{L-1}
+  float* dzprev;           // [n,256] dZ_{L-1} = (dZ_L . W_L) * (1 - H_{L-1}^2)
+  float* dW;               // [256,256] += dZ_L^T . H_{L-1}
+  float* colsum;           // [256] += column sums of dZ_{L-1}, or NULL
+  const float* amax_in;    // device max|dZ_L| or NULL
+  float* amax_out;         // atomicMax of |dZ_{L-1}|, or NULL
+  float* scratch;          // with colsum: [ceil(n/16), 256] floats of 16-row column sums (may be a dead [n,256] tensor)
+};
+// Both GEMMs of the layer in one pass over dZ_L and H_{L-1} (bit 2 of g_debug_flags: the wgrad + launch pair).
+int dgrad_wgrad(const BackwardLaunch* groups, int ngroups, int64_t n, cudaStream_t st);
 // Weight packs (one launch for all matrices).  Forward pack: k-block kb (32 input features) = the [256 out x 32 k] tile
 // in the K-major SWIZZLE_64B layout, hi (16 KB) then lo (16 KB).  Dgrad pack: k-block kb (32 OUTPUT features = the
 // reduction index of dZ . W) = four [32 out x 64 in] SWIZZLE_128B groups, hi (16 KB) then lo (16 KB).  Both are what

@@ -11,6 +11,7 @@
 
 #include "common.cuh"
 #include "tc_gemm.cuh"
+#include "tc_half.cuh"
 #include "tma.cuh"
 #include "wgmma.cuh"
 
@@ -38,75 +39,10 @@ constexpr int kRingBytes = kStages * kStageBytes;  // 192 KB
 constexpr int kThreads = 384;
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file");
-constexpr int kWeightScaleLog2 = 10;  // weights are stored as fp16 (hi, lo) of w * 2^10 (|w| <~ 1: both halves normal)
-
-// 1-D bulk copy global -> shared, completion counted on an mbarrier
-__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   tma::smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(tma::smem_u32(bar))
-               : "memory");
-}
-// one warp's share of freeing a ring slot (the barrier counts one arrival per reading warp)
-__device__ __forceinline__ void warp_arrive(uint64_t* bar) {
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) tma::mbar_arrive(bar);
-}
-
-// Operand layouts: K-major SWIZZLE_64B (forward pack: 64-B rows, SBO 512), MN-major SWIZZLE_128B (dgrad pack: SBO 1024 B
-// between 8 K-rows, LBO 4096 B between 64-wide N groups), MN-major SWIZZLE_64B (wgrad H: SBO 512, LBO 2048).
-constexpr uint32_t kSw128 = 1, kSw64 = 2;
 
 __device__ __forceinline__ float tanh_fast(float x) {
   const float t = __expf(-2.0f * fabsf(x));
   return copysignf(__fdividef(1.0f - t, 1.0f + t), x);
-}
-
-// 2^s as a float (s in [-126, 127])
-__device__ __forceinline__ float pow2i(int s) { return __int_as_float((s + 127) << 23); }
-// power-of-two scale that brings max|x| = amax to [2^13, 2^14): fp16 keeps 11 bits for every |x| >= amax * 2^-27
-__device__ __forceinline__ int scale_log2_for(float amax) {
-  const int e = (int)((__float_as_uint(amax) >> 23) & 0xffu) - 127;
-  if (!(amax > 0.0f) || e < -120) return 0;
-  int s = 13 - e;
-  return s > 100 ? 100 : (s < -100 ? -100 : s);
-}
-
-// (x0, x1) -> packed fp16 pairs hi = rn(x), lo = rn(x - hi)
-__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const __half2 hh = __floats2half2_rn(x0, x1);
-  const float2 hf = __half22float2(hh);
-  const __half2 ll = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-  hi = *reinterpret_cast<const uint32_t*>(&hh);
-  lo = *reinterpret_cast<const uint32_t*>(&ll);
-}
-
-// fp32 [R rows x 32 floats] SWIZZLE_128B tile -> fp16 hi / lo [R rows x 32 halfs] SWIZZLE_64B tiles; item = (row, 8 floats)
-template <int NT>
-__device__ __forceinline__ void split_tile(const uint8_t* __restrict__ src, uint8_t* __restrict__ hi, uint8_t* __restrict__ lo,
-                                           int rows, int t, float scale) {
-  const int items = rows * 4;
-#pragma unroll 2
-  for (int i = t; i < items; i += NT) {
-    const int r = i >> 2, cp = i & 3;
-    const uint8_t* srow = src + r * 128;
-    const float4 x0 = *reinterpret_cast<const float4*>(srow + (((2 * cp) ^ (r & 7)) << 4));
-    const float4 x1 = *reinterpret_cast<const float4*>(srow + (((2 * cp + 1) ^ (r & 7)) << 4));
-    const float v[8] = {x0.x * scale, x0.y * scale, x0.z * scale, x0.w * scale,
-                        x1.x * scale, x1.y * scale, x1.z * scale, x1.w * scale};
-    uint32_t h[4], l[4];  // packed half2 words (no 16-byte reinterpretation of a 4-byte-aligned local array)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const __half2 hh = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
-      const float2 hf = __half22float2(hh);
-      const __half2 ll = __floats2half2_rn(v[2 * j] - hf.x, v[2 * j + 1] - hf.y);
-      h[j] = *reinterpret_cast<const uint32_t*>(&hh);
-      l[j] = *reinterpret_cast<const uint32_t*>(&ll);
-    }
-    const int doff = r * 64 + ((cp ^ ((r >> 1) & 3)) << 4);
-    *reinterpret_cast<uint4*>(hi + doff) = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(lo + doff) = make_uint4(l[0], l[1], l[2], l[3]);
-  }
 }
 
 // wgmma A fragment (m64k16, this thread's rows r0 / r0 + 8, k columns c0 + 2t + {0, 1, 8, 9}) of a row-major fp32

@@ -1,5 +1,6 @@
 // sm_90a wgmma wrappers: D[64 x N] (+)= A[64 x 16] . B[16 x N], fp16 in, fp32 accumulators in registers.  Mma: A from
-// registers (the m64k16 fragment of the PTX ISA), B from a descriptor (TB = 1: MN-major).  MmaSS: both K-major descriptors.
+// registers (the m64k16 fragment of the PTX ISA), B from a descriptor (TB = 1: MN-major).  MmaSS: both from descriptors
+// (TA / TB = 1: MN-major; K-major by default).
 // Accumulator fragment: for each 8-column block j, d[4j + {0,1}] = (row g, cols 8j + 2t + {0,1}) and d[4j + {2,3}] =
 // (row g + 8, same cols), rows relative to 16 * (warp % 4), g = lane / 4, t = lane % 4.
 #pragma once
@@ -33,7 +34,7 @@ __device__ __forceinline__ uint64_t desc(uint32_t saddr, uint32_t lbo, uint32_t 
 
 template <int N, int TB>
 struct Mma;
-template <int N>
+template <int N, int TA = 0, int TB = 0>
 struct MmaSS;
 
 template <int TB>
@@ -64,27 +65,40 @@ struct Mma<256, TB> {
   }
 };
 
-template <>
-struct MmaSS<32> {
+template <int TA, int TB>
+struct MmaSS<32, TA, TB> {
   __device__ __forceinline__ static void run(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {"
                  "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
-                 "}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+                 "}, %16, %17, p, 1, 1, %19, %20;\n}\n"
                  : RB_WG_D16(0)
-                 : "l"(a), "l"(b), "r"(scale_d));
+                 : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
   }
 };
 
-template <>
-struct MmaSS<64> {
+template <int TA, int TB>
+struct MmaSS<64, TA, TB> {
   __device__ __forceinline__ static void run(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
                  "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
-                 "}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+                 "}, %32, %33, p, 1, 1, %35, %36;\n}\n"
                  : RB_WG_D16(0), RB_WG_D16(16)
-                 : "l"(a), "l"(b), "r"(scale_d));
+                 : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
+
+template <int TA, int TB>
+struct MmaSS<128, TA, TB> {
+  __device__ __forceinline__ static void run(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+                 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+                 "}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+                 : RB_WG_D64(0)
+                 : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
   }
 };
 
