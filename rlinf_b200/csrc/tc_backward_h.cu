@@ -31,31 +31,34 @@ using rb::tc::BN;
 // stays resident in shared memory: streamed per k-block it is 128 KB of L2 reads per 48 KB of activations, and a
 // ring small enough to fit next to the operand tiles leaves the wgmmas waiting on L2 latency.
 // Warpgroups 0 / 1: consumers.  Consumer w owns dW rows [128 w, +128) (two m64n128 accumulators, 128 registers) and
-// dZ_{L-1} columns 128 half + [64 w, +64) (one m64n32 accumulator per k-block, 16 registers).  Warpgroup 2: warp 8 lane 0
-// issues the weight load and the TMA loads of the landing stage; warps 9-11 split the landed fp32 tiles into the fp16
-// operand slot.  The landing stage is free as soon as it is split (the dgrad epilogue reads its H rows from global
-// memory / L2, as tc_h_gemm_kernel<1> does), so the next k-block's TMA overlaps this k-block's wgmmas.
+// dZ_{L-1} columns 128 half + [64 w, +64) (one m64n32 accumulator per k-block, 16 registers; its epilogue runs behind
+// the same k-block's wgrad wgmmas).  Warpgroup 2: warp 8 lane 0 issues the weight load and the TMA loads of the two
+// stages; warps 9-11 split each landed fp32 box into fp16 (hi, lo) in place.  A stage is busy from its TMA until its
+// wgmmas retire (the dgrad epilogue reads its H rows from global memory / L2, as tc_h_gemm_kernel<1> does), so with
+// two stages the TMA and split of k-block i + 1 overlap the wgmmas of k-block i.
 constexpr int kBwThreads = 384;
 constexpr int kBwZ32 = BK * BN * 4;                       // 32 KB: dZ of a k-block, 8 boxes [32 samples x 32 features]
 constexpr int kBwH32 = BK * 128 * 4;                      // 16 KB: the CTA's 128 columns of H, 4 boxes
-constexpr int kBwLandBytes = kBwZ32 + kBwH32;             // 48 KB
-constexpr int kBwZ16 = BK * BN * 2, kBwH16 = BK * 128 * 2;  // 16 KB / 8 KB per fp16 half
-constexpr int kBwOpBytes = 2 * kBwZ16 + 2 * kBwH16;       // 48 KB: dZ hi | dZ lo | H hi | H lo
+constexpr int kBwStageBytes = kBwZ32 + kBwH32;            // 48 KB: 12 boxes of 4 KB, each fp32 as landed, then hi | lo
+constexpr int kBwBox = 4096, kBwLo = 2048;                // box stride; lo half of a split box
 constexpr int kBwW16 = BK * 128 * 2;                      // 8 KB: two 64-column groups of a dgrad-pack k-block, one half
 constexpr int kBwWBytes = 2 * kBwW16;                     // 16 KB per k-block: hi | lo
 constexpr int kBwWAll = (BN / BK) * kBwWBytes;            // 128 KB: the CTA's half of the whole pack
-constexpr int kBwRingBytes = kBwLandBytes + kBwOpBytes + kBwWAll;  // 48 + 48 + 128 KB
+constexpr int kBwRingBytes = 2 * kBwStageBytes + kBwWAll;  // 2 x 48 + 128 KB
 constexpr int kBwSplitThreads = 96;                       // warps 9-11
-constexpr int kBwProducerRegs = 56, kBwConsumerRegs = 224;
-static_assert(128 * kBwProducerRegs + 256 * kBwConsumerRegs <= 65536, "register file");
+// Launched at 168 registers per thread (__launch_bounds__(384, 1)), the CTA can only raise the consumers by what the
+// producers give back; setmaxnreg.inc waits until it can.  A split warp holds a whole box (32 words): 64 producer
+// registers, so 216 for the consumers.
+constexpr int kBwLaunchRegs = 65536 / kBwThreads / 8 * 8;
+constexpr int kBwProducerRegs = 64, kBwConsumerRegs = 216;
+static_assert(128 * (kBwLaunchRegs - kBwProducerRegs) >= 256 * (kBwConsumerRegs - kBwLaunchRegs), "register pool");
 constexpr int64_t kBwSlot = 256 * 256;                    // per (chunk, group) partial of dW
 
 struct BwBarriers {
-  uint64_t full;      // landing stage: TMA tx bytes
-  uint64_t empty;     // landing stage split (one arrival per split warp)
-  uint64_t op_full;   // operand slot written by the split threads (one arrival per thread, after its proxy fence)
-  uint64_t op_empty;  // wgmmas reading the operand slot retired (one arrival per consumer warp)
-  uint64_t w_full;    // resident weights: bulk-copy tx bytes
+  uint64_t full[2];      // stage landed: TMA tx bytes
+  uint64_t op_full[2];   // stage split (one arrival per split thread, after its proxy fence)
+  uint64_t op_empty[2];  // wgmmas reading the stage retired (one arrival per consumer warp)
+  uint64_t w_full;       // resident weights: bulk-copy tx bytes
 };
 
 struct BwParams {
@@ -74,9 +77,7 @@ struct BwParams {
 __global__ void __launch_bounds__(kBwThreads, 1) tc_h_dgrad_wgrad_kernel(const __grid_constant__ BwParams P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tma::smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* land = smem;
-  uint8_t* ops = land + kBwLandBytes;
-  uint8_t* wst = ops + kBwOpBytes;
+  uint8_t* wst = smem + 2 * kBwStageBytes;
   BwBarriers* bars = reinterpret_cast<BwBarriers*>(smem + kBwRingBytes);
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int grp = blockIdx.x % P.ngroups;
@@ -90,29 +91,29 @@ __global__ void __launch_bounds__(kBwThreads, 1) tc_h_dgrad_wgrad_kernel(const _
   const int s_z = P.amax_in[grp] ? scale_log2_for(__ldg(P.amax_in[grp])) : 0;
 
   if (threadIdx.x == 0) {
-    tma::mbar_init(&bars->full, 1);
-    tma::mbar_init(&bars->empty, kBwSplitThreads / 32);
-    tma::mbar_init(&bars->op_full, kBwSplitThreads);
-    tma::mbar_init(&bars->op_empty, 8);
+    for (int s = 0; s < 2; ++s) {
+      tma::mbar_init(&bars->full[s], 1);
+      tma::mbar_init(&bars->op_full[s], kBwSplitThreads);
+      tma::mbar_init(&bars->op_empty[s], 8);
+    }
     tma::mbar_init(&bars->w_full, 1);
     tma::fence_barrier_init();
   }
   __syncthreads();
   if (n_kb <= 0) return;
 
+  // k-block it uses stage it & 1, for the (it >> 1)-th time: its barriers complete phase it >> 1
   if (wg == 2) {
     wg::setmaxnreg_dec<kBwProducerRegs>();
-    if (warp > 8) {  // split: landing stage -> operand slot
+    if (warp > 8) {  // split: warp 9 + w owns boxes w, w + 3, w + 6, w + 9 of a stage (dZ 0-7, H 8-11)
       const float z_scale = pow2i(s_z);
       for (int it = 0; it < n_kb; ++it) {
-        tma::mbar_wait(&bars->full, it & 1u);
-        tma::mbar_wait(&bars->op_empty, (it & 1u) ^ 1u);
-        // [32 samples x 32 floats] boxes (4 KB) -> [32 samples x 32 halfs] (2 KB), contiguous on both sides
-        split_tile<kBwSplitThreads>(land, ops, ops + kBwZ16, BN, threadIdx.x - 288, z_scale);
-        split_tile<kBwSplitThreads>(land + kBwZ32, ops + 2 * kBwZ16, ops + 2 * kBwZ16 + kBwH16, 128, threadIdx.x - 288, 1.0f);
+        uint8_t* st = smem + (it & 1) * kBwStageBytes;
+        tma::mbar_wait(&bars->full[it & 1], (it >> 1) & 1u);
+#pragma unroll 1
+        for (int b = warp - 9; b < 12; b += 3) split_box_in_place(st + b * kBwBox, lane, b < BN / 32 ? z_scale : 1.0f);
         tma::fence_proxy_async();  // generic-proxy stores -> the wgmmas' async-proxy reads
-        tma::mbar_arrive(&bars->op_full);
-        warp_arrive(&bars->empty);
+        tma::mbar_arrive(&bars->op_full[it & 1]);
       }
     } else if (lane == 0) {  // warp 8: loads
       tma::prefetch_desc(&P.z[grp]);
@@ -125,11 +126,13 @@ __global__ void __launch_bounds__(kBwThreads, 1) tc_h_dgrad_wgrad_kernel(const _
         bulk_load(wst + kb * kBwWBytes + kBwW16, wsrc + (size_t)kb * 32768 + 16384, kBwW16, &bars->w_full);
       }
       for (int it = 0; it < n_kb; ++it) {
-        tma::mbar_wait(&bars->empty, (it & 1u) ^ 1u);
-        tma::mbar_arrive_expect_tx(&bars->full, kBwLandBytes);
+        uint8_t* st = smem + (it & 1) * kBwStageBytes;
+        uint64_t* full = &bars->full[it & 1];
+        tma::mbar_wait(&bars->op_empty[it & 1], ((it >> 1) & 1u) ^ 1u);  // wgmmas of k-block it - 2 retired
+        tma::mbar_arrive_expect_tx(full, kBwStageBytes);
         const int m0 = (kb0 + it) * BK;  // samples >= n are zero-filled
-        for (int b = 0; b < BN / 32; ++b) tma::load_2d(land + b * 4096, &P.z[grp], b * 32, m0, &bars->full);
-        for (int b = 0; b < 4; ++b) tma::load_2d(land + kBwZ32 + b * 4096, &P.h[grp], half * 128 + b * 32, m0, &bars->full);
+        for (int b = 0; b < BN / 32; ++b) tma::load_2d(st + b * kBwBox, &P.z[grp], b * 32, m0, full);
+        for (int b = 0; b < 4; ++b) tma::load_2d(st + kBwZ32 + b * kBwBox, &P.h[grp], half * 128 + b * 32, m0, full);
       }
     }
   } else {
@@ -147,31 +150,28 @@ __global__ void __launch_bounds__(kBwThreads, 1) tc_h_dgrad_wgrad_kernel(const _
 #pragma unroll
       for (int i = 0; i < 64; ++i) accw[mt][i] = 0.f;
     float vmax = 0.f;
-    const uint32_t zb = tma::smem_u32(ops), hb = zb + 2 * kBwZ16, wb0 = tma::smem_u32(wst) + wg * 4096;
+    const uint32_t st0 = tma::smem_u32(smem), wb0 = tma::smem_u32(wst) + wg * 4096;
+    // Per k-block, two commit groups: the dgrad wgmmas, then the wgrad wgmmas.  wait<1> retires the dgrad group, and
+    // the dgrad epilogue runs while the wgrad group keeps the tensor cores busy; wait<0> then frees the stage.  Both
+    // groups are drained before the next k-block: with an accumulator of an in-flight group live across the loop's
+    // back-edge, ptxas (CUDA 12.9) serialises every wgmma of the kernel (C7514).
     tma::mbar_wait_brk(&bars->w_full, 0u);
     for (int it = 0; it < n_kb; ++it) {
-      tma::mbar_wait_brk(&bars->op_full, it & 1u);
+      const int64_t m_base = (int64_t)(kb0 + it) * BK;
+      float hv[16];  // the epilogue's H values from L2, loaded before the wgmmas to hide the latency
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int64_t row = m_base + 8 * (i >> 2) + 2 * t + (i & 1);
+        hv[i] = row < P.n ? __ldg(hg + row * BN + c_lo + 8 * ((i >> 1) & 1)) : 0.f;
+      }
+      const uint32_t zb = st0 + (it & 1) * kBwStageBytes, hb = zb + kBwZ32;
+      tma::mbar_wait_brk(&bars->op_full[it & 1], (it >> 1) & 1u);
       float accd[16];
 #pragma unroll
       for (int i = 0; i < 16; ++i) accd[i] = 0.f;
       wg::fence();
-      // wgrad: A = dZ^T (features of this warpgroup, MN-major: 32-feature boxes 2 KB apart, 16 samples = 1 KB),
-      // B = H (the CTA's 128 columns, MN-major)
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {
-        const uint64_t b_hi = wg::desc(hb + k * 1024, 2048, 512, kSw64);
-        const uint64_t b_lo = wg::desc(hb + kBwH16 + k * 1024, 2048, 512, kSw64);
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          const uint32_t za = zb + (4 * wg + 2 * mt) * 2048 + k * 1024;
-          const uint64_t a_hi = wg::desc(za, 2048, 512, kSw64), a_lo = wg::desc(za + kBwZ16, 2048, 512, kSw64);
-          wg::MmaSS<128, 1, 1>::run(accw[mt], a_lo, b_hi, 1u);  // small terms first
-          wg::MmaSS<128, 1, 1>::run(accw[mt], a_hi, b_lo, 1u);
-          wg::MmaSS<128, 1, 1>::run(accw[mt], a_hi, b_hi, 1u);
-        }
-      }
       // dgrad (transposed): A = W^T (this warpgroup's 64 output columns of weight k-block kb, MN-major SW128),
-      // B = dZ (K-major: box kb holds features 32 kb + [0, 32) of the 32 samples)
+      // B = dZ (K-major: box kb holds features 32 kb + [0, 32) of the 32 samples, hi | lo)
 #pragma unroll 1
       for (int kb = 0; kb < BN / BK; ++kb) {
         const uint32_t wb = wb0 + kb * kBwWBytes;
@@ -179,18 +179,33 @@ __global__ void __launch_bounds__(kBwThreads, 1) tc_h_dgrad_wgrad_kernel(const _
         for (int k = 0; k < BK / 16; ++k) {
           const uint64_t a_hi = wg::desc(wb + k * 2048, 4096, 1024, kSw128);
           const uint64_t a_lo = wg::desc(wb + kBwW16 + k * 2048, 4096, 1024, kSw128);
-          const uint64_t b_hi = wg::desc(zb + kb * 2048 + k * 32, 16, 512, kSw64);
-          const uint64_t b_lo = wg::desc(zb + kBwZ16 + kb * 2048 + k * 32, 16, 512, kSw64);
+          const uint64_t b_hi = wg::desc(zb + kb * kBwBox + k * 32, 16, 512, kSw64);
+          const uint64_t b_lo = wg::desc(zb + kb * kBwBox + kBwLo + k * 32, 16, 512, kSw64);
           wg::MmaSS<32, 1, 0>::run(accd, a_hi, b_lo, 1u);  // dZ lo . W hi first, as in the dgrad kernel
           wg::MmaSS<32, 1, 0>::run(accd, a_lo, b_hi, 1u);
           wg::MmaSS<32, 1, 0>::run(accd, a_hi, b_hi, 1u);
         }
       }
       wg::commit();
-      wg::wait<0>();
-      warp_arrive(&bars->op_empty);
+      // wgrad: A = dZ^T (features of this warpgroup, MN-major: 32-feature boxes 4 KB apart, 16 samples = 1 KB),
+      // B = H (the CTA's 128 columns, MN-major)
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t b_hi = wg::desc(hb + k * 1024, kBwBox, 512, kSw64);
+        const uint64_t b_lo = wg::desc(hb + kBwLo + k * 1024, kBwBox, 512, kSw64);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+          const uint32_t za = zb + (4 * wg + 2 * mt) * kBwBox + k * 1024;
+          const uint64_t a_hi = wg::desc(za, kBwBox, 512, kSw64), a_lo = wg::desc(za + kBwLo, kBwBox, 512, kSw64);
+          wg::MmaSS<128, 1, 1>::run(accw[mt], a_lo, b_hi, 1u);  // small terms first
+          wg::MmaSS<128, 1, 1>::run(accw[mt], a_hi, b_lo, 1u);
+          wg::MmaSS<128, 1, 1>::run(accw[mt], a_hi, b_hi, 1u);
+        }
+      }
+      wg::commit();
+      wg::wait<1>();
+      wg::fence_operand(accd);
       // ---- dgrad epilogue: accd[4j + 2hh + e] = (column c_lo + 8 hh, sample 8j + 2t + e) ----
-      const int64_t m_base = (int64_t)(kb0 + it) * BK;
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int c = c_lo + 8 * hh;
@@ -201,7 +216,7 @@ __global__ void __launch_bounds__(kBwThreads, 1) tc_h_dgrad_wgrad_kernel(const _
           for (int e = 0; e < 2; ++e) {
             const int64_t row = m_base + 8 * j + 2 * t + e;
             const bool ok = row < P.n;
-            const float h = ok ? __ldg(hg + row * BN + c) : 0.f;
+            const float h = hv[4 * j + 2 * hh + e];
             float x = accd[4 * j + 2 * hh + e] * dgrad_scale;
             x = ok ? x * (1.0f - h * h) : 0.f;
             vmax = fmaxf(vmax, fabsf(x));
@@ -221,7 +236,11 @@ __global__ void __launch_bounds__(kBwThreads, 1) tc_h_dgrad_wgrad_kernel(const _
           }
         }
       }
+      wg::wait<0>();
+      warp_arrive(&bars->op_empty[it & 1]);
     }
+    wg::fence_operand(accw[0]);
+    wg::fence_operand(accw[1]);
     // ---- dW partial of the chunk (this CTA's columns) ----
     float* slot = P.part + (size_t)(chunk * P.ngroups + grp) * kBwSlot;
 #pragma unroll

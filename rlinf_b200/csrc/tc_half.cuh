@@ -47,7 +47,20 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
   lo = *reinterpret_cast<const uint32_t*>(&ll);
 }
 
-// fp32 [R rows x 32 floats] SWIZZLE_128B tile -> fp16 hi / lo [R rows x 32 halfs] SWIZZLE_64B tiles; item = (row, 8 floats)
+// One split item = (row r, 8 floats cp of its 32): the two 16-byte chunks of fp32 row r (SWIZZLE_128B, 128-B rows) ->
+// one 16-byte chunk each of fp16 hi and lo row r (SWIZZLE_64B, 64-B rows), as packed half2 words of x * scale
+__device__ __forceinline__ void split_item(const uint8_t* src, int r, int cp, float scale, uint4& hi, uint4& lo) {
+  const uint8_t* srow = src + r * 128;
+  const float4 x0 = *reinterpret_cast<const float4*>(srow + (((2 * cp) ^ (r & 7)) << 4));
+  const float4 x1 = *reinterpret_cast<const float4*>(srow + (((2 * cp + 1) ^ (r & 7)) << 4));
+  split2(x0.x * scale, x0.y * scale, hi.x, lo.x);
+  split2(x0.z * scale, x0.w * scale, hi.y, lo.y);
+  split2(x1.x * scale, x1.y * scale, hi.z, lo.z);
+  split2(x1.z * scale, x1.w * scale, hi.w, lo.w);
+}
+__device__ __forceinline__ int split_item_dst(int r, int cp) { return r * 64 + ((cp ^ ((r >> 1) & 3)) << 4); }
+
+// fp32 [R rows x 32 floats] SWIZZLE_128B tile -> fp16 hi / lo [R rows x 32 halfs] SWIZZLE_64B tiles
 template <int NT>
 __device__ __forceinline__ void split_tile(const uint8_t* __restrict__ src, uint8_t* __restrict__ hi, uint8_t* __restrict__ lo,
                                            int rows, int t, float scale) {
@@ -55,23 +68,26 @@ __device__ __forceinline__ void split_tile(const uint8_t* __restrict__ src, uint
 #pragma unroll 2
   for (int i = t; i < items; i += NT) {
     const int r = i >> 2, cp = i & 3;
-    const uint8_t* srow = src + r * 128;
-    const float4 x0 = *reinterpret_cast<const float4*>(srow + (((2 * cp) ^ (r & 7)) << 4));
-    const float4 x1 = *reinterpret_cast<const float4*>(srow + (((2 * cp + 1) ^ (r & 7)) << 4));
-    const float v[8] = {x0.x * scale, x0.y * scale, x0.z * scale, x0.w * scale,
-                        x1.x * scale, x1.y * scale, x1.z * scale, x1.w * scale};
-    uint32_t h[4], l[4];  // packed half2 words (no 16-byte reinterpretation of a 4-byte-aligned local array)
+    uint4 h, l;
+    split_item(src, r, cp, scale, h, l);
+    *reinterpret_cast<uint4*>(hi + split_item_dst(r, cp)) = h;
+    *reinterpret_cast<uint4*>(lo + split_item_dst(r, cp)) = l;
+  }
+}
+
+// One warp: a landed fp32 [32 rows x 32 floats] SWIZZLE_128B box (4 KB) split over itself - fp16 hi [32 x 32 halfs]
+// SWIZZLE_64B in its first 2 KB, lo in the second.  A (hi, lo) pair takes the 4 bytes of its float, so it fits; every
+// lane holds its 4 items in registers until the whole warp has read the box.
+__device__ __forceinline__ void split_box_in_place(uint8_t* box, int lane, float scale) {
+  uint4 h[4], l[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const __half2 hh = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
-      const float2 hf = __half22float2(hh);
-      const __half2 ll = __floats2half2_rn(v[2 * j] - hf.x, v[2 * j + 1] - hf.y);
-      h[j] = *reinterpret_cast<const uint32_t*>(&hh);
-      l[j] = *reinterpret_cast<const uint32_t*>(&ll);
-    }
-    const int doff = r * 64 + ((cp ^ ((r >> 1) & 3)) << 4);
-    *reinterpret_cast<uint4*>(hi + doff) = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(lo + doff) = make_uint4(l[0], l[1], l[2], l[3]);
+  for (int j = 0; j < 4; ++j) split_item(box, (lane >> 2) + 8 * j, lane & 3, scale, h[j], l[j]);
+  __syncwarp();
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int d = split_item_dst((lane >> 2) + 8 * j, lane & 3);
+    *reinterpret_cast<uint4*>(box + d) = h[j];
+    *reinterpret_cast<uint4*>(box + 2048 + d) = l[j];
   }
 }
 

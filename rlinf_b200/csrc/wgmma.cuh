@@ -13,6 +13,13 @@ __device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned
 __device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins accumulator registers here: volatile asm keeps its order, so reads of a wgmma's results placed after the wait
+// that retires it are not scheduled above that wait (where ptxas would serialise the wgmmas to make them safe).
+template <int N>
+__device__ __forceinline__ void fence_operand(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 // warpgroup register reallocation (every warp of the warpgroup executes the same one): a producer warpgroup gives
 // registers back to the pool, the consumer warpgroups take them (R: multiple of 8 in [24, 256])
