@@ -36,6 +36,24 @@ constexpr int kThreads = 13 * 32;
 constexpr int kWScaleLog2 = 10;  // weights are stored as fp16 (hi, lo) of w * 2^10
 constexpr float kHalfLog2Pi = 0.91893853320467274178f;
 
+// Cycle probe, off by default (-DRB200_ROLLOUT_TC_PROBE, built and read by tools/rollout_tc_probe.py): clock64() sums
+// per CTA over the rollout, one 8-byte slot each.  Waits are summed by the waiting thread (the producer lane, thread 0
+// of each consumer warpgroup); kT* slots are sums over steps t < T of (stamp - the step's obs-ready stamp).
+#ifdef RB200_ROLLOUT_TC_PROBE
+#define TC_PROBE(...) __VA_ARGS__
+enum ProbeSlot {
+  kPrEmptyWait, kPrEmptyPolls, kPrStages,  // producer: cycles in unsuccessful empty waits, their number, stages issued
+  kPwEnvFull, kPwActFull, kPwValFull,      // consumer waits on full (env, actor, value warpgroup: tid >> 7)
+  kTActTower, kTSample,                    // actor: tower done, actions sampled (thread 128)
+  kTEnvProduct, kTEnvVhead, kTObsReady,    // env: x.W_s done, value head seen, next observation ready (thread 0)
+  kTValTower, kTValHead,                   // value: tower done, head done (thread 256)
+  kTSteps, kProbeSlots
+};
+__device__ unsigned long long* g_tc_probe;  // [grid][kProbeSlots]
+#else
+#define TC_PROBE(...)
+#endif
+
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr int kOffRing = 0;
 constexpr int kOffObuf = kOffRing + kStages * kStageBytes;  // [hi|lo][kb<=4][64 rows][64 B]: rows 0-31 obs, 32-63 final obs
@@ -58,6 +76,7 @@ struct Misc {
   int nflag;
   uint64_t full[kStages], empty[kStages];
   uint64_t vhead, obs_ready;
+  TC_PROBE(unsigned long long probe[kProbeSlots]; long long t_obs;)
 };
 constexpr int kArgsBytes = 512;  // shared-memory copy of the kernel arguments for the out-of-line helpers
 constexpr int kOffArgs = kOffMisc + (((int)sizeof(Misc) + 15) & ~15);
@@ -406,7 +425,9 @@ __device__ __forceinline__ void layer_mma(LayerAcc<N, NT>& acc, Misc* ms, uint32
     for (int m = 0; m < NT; ++m) {
       const uint32_t idx = stage0 + (uint32_t)(kb * NT + m);
       const uint32_t slot = (uint32_t)slot0 + idx % (uint32_t)nslots, ph = (idx / (uint32_t)nslots) & 1u;
+      TC_PROBE(const long long pt0 = clock64();)
       mbar_wait(&ms->full[slot], ph);
+      TC_PROBE(if ((threadIdx.x & 127) == 0) ms->probe[kPwEnvFull + (threadIdx.x >> 7)] += clock64() - pt0;)
       const uint32_t a = ring_a + slot * kStageBytes;
       rb::wg::fence();
 #pragma unroll
@@ -511,6 +532,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
     mbar_init(&ms->vhead, 4);
     mbar_init(&ms->obs_ready, 1);
     ms->nflag = 0;
+    TC_PROBE(for (int s = 0; s < kProbeSlots; ++s) ms->probe[s] = 0ull; ms->t_obs = clock64();)
     rb::tma::fence_barrier_init();
   }
   const int Cn = kChunk ? p.C : 1;
@@ -543,7 +565,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
   // per-step stream lengths (in stages) of the three consumers: env product, actor tower, value tower
   const uint32_t n_env = (uint32_t)sg.nkb0, n_tower = 2u * (uint32_t)sg.nkb0 + 32u;
   if (warp == 12) {
-    // ================= weight-stream producer: three rings, polled (no ring waits for another) =================
+    // ======== weight-stream producer: three rings, polled with test_wait (no ring waits for another) ========
     if (lane == 0) {
       const uint32_t total[3] = {(uint32_t)(T * Cn) * n_env, (uint32_t)T * n_tower, (uint32_t)(T + 1) * n_tower};
       const int slot0[3] = {kEnvSlot0, kActSlot0, kValSlot0}, nslots[3] = {kEnvSlots, kActSlots, kValSlots};
@@ -553,7 +575,12 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
         for (int q = 0; q < 3; ++q) {
           if (j[q] >= total[q]) continue;
           const uint32_t slot = (uint32_t)slot0[q] + j[q] % (uint32_t)nslots[q], ph = (j[q] / (uint32_t)nslots[q]) & 1u;
-          if (!rb::tma::mbar_try_wait(&ms->empty[slot], ph ^ 1u)) continue;
+          TC_PROBE(const long long pt0 = clock64();)
+          if (!rb::tma::mbar_test_wait(&ms->empty[slot], ph ^ 1u)) {
+            TC_PROBE(ms->probe[kPrEmptyWait] += clock64() - pt0; ++ms->probe[kPrEmptyPolls];)
+            continue;
+          }
+          TC_PROBE(++ms->probe[kPrStages];)
           // pack stage of position j in this stream (pack order: env, a0, v0, a1, v1, a2, v2)
           int stage;
           if (q == 0) {
@@ -580,6 +607,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
         mbar_wait(&ms->obs_ready, p_obs);
         p_obs ^= 1u;
       }
+      TC_PROBE(const long long t_obs = *reinterpret_cast<volatile long long*>(&ms->t_obs);)
       const uint32_t base = (uint32_t)t * n_tower, l0 = 2u * (uint32_t)sg.nkb0;
       tower_layer<kNE>(ms, ring_a, kActSlot0, base, sg.nkb0, obuf_a, ob_half, 4096u, bias[0], abuf, kAbufHalf, 2048u, 0, 1, w,
                        lane);
@@ -587,6 +615,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
                        w, lane);
       tower_layer<kNE>(ms, ring_a, kActSlot0, base + l0 + 16, 8, abuf_a, kAbufHalf, 2048u, bias[2], abuf, kAbufHalf, 2048u, 1,
                        1, w, lane);
+      TC_PROBE(if (gt == 0) ms->probe[kTActTower] += clock64() - t_obs;)
       if constexpr (kChunk) {
         // ---- chunked mean head [C*A, 256] from L2: warp w takes actions w, w+4, ..., its weight row in registers,
         //      one warp-reduced dot product per environment; lane e then samples (e, a) ----
@@ -658,6 +687,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
         }
       }
       }
+      TC_PROBE(if (gt == 0) ms->probe[kTSample] += clock64() - t_obs;)
       // ---- env finish, shared with the env warps (barrier 4 = actor + env groups): #1 actions sampled / h3 dead,
       //      #2 zs + eps in the actor buffer, #3 next observation operand complete (#2 and #3 once per sub-step) ----
       named_sync(4, 256);
@@ -684,6 +714,8 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
       // the value tower runs with N = 64 columns when any environment was flagged for the truncation bootstrap
       // (columns 32..63 = its pre-reset observation)
       const int nv = (*reinterpret_cast<volatile int*>(&ms->nflag) > 0) ? 2 * kNE : kNE;
+      TC_PROBE(const long long t_obs = *reinterpret_cast<volatile long long*>(&ms->t_obs);
+               const bool pr = (tid & 127) == 0 && t < T;)
       const uint32_t s0 = (uint32_t)t * n_tower, s1 = s0 + 2u * (uint32_t)sg.nkb0, s2 = s1 + 16u;
       if (nv == kNE) {
         tower_layer<kNE>(ms, ring_a, kValSlot0, s0, sg.nkb0, obuf_a, ob_half, 4096u, bias[0], vbuf, kVbufHalf, 4096u, 0, 2, w, lane);
@@ -694,6 +726,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
         tower_layer<2 * kNE>(ms, ring_a, kValSlot0, s1, 8, vbuf_a, kVbufHalf, 4096u, bias[1], vbuf, kVbufHalf, 4096u, 0, 2, w, lane);
         tower_layer<2 * kNE>(ms, ring_a, kValSlot0, s2, 8, vbuf_a, kVbufHalf, 4096u, bias[2], vbuf, kVbufHalf, 4096u, 1, 2, w, lane);
       }
+      TC_PROBE(if (pr) ms->probe[kTValTower] += clock64() - t_obs;)
       // ---- value head (columns 0..31: V(obs_t)) and bootstrap (columns 32..63: V(final_obs_{t-1}) where flagged) ----
       //      chunked: C outputs per environment, the bootstrap uses output 0 and goes to the chunk's last column
       if constexpr (kChunk) {
@@ -730,6 +763,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
       }
       }
       __syncwarp();
+      TC_PROBE(if (pr) ms->probe[kTValHead] += clock64() - t_obs;)
       if (lane == 0) mbar_arrive(&ms->vhead);
     }
   } else {
@@ -769,6 +803,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
       // ---- 2. x.W_s of this step (the observation operand is complete: barrier #3 of the previous step) ----
       LayerAcc<kNE, 1> zacc;
       layer_mma<kNE, 1>(zacc, ms, ring_a, kEnvSlot0, kEnvSlots, (uint32_t)t * n_env, sg.nkb0, obuf_a, ob_half, 4096u, lane);
+      TC_PROBE(if (gt == 0 && sub == 0) ms->probe[kTEnvProduct] += clock64() - ms->t_obs;)
       // ---- 3. wait for the value head, meet the actor group (#1: h3 dead, actions sampled), then park x.W_s
       //         (fp32 [32][obs]) and this step's draws in the free actor buffer ----
       //         (chunked: at the first sub-step; the later ones overwrite only the actor buffer and the observation
@@ -776,6 +811,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
       if (sub == 0) {
         mbar_wait(&ms->vhead, p_vh);  // the value head of this step has consumed flag / rew of the previous step
         p_vh ^= 1u;
+        TC_PROBE(if (gt == 0) ms->probe[kTEnvVhead] += clock64() - ms->t_obs;)
         named_sync(4, 256);
       }
 #pragma unroll
@@ -810,6 +846,8 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
         int n = 0;
         for (int e = 0; e < kNE; ++e) n += ms->flag[e];
         ms->nflag = n;
+        TC_PROBE(const long long now = clock64(); ms->probe[kTObsReady] += now - ms->t_obs; ++ms->probe[kTSteps];
+                 ms->t_obs = now;)
         __threadfence_block();
         mbar_arrive(&ms->obs_ready);
       }
@@ -818,6 +856,7 @@ __global__ void __launch_bounds__(kThreads, 1) rollout_tc_kernel(const TcArgs p,
     if constexpr (kStats)
       if (gt < nE) es.ret[e0 + gt] = stats_smem<kChunk>(ms)->ret[gt];
   }
+  TC_PROBE(__syncthreads(); if (tid < kProbeSlots) g_tc_probe[blockIdx.x * kProbeSlots + tid] = ms->probe[tid];)
 }
 
 // ---- weight packing: fp32 parameters -> the streamed [stage][hi|lo][128 rows x 32 k] SWIZZLE_64B fp16 tiles --------------
@@ -948,6 +987,15 @@ int launch_rollout_tc(const rb200_mlp_layout* L, const float* params, const void
   RB_RETURN_LAUNCH();
 }
 }  // namespace
+
+#ifdef RB200_ROLLOUT_TC_PROBE
+// probe builds only: where the next rollout_tc_kernel launches write their slots ([grid][slots] uint64, device memory)
+extern "C" int rb200_rollout_tc_probe_buffer(unsigned long long* buf) {
+  RB_CHECK_CUDA(cudaMemcpyToSymbol(g_tc_probe, &buf, sizeof(buf)));
+  return RB200_OK;
+}
+extern "C" int rb200_rollout_tc_probe_slots() { return kProbeSlots; }
+#endif
 
 extern "C" int rb200_rollout_tc(const rb200_mlp_layout* L, const float* params, const void* pack,
                                 const rb200_rollout_args* a, rb200_stream_t stream) {
