@@ -308,7 +308,14 @@ int rb200_mlp_prepare_weights(const rb200_mlp_layout* L, const float* params, fl
 int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params, const float* wsplit,
                       const float* states, const float* action, const int64_t* idx, int64_t n,
                       float* logprobs, float* entropy, float* values, float* acts, float* work,
-                      rb200_stream_t stream);
+                      const float* states_amax, rb200_stream_t stream);
+/* Layer 0 on the tensor cores scales the fp16 split of the states by powers of two where their range calls for it (any
+ * finite observations keep fp32-level accuracy): by max|states| in the forward and by the max of each column in the
+ * weight gradient.  states_amax: device maxima of the rows' batch as rb200_absmax writes them (4 + obs floats for
+ * obs <= 256, else 1), e.g. over the whole batch once per update; NULL: rb200_mlp_forward computes them (one pass over
+ * the rows).  rb200_absmax: out[0] = max|x| of x [rows, cols] (16-byte aligned, cols % 4 == 0) and, for cols <= 256,
+ * out[4 + c] = max|x[:, c]|. */
+int rb200_absmax(const float* x, int64_t rows, int cols, float* out, rb200_stream_t stream);
 
 /* Backward: given d_logprobs [n,act], d_entropy [n,act] or NULL, d_values [n,value_dim] or NULL,
  * ACCUMULATES (+=) parameter gradients into grads (flat, same layout). `acts` from forward. */

@@ -100,6 +100,10 @@ class EmbodiedActor:
         self._static_batch: dict = {}
         self._step_graphs: dict = {}
         self._train_calls = 0
+        # maxima of |states| over the update batch (one pass per run_training), by which layer 0 on the tensor cores scales
+        # its fp16 split; a fixed buffer, so captured optimiser-step graphs read the current batch's values
+        self._states_amax = torch.zeros(4 + m.obs_dim if m.obs_dim <= 256 else 1, dtype=torch.float32,
+                                        device=self.device) if m.obs_dim % 32 == 0 else None
 
     # ---- rollout intake ---------------------------------------------------------------------------
     def recv_rollout_trajectories(self, batch: dict) -> None:
@@ -187,6 +191,8 @@ class EmbodiedActor:
         if graphed:
             batch = self._persist_batch(batch)
             self.rollout_batch = batch
+        if self._states_amax is not None:
+            ops.absmax(batch["forward_inputs"]["states"], out=self._states_amax)
         for _ in range(update_epoch):
             for gb in range(n_global):
                 if graphed:
@@ -298,7 +304,7 @@ class EmbodiedActor:
         ent_bonus = float(cfg.algorithm.get("entropy_bonus", 0) or 0)
         warm = self.optimizer_steps < self.critic_warmup_steps
         out = self.model.forward_train(fi["states"][lo:hi], fi["action"][lo:hi], compute_entropy=ent_bonus > 0,
-                                       compute_values=with_critic)
+                                       compute_values=with_critic, states_amax=self._states_amax)
         A = cfg.actor.model.get("action_dim", 7)
         Cc = out["logprobs"].shape[1] // A
         U = 1 if cfg.algorithm.logprob_type == "chunk_level" else Cc

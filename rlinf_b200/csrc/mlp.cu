@@ -39,6 +39,34 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ Z
   }
 }
 
+// max|x| of a row-major [rows, 4 * cols4] matrix: out[0] = max(out[0], max |x|) and, with cols, out[4 + c] =
+// max(out[4 + c], max over rows |x[:, c]|).  Non-negative floats order like their bit patterns, so the results do not
+// depend on the order of the atomics.  The block size is a multiple of cols4 and so is the grid stride: every thread
+// keeps one column group of 4.
+__global__ void __launch_bounds__(256) absmax_kernel(const float4* __restrict__ x, int64_t n4, int cols4, int cols,
+                                                     float* __restrict__ out) {
+  __shared__ unsigned int s_col[256];
+  __shared__ unsigned int s_all;
+  for (int c = threadIdx.x; c < 256; c += blockDim.x) s_col[c] = 0u;
+  if (threadIdx.x == 0) s_all = 0u;
+  __syncthreads();
+  float4 m = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    const float4 v = __ldg(x + i);
+    m.x = fmaxf(m.x, fabsf(v.x)); m.y = fmaxf(m.y, fabsf(v.y)); m.z = fmaxf(m.z, fabsf(v.z)); m.w = fmaxf(m.w, fabsf(v.w));
+  }
+  atomicMax(&s_all, __float_as_uint(fmaxf(fmaxf(m.x, m.y), fmaxf(m.z, m.w))));
+  if (cols) {
+    const int c0 = 4 * (threadIdx.x % cols4);
+    atomicMax(&s_col[c0], __float_as_uint(m.x)); atomicMax(&s_col[c0 + 1], __float_as_uint(m.y));
+    atomicMax(&s_col[c0 + 2], __float_as_uint(m.z)); atomicMax(&s_col[c0 + 3], __float_as_uint(m.w));
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_all) atomicMax(reinterpret_cast<unsigned int*>(out), s_all);
+  for (int c = threadIdx.x; c < cols; c += blockDim.x)
+    if (s_col[c]) atomicMax(reinterpret_cast<unsigned int*>(out + 4 + c), s_col[c]);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Fused heads.  One warp per sample row; H = 256 hidden units -> 8 per lane (two float4).
 // ------------------------------------------------------------------------------------------------
@@ -472,13 +500,54 @@ struct TowerIO {  // one tower of a grouped forward / backward
   float* amax;                                       // backward: [3] max|dZ3|, max|dZ2|, max|dZ1| (device)
 };
 
-// X -> H1 -> H2 -> H3 for `nt` towers sharing the input X
-int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, TowerIO* t, int nt, cudaStream_t st) {
+// Layer 0 on the tensor cores: the observations X are not bounded like the tanh outputs of the hidden layers.  max|X|
+// and, for obs <= 256, the max of every column are published into the x_amax slot.  Where such a max lies outside
+// [2^-1, 2^15), the fp16 split of X is scaled by a power of two (rb::tch::input_scale_log2_for): by max|X| in the forward,
+// whose products sum over all of a row, and column by column in the backward's weight gradient, whose column c only sees
+// column c of X.  Without that, |x| >= 65520 turns into inf, and small inputs lose low bits to fp16 subnormals.  Inside the
+// range the unscaled split is fp32-accurate already and is kept, bit for bit.
+bool layer0_on_tc(const int64_t* idx, int in_dim) { return idx == nullptr && in_dim % rb::tc::BK == 0; }
+
+// the max|X| slot, behind the six activation tensors and the saved mean (in the spare floats of
+// rb200_mlp_fwd_scratch_floats), in `acts` of the training forward and in `work` of the inference entries:
+// [0] max|X|, [4 + c] max|X[:, c]| for obs <= 256
+float* x_amax_slot(const rb200_mlp_layout* L, float* buf, int64_t n) { return buf + 6 * n * kH + n * L->act_dim; }
+int64_t x_amax_floats(int cols) { return cols <= 256 ? 4 + cols : 1; }
+
+int publish_absmax(const float* X, int64_t rows, int cols, float* out, cudaStream_t st) {
+  if (reinterpret_cast<uintptr_t>(X) & 15) return RB200_E_ALIGN;  // as the TMA descriptor of the GEMM requires
+  if (cols % 4 != 0) return RB200_E_SHAPE;
+  cudaError_t ce = cudaMemsetAsync(out, 0, sizeof(float) * x_amax_floats(cols), st);
+  if (ce != cudaSuccess) return (int)ce;
+  const int cols4 = cols / 4, col_out = cols <= 256 ? cols : 0;
+  const int threads = col_out ? cols4 * (256 / cols4) : 256;
+  const int64_t n4 = rows * cols4;
+  int64_t blocks = (n4 + threads - 1) / threads;
+  const int64_t cap = (int64_t)rb::sm_count() * 4;
+  if (blocks > cap) blocks = cap;
+  absmax_kernel<<<(int)(blocks < 1 ? 1 : blocks), threads, 0, st>>>(reinterpret_cast<const float4*>(X), n4,
+                                                                    col_out ? cols4 : 1, col_out, out);
+  rb::count_launch();
+  ce = cudaPeekAtLastError();
+  return ce == cudaSuccess ? 0 : (int)ce;
+}
+
+// X -> H1 -> H2 -> H3 for `nt` towers sharing the input X.  x_amax_in: caller-provided maxima in the x_amax slot's
+// layout (e.g. over the whole batch the micro-batch is cut from, computed once by rb200_absmax), or NULL: this call
+// computes them itself.
+int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, TowerIO* t, int nt, float* x_amax,
+                     const float* x_amax_in, cudaStream_t st) {
   int e;
-  const bool l0_tc = idx == nullptr && (in_dim % rb::tc::BK == 0);
+  const bool l0_tc = layer0_on_tc(idx, in_dim);
   rb::tch::GemmLaunch g[2];
   if (l0_tc) {
-    for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{X, t[i].wh.w0f, nullptr, t[i].H1, t[i].w.b0, nullptr, nullptr, nullptr, nullptr};
+    if (x_amax_in) {
+      cudaError_t ce = cudaMemcpyAsync(x_amax, x_amax_in, sizeof(float) * x_amax_floats(in_dim), cudaMemcpyDeviceToDevice, st);
+      if (ce != cudaSuccess) return (int)ce;
+    } else if ((e = publish_absmax(X, n, in_dim, x_amax, st))) {
+      return e;
+    }
+    for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{X, t[i].wh.w0f, nullptr, t[i].H1, t[i].w.b0, nullptr, nullptr, nullptr, nullptr, x_amax};
     if ((e = rb::tch::launch(g, nt, n, in_dim, rb::tc::EPI_BIAS_TANH, 0, st))) return e;
   } else {
     for (int i = 0; i < nt; ++i)
@@ -490,8 +559,21 @@ int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, 
   return rb::tch::launch(g, nt, n, kH, rb::tc::EPI_BIAS_TANH, 0, st);
 }
 
-// backward through the hidden layers of `nt` towers given their dZ3 (and max|dZ3| in amax[0])
-int towers_backward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, TowerIO* t, int nt, cudaStream_t st) {
+// Row chunks of the SIMT layer-0 weight gradient: a function of n and the device only, so the chunk-order sum is the
+// same in every run (at most SMs / 2 chunks, as rb::tch::wgrad, and at least 256 rows each).
+int simt_wgrad_chunks(int64_t n, int64_t* rows_per_chunk) {
+  int64_t chunks = (n + 255) / 256;
+  const int64_t cap = rb::sm_count() / 2 > 1 ? rb::sm_count() / 2 : 1;
+  if (chunks > cap) chunks = cap;
+  const int64_t rows = (n + chunks - 1) / chunks;
+  *rows_per_chunk = rows;
+  return (int)((n + rows - 1) / rows);  // every chunk non-empty: each stores its slab
+}
+
+// backward through the hidden layers of `nt` towers given their dZ3 (and max|dZ3| in amax[0]); x_amax: the slot
+// of maxima of X as the forward published it (read when layer 0 runs on the tensor cores)
+int towers_backward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, TowerIO* t, int nt,
+                      const float* x_amax, cudaStream_t st) {
   int e;
   rb::tch::WgradLaunch w[2];
   rb::tch::BackwardLaunch b[2];
@@ -506,17 +588,29 @@ int towers_backward_h(const float* X, const int64_t* idx, int64_t n, int in_dim,
                                    const_cast<float*>(t[i].dZ3)};
   if ((e = rb::tch::dgrad_wgrad(b, nt, n, st))) return e;
   // layer 0: dW0 += dZ1^T . X
-  if (idx == nullptr && (in_dim % rb::tc::BK == 0) && in_dim <= 256) {
-    for (int i = 0; i < nt; ++i) w[i] = rb::tch::WgradLaunch{t[i].tB, X, t[i].g_w0, t[i].amax + 2};
+  if (layer0_on_tc(idx, in_dim) && in_dim <= 256) {
+    for (int i = 0; i < nt; ++i) w[i] = rb::tch::WgradLaunch{t[i].tB, X, t[i].g_w0, t[i].amax + 2, x_amax + 4};
     return rb::tch::wgrad(w, nt, n, in_dim, st);
   }
-  const int64_t rows_per_split = 4096;
-  const int splits = (int)((n + rows_per_split - 1) / rows_per_split);
-  for (int i = 0; i < nt; ++i) {
+  // SIMT: each row chunk stores its own [256, in_dim] partial, summed into dW in chunk order (deterministic)
+  int64_t rows = 0;
+  const int chunks = simt_wgrad_chunks(n, &rows);
+  const int64_t slab = (int64_t)kH * in_dim;
+  float* part = rb::partials_scratch(chunks * slab);
+  if (!part) return RB200_E_UNSUPPORTED;
+  for (int i = 0; i < nt; ++i) {  // one tower at a time: the partials scratch holds one tower's slabs
     GemmArgs a{};
-    a.A = t[i].tB; a.lda = kH; a.B = X; a.ldb = in_dim; a.b_rows = idx; a.C = t[i].g_w0;
-    a.ldc = in_dim; a.M = kH; a.N = in_dim; a.K = n; a.k_per_split = rows_per_split;
-    if ((e = launch_gemm<A_MCONTIG, B_NCONTIG, EPI_ATOMIC>(a, splits, st))) return e;
+    a.A = t[i].tB; a.lda = kH; a.B = X; a.ldb = in_dim; a.b_rows = idx; a.C = part; a.c_split_stride = slab;
+    a.ldc = in_dim; a.M = kH; a.N = in_dim; a.K = n; a.k_per_split = rows;
+    if ((e = launch_gemm<A_MCONTIG, B_NCONTIG, EPI_STORE>(a, chunks, st))) return e;
+    rb::tch::SlotSums ss{};
+    ss.count = 1;
+    ss.nslab = chunks;
+    ss.stride = slab;
+    ss.part[0] = part;
+    ss.out[0] = t[i].g_w0;
+    ss.len[0] = (int)slab;
+    if ((e = rb::tch::sum_slots(ss, st))) return e;
   }
   return 0;
 }
@@ -545,10 +639,10 @@ extern "C" int rb200_mlp_layout_init(rb200_mlp_layout* L, int obs_dim, int act_d
   L->mw = take((int64_t)act_dim * hidden); L->mb = take(act_dim);
   L->total = (o + 3) & ~int64_t(3);
   // size the per-CTA partial-sum scratch of the backward for this layout now, outside any CUDA-graph capture (largest
-  // of: head_bwd <= 4 blocks per SM, wgrad <= SMs / 2 chunk slots of 256 x 256 (+ <= SMs dgrad column-sum slots
-  // of 256 in the fused dgrad_wgrad), dgrad column sums); no device: no-op
+  // of: head_bwd <= 4 blocks per SM, wgrad <= SMs / 2 chunk slots of 256 x max(256, obs) (+ <= SMs dgrad column-sum
+  // slots of 256 in the fused dgrad_wgrad), dgrad column sums); no device: no-op
   const int64_t sms = rb::sm_count(), head = 4 * sms * ((act_dim + value_dim) * hidden + 64 + 2 * hidden);
-  const int64_t wg = sms / 2 * hidden * hidden + sms * hidden;
+  const int64_t wg = sms / 2 * hidden * (obs_dim > hidden ? obs_dim : hidden) + sms * hidden;
   if (!rb::partials_scratch(head > wg ? head : wg)) (void)cudaGetLastError();
   return RB200_OK;
 }
@@ -559,7 +653,7 @@ static inline int64_t act_floats(int64_t n) { return n * kH; }
 
 extern "C" int64_t rb200_mlp_fwd_scratch_floats(const rb200_mlp_layout* L, int64_t n) {
   if (!L || n <= 0) return 0;
-  return 6 * act_floats(n) + n * L->act_dim + 64;
+  return 6 * act_floats(n) + n * L->act_dim + 64 + 256;  // the tail holds the x_amax slot
 }
 
 // wsplit: the fp16-split weight cache, per tower (value tower first, then backbone), 4 bytes (hi + lo) per weight:
@@ -626,7 +720,7 @@ extern "C" int rb200_mlp_prepare_weights(const rb200_mlp_layout* L, const float*
 extern "C" int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params, const float* wsplit,
                                  const float* states, const float* action, const int64_t* idx, int64_t n,
                                  float* logprobs, float* entropy, float* values, float* acts, float* work,
-                                 rb200_stream_t stream) {
+                                 const float* states_amax, rb200_stream_t stream) {
   int e = check_layout(L);
   if (e) return e;
   if (!params || !states || !action || !logprobs || !acts || !work) return RB200_E_NULL;
@@ -641,7 +735,7 @@ extern "C" int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params,
     TowerIO t[2] = {};
     t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
     t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
-    if ((e = towers_forward_h(states, idx, n, L->obs_dim, t, values ? 2 : 1, st))) return e;
+    if ((e = towers_forward_h(states, idx, n, L->obs_dim, t, values ? 2 : 1, x_amax_slot(L, acts, n), states_amax, st))) return e;
   } else {
     if ((e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
     if (values && (e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
@@ -736,7 +830,8 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params
     t[1].H1 = const_cast<float*>(G1); t[1].H2 = const_cast<float*>(G2); t[1].dZ3 = dY3; t[1].tA = uA; t[1].tB = uB;
     t[1].g_w0 = G + L->vw0; t[1].g_b0 = G + L->vb0; t[1].g_w1 = G + L->vw1; t[1].g_b1 = G + L->vb1;
     t[1].g_w2 = G + L->vw2; t[1].g_b2 = G + L->vb2; t[1].amax = amax + 3;
-    return towers_backward_h(states, idx, n, L->obs_dim, t, d_values ? 2 : 1, st);
+    return towers_backward_h(states, idx, n, L->obs_dim, t, d_values ? 2 : 1, x_amax_slot(L, const_cast<float*>(acts), n),
+                             st);
   }
   if ((e = tower_backward(states, idx, n, L->obs_dim, tower_w(L, P, false), H1, H2,
                           dZ3, tA, tB, G + L->bw0, G + L->bb0, G + L->bw1, G + L->bb1, G + L->bw2, G + L->bb2, st)))
@@ -766,7 +861,7 @@ extern "C" int rb200_mlp_sample(const rb200_mlp_layout* L, const float* params, 
     TowerIO t[2] = {};
     t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
     t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
-    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, st))) return e;
+    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, x_amax_slot(L, work, n), nullptr, st))) return e;
   } else {
     if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
     if (values && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
@@ -796,7 +891,7 @@ int mlp_mean_forward(const rb200_mlp_layout* L, const float* params, const float
     TowerIO t[2] = {};
     t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
     t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
-    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, st))) return e;
+    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, x_amax_slot(L, work, n), nullptr, st))) return e;
   } else {
     if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
     if (values && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
@@ -811,6 +906,14 @@ int mlp_mean_forward(const rb200_mlp_layout* L, const float* params, const float
   RB_RETURN_LAUNCH();
 }
 }  // namespace rb
+
+// the maxima rb200_mlp_forward's states_amax takes: out[0] = max|x| of x [rows, cols] (16-byte aligned, cols % 4 == 0)
+// and, for cols <= 256, out[4 + c] = max|x[:, c]|
+extern "C" int rb200_absmax(const float* x, int64_t rows, int cols, float* out, rb200_stream_t stream) {
+  if (!x || !out) return RB200_E_NULL;
+  if (rows <= 0 || cols <= 0 || cols % 4 != 0) return RB200_E_SHAPE;
+  return publish_absmax(x, rows, cols, out, rb::as_stream(stream));
+}
 
 // value tower + last linear layer only (no bias on the last layer: value_head.py:46)
 namespace {
@@ -832,7 +935,7 @@ __global__ void __launch_bounds__(256) value_head_kernel(const float* __restrict
 }
 }  // namespace
 
-// work: 3 activation tensors
+// work: rb200_mlp_fwd_scratch_floats(L, n) floats (3 activation tensors and the max|X| slot behind the 6 of the header)
 extern "C" int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, const float* wsplit,
                                const float* states, int64_t n, float* values, float* work, rb200_stream_t stream) {
   int e = check_layout(L);
@@ -845,7 +948,7 @@ extern "C" int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, c
   if (wsplit) {
     TowerIO t[1] = {};
     t[0].w = tower_w(L, params, true); t[0].wh = tower_wh(L, wsplit, true); t[0].H1 = G1; t[0].H2 = G2; t[0].H3 = G3;
-    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, 1, st))) return e;
+    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, 1, x_amax_slot(L, work, n), nullptr, st))) return e;
   } else if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, params, true), G1, G2, G3, st))) {
     return e;
   }

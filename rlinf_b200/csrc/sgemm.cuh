@@ -1,7 +1,8 @@
 // fp32 SIMT GEMM used by the MLP towers and the synthetic env (exact fp32 FMA accumulation).
 // C[M,N] = epilogue( sum_k A(m,k) * B(k,n) ), 128x128x8 tiles, 256 threads, 8x8 micro-tile per thread,
 // register-prefetched double-buffered shared memory.  Operand layouts are template parameters so the same
-// kernel serves forward (X.W^T), dgrad (dZ.W) and wgrad (dZ^T.H, split over the sample axis + atomics).
+// kernel serves forward (X.W^T), dgrad (dZ.W) and wgrad (dZ^T.H, split over the sample axis: atomics, or one stored
+// partial per split that the caller sums in split order).
 #pragma once
 #include "common.cuh"
 
@@ -29,6 +30,7 @@ struct GemmArgs {
   int N, lda, ldb, ldc, ldaux;
   int64_t K;
   int64_t k_per_split;  // reduction range per blockIdx.z
+  int64_t c_split_stride;  // EPI_STORE: split z writes its partial to C + z * c_split_stride (0: all splits share C)
 };
 
 __device__ __forceinline__ float4 ld4(const float* p, bool vec, int valid) {
@@ -199,7 +201,7 @@ __global__ void __launch_bounds__(NT) sgemm_kernel(GemmArgs p) {
       for (int j = 0; j < 4; ++j) {
         if (n + j >= p.N) continue;
         float v = acc[i][jh * 4 + j];
-        float* dst = p.C + m * p.ldc + n + j;
+        float* dst = p.C + blockIdx.z * p.c_split_stride + m * p.ldc + n + j;
         if (EPI == EPI_BIAS_TANH) {
           v = tanhf(v + p.bias[n + j]);
           *dst = v;

@@ -30,12 +30,15 @@ struct GemmLaunch {        // one group (tower) of a forward / dgrad launch
   float* colsum;           // EPI_TANHGRAD: [256] += column sums of the output, or NULL
   const float* amax_in;    // device max|a| (gradient operands: scaled into fp16 range), or NULL
   float* amax_out;         // EPI_TANHGRAD: atomicMax of |output| (feeds the next gradient GEMM), or NULL
+  const float* amax_x;     // device max|a| of an INPUT operand (observations; input_scale_log2_for), or NULL
 };
 struct WgradLaunch {
   const float* z;          // [n,256] activation gradients
   const float* h;          // [n,IN]  layer inputs
   float* dW;               // [256,IN] +=
   const float* amax_z;     // device max|z| or NULL
+  const float* amax_h;     // device [IN] per-column max|h| of an INPUT operand (observations; input_scale_log2_for per
+                           // column), or NULL (unscaled, as for the tanh outputs in [-1, 1] of the hidden layers)
 };
 struct SplitSpec {
   const float* src;        // weight matrix [256 out, K in] fp32

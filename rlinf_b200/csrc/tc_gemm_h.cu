@@ -4,7 +4,10 @@
 // Weights come as pre-swizzled fp16 (hi | lo) packs per k-block; activations stay plain fp32 in HBM and are split in
 // registers; one launch serves both towers.
 // Gradients are tiny (1e-6 .. 1e-10): their producer publishes max|x| and the consumer scales by 2^s (exact) so that the
-// maximum sits at 2^13; the fp32 accumulator is scaled back in the epilogue (exact).
+// maximum sits at 2^13; the fp32 accumulator is scaled back in the epilogue (exact).  Layer 0's input (the observations,
+// unbounded) is scaled the same way when its max lies outside [2^-1, 2^15) (input_scale_log2_for; inside, the unscaled
+// split is fp32-accurate already): the forward by max|X|, the weight gradient column by column (dW[:, c] only sees
+// column c of X, so a small feature is judged by its own max).
 // Reference op chains replaced: nn.Linear + tanh of MLPPolicy.backbone / ValueHead.mlp
 // (rlinf/models/embodiment/mlp_policy/mlp_policy.py:91-98, modules/value_head.py:37-45) and autograd's dgrad / wgrad.
 #include <cuda_fp16.h>
@@ -69,6 +72,7 @@ struct Group {
   const float* h;       // [M,256] previous activation   (EPI_TANHGRAD)
   float* colsum;        // [256] += column sums of the output, or NULL
   const float* amax_in; // [1] max|A| published by A's producer (gradient GEMMs), or NULL = no scaling
+  const float* amax_x;  // [1] max|A| of an input operand (layer 0's observations: input_scale_log2_for), or NULL
   float* amax_out;      // [1] atomicMax of |output| for the next gradient GEMM, or NULL
   float* c;             // [M,256] output
 };
@@ -132,7 +136,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_gemm_kernel(const __grid_con
     const int g = lane >> 2, t = lane & 3;
     const int r_lo = cw * 64 + (warp & 3) * 16 + g;  // this thread's tile rows r_lo and r_lo + 8
     // operand scaling: A by 2^sa (from the published amax), weights are stored * 2^kWeightScaleLog2
-    const int sa = G.amax_in ? scale_log2_for(__ldg(G.amax_in)) : 0;
+    const int sa = G.amax_in ? scale_log2_for(__ldg(G.amax_in)) : (G.amax_x ? input_scale_log2_for(__ldg(G.amax_x)) : 0);
     const float a_scale = pow2i(sa);
     const float out_scale = pow2i(-(sa + kWeightScaleLog2));
     float vmax = 0.f;
@@ -251,6 +255,8 @@ struct WgBarriers {
   uint64_t empty[kWgLand];  // landing stage read: dZ by the 8 consumer warps, H by the 3 split warps (one per warp)
   uint64_t op_full[2];      // operand slot written by the split threads (one arrival per thread, after its proxy fence)
   uint64_t op_empty[2];     // wgmmas reading the operand slot retired (one arrival per consumer warp)
+  alignas(16) float hsc[256];   // per-column scale of H (2^s, input_scale_log2_for of the column's max) and its inverse
+  alignas(16) float hinv[256];
 };
 
 struct WgradParams {
@@ -258,6 +264,7 @@ struct WgradParams {
   float* dW[2];
   float* part;             // [chunk][group][256 x IN] per-CTA partials of dW (summed in chunk order by sum_slots)
   const float* amax_z[2];  // max|dZ| per group (or NULL)
+  const float* amax_h[2];  // [IN] per-column max|H| per group (or NULL)
   int64_t n;
   int IN, kb_per_chunk, ngroups;
 };
@@ -290,7 +297,16 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
     }
     tma::fence_barrier_init();
   }
-  __syncthreads();
+  // H is an input operand (layer 0's observations) when amax_h is given: dW[:, c] is linear in column c of H, so each
+  // column takes its own power-of-two scale, undone exactly in the epilogue
+  int scaled = 0;
+  for (int c = threadIdx.x; c < IN; c += kThreads) {
+    const int s = P.amax_h[grp] ? input_scale_log2_for(__ldg(P.amax_h[grp] + c)) : 0;
+    bars->hsc[c] = pow2i(s);
+    bars->hinv[c] = pow2i(-s);
+    scaled |= s != 0;
+  }
+  const bool h_scaled = __syncthreads_or(scaled) != 0;  // no column scaled: the plain split, as for tanh outputs
   if (n_kb <= 0) return;
 
   if (wg == 2) {
@@ -302,7 +318,20 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
         tma::mbar_wait(&bars->op_empty[o], ((it >> 1) & 1u) ^ 1u);  // wgmmas of k-block it - 2 retired
         uint8_t* hop = op + o * kWgOpBytes;
         // H groups of [32 samples x 32 floats] (4 KB) -> [32 samples x 32 halfs] (2 KB), contiguous on both sides
-        split_tile<kWgSplitThreads>(smem + s * kWgLandBytes + kWgA32, hop, hop + kWgB16, IN, threadIdx.x - 288, 1.0f);
+        // item (row r = 32-column box r / 32 x sample r % 32, 8 floats cp): columns 32 * (r >> 5) + 8 * cp + 0..7
+        const uint8_t* hsrc = smem + s * kWgLandBytes + kWgA32;
+        if (!h_scaled) {
+          split_tile<kWgSplitThreads>(hsrc, hop, hop + kWgB16, IN, threadIdx.x - 288, 1.0f);
+        } else {
+#pragma unroll 2
+          for (int i = threadIdx.x - 288; i < IN * 4; i += kWgSplitThreads) {
+            const int r = i >> 2, cp = i & 3;
+            uint4 h, l;
+            split_item_cols(hsrc, r, cp, &bars->hsc[(r >> 5) * 32 + cp * 8], h, l);
+            *reinterpret_cast<uint4*>(hop + split_item_dst(r, cp)) = h;
+            *reinterpret_cast<uint4*>(hop + kWgB16 + split_item_dst(r, cp)) = l;
+          }
+        }
         tma::fence_proxy_async();  // generic-proxy stores -> the wgmmas' async-proxy reads
         tma::mbar_arrive(&bars->op_full[o]);
         warp_arrive(&bars->empty[s]);
@@ -389,10 +418,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_h_wgrad_kernel(const __grid_co
     for (int j = 0; j < NW / 8; ++j) {
       const int col = 8 * j + 2 * t;
       if (col < IN) {
+        // two exact power-of-two factors (one product could leave the float range)
+        const float i0 = bars->hinv[col], i1 = bars->hinv[col + 1];
         *reinterpret_cast<float2*>(slot + (size_t)row0 * IN + col) =
-            make_float2(acc[4 * j] * out_scale, acc[4 * j + 1] * out_scale);
+            make_float2(acc[4 * j] * out_scale * i0, acc[4 * j + 1] * out_scale * i1);
         *reinterpret_cast<float2*>(slot + (size_t)(row0 + 8) * IN + col) =
-            make_float2(acc[4 * j + 2] * out_scale, acc[4 * j + 3] * out_scale);
+            make_float2(acc[4 * j + 2] * out_scale * i0, acc[4 * j + 3] * out_scale * i1);
       }
     }
   }
@@ -462,7 +493,7 @@ int launch(const GemmLaunch* L, int ngroups, int64_t M, int K, int epi, int b_mn
     if (al & 15) return RB200_E_ALIGN;
     if (encode_f32_sw128(&P.a[g], l.a, (uint64_t)M, (uint64_t)K, BM)) return RB200_E_UNSUPPORTED;
     P.wpack[g] = reinterpret_cast<const uint8_t*>(l.b_hi);
-    P.g[g] = Group{l.bias, l.h, l.colsum, l.amax_in, l.amax_out, l.c};
+    P.g[g] = Group{l.bias, l.h, l.colsum, l.amax_in, l.amax_x, l.amax_out, l.c};
   }
   static bool attr_done = false;
   constexpr int kSmem = kRingBytes + 1024 + (int)sizeof(Barriers);
@@ -510,6 +541,7 @@ int wgrad(const WgradLaunch* L, int ngroups, int64_t n, int IN, cudaStream_t st)
     if (e) return RB200_E_UNSUPPORTED;
     P.dW[g] = L[g].dW;
     P.amax_z[g] = L[g].amax_z;
+    P.amax_h[g] = L[g].amax_h;
   }
   static bool attr_done = false;
   constexpr int kSmem = kWgRingBytes + 1024 + (int)sizeof(WgBarriers);

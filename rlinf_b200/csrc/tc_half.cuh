@@ -38,6 +38,16 @@ __device__ __forceinline__ int scale_log2_for(float amax) {
   return s > 100 ? 100 : (s < -100 ? -100 : s);
 }
 
+// Scale of an input operand (the observations of layer 0).  Unscaled, the (hi, lo) split of x is exact to 2^-22
+// relative down to |x| = 2^-3 and to 2^-25 absolute below (lo in fp16's subnormals), and hi stays finite below 65520; so
+// for max|x| in [2^-1, 2^15) every element is split to within 2^-24 * max|x|, fp32-level against the |W|.|x| of the
+// product, and the operand stays unscaled: its results are those of the unscaled split bit for bit.  Outside that range
+// (tiny inputs lose bits to subnormals, huge ones overflow to inf) it is scaled like a gradient operand.
+__device__ __forceinline__ int input_scale_log2_for(float amax) {
+  const int e = (int)((__float_as_uint(amax) >> 23) & 0xffu) - 127;
+  return (e >= -1 && e <= 14) ? 0 : scale_log2_for(amax);
+}
+
 // (x0, x1) -> packed fp16 pairs hi = rn(x), lo = rn(x - hi)
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   const __half2 hh = __floats2half2_rn(x0, x1);
@@ -57,6 +67,17 @@ __device__ __forceinline__ void split_item(const uint8_t* src, int r, int cp, fl
   split2(x0.z * scale, x0.w * scale, hi.y, lo.y);
   split2(x1.x * scale, x1.y * scale, hi.z, lo.z);
   split2(x1.z * scale, x1.w * scale, hi.w, lo.w);
+}
+// split_item with a scale per column: sc[0..7] for the 8 floats of the item
+__device__ __forceinline__ void split_item_cols(const uint8_t* src, int r, int cp, const float* sc, uint4& hi, uint4& lo) {
+  const uint8_t* srow = src + r * 128;
+  const float4 x0 = *reinterpret_cast<const float4*>(srow + (((2 * cp) ^ (r & 7)) << 4));
+  const float4 x1 = *reinterpret_cast<const float4*>(srow + (((2 * cp + 1) ^ (r & 7)) << 4));
+  const float4 s0 = *reinterpret_cast<const float4*>(sc), s1 = *reinterpret_cast<const float4*>(sc + 4);
+  split2(x0.x * s0.x, x0.y * s0.y, hi.x, lo.x);
+  split2(x0.z * s0.z, x0.w * s0.w, hi.y, lo.y);
+  split2(x1.x * s1.x, x1.y * s1.y, hi.z, lo.z);
+  split2(x1.z * s1.z, x1.w * s1.w, hi.w, lo.w);
 }
 __device__ __forceinline__ int split_item_dst(int r, int cp) { return r * 64 + ((cp ^ ((r >> 1) & 3)) << 4); }
 

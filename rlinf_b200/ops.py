@@ -78,6 +78,17 @@ def grpo_advantages(scores, loss_mask, T, group_size, eps=1e-6) -> torch.Tensor:
     return adv
 
 
+def absmax(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Maxima of |x| for x [rows, cols] (contiguous fp32, 16-byte aligned, cols % 4 == 0) as an fp32 device tensor:
+    [0] max|x| and, for cols <= 256, [4 + c] max|x[:, c]| (4 + cols floats, else 1) - MLPPolicy.forward_train's
+    `states_amax`."""
+    lib = L.load()
+    rows, cols = x.shape[0], x[0].numel()
+    out = out if out is not None else torch.empty(4 + cols if cols <= 256 else 1, dtype=torch.float32, device=x.device)
+    L.check(lib.rb200_absmax(L.ptr(x), rows, cols, L.ptr(out), L.stream_ptr()), "absmax")
+    return out
+
+
 def gather_rows(src: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     """dst = src.reshape(N, -1)[idx] with the trailing shape kept (bit-exact row gather)."""
     lib = L.load()

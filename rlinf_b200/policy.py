@@ -154,9 +154,12 @@ class MLPPolicy:
             self._scratch[key] = t
         return t
 
-    def forward_train(self, states, action, idx=None, n=None, compute_entropy=True, compute_values=True):
+    def forward_train(self, states, action, idx=None, n=None, compute_entropy=True, compute_values=True,
+                      states_amax=None):
         """default_forward (mlp_policy.py:202-236). states/action may be the whole rollout buffer with
-        `idx` (int64) selecting this micro-batch's rows.  Keeps activations for `backward`."""
+        `idx` (int64) selecting this micro-batch's rows.  Keeps activations for `backward`.  `states_amax`: optional
+        maxima of the batch these rows are cut from (`ops.absmax`), which save the forward its own pass over the
+        states."""
         lib = L.load()
         n = int(n if n is not None else (idx.numel() if idx is not None else states.shape[0]))
         nscr = lib.rb200_mlp_fwd_scratch_floats(C.byref(self.layout), n)
@@ -168,7 +171,7 @@ class MLPPolicy:
             compute_values and self.value_dim > 0) else None
         L.check(lib.rb200_mlp_forward(C.byref(self.layout), L.ptr(self.flat_params), self._ws(), L.ptr(states),
                                       L.ptr(action), L.ptr(idx), n, L.ptr(logp), L.ptr(ent), L.ptr(vals), L.ptr(acts),
-                                      L.ptr(work), L.stream_ptr()), "mlp_forward")
+                                      L.ptr(work), L.ptr(states_amax), L.stream_ptr()), "mlp_forward")
         self._last = (states, action, idx, n, acts)
         out = {"logprobs": logp}
         if ent is not None:
