@@ -333,7 +333,9 @@ int rb200_mlp_sample(const rb200_mlp_layout* L, const float* params, const float
                      float* work, rb200_stream_t stream);
 
 /* Unit-test entries of the fp16-split tensor-core GEMMs of the MLP towers (csrc/tc_gemm_h.cu, wgmma, fp32 in/out).
- * mode 0: C = A[M,K] . B[256,K]^T; mode 1 (dgrad form, K = 256): C = A[M,256] . B[256,256].  amax: device float holding
+ * mode 0: C = A[M,K] . B[256,K]^T through the forward kernel the towers run (tc_h_fwd_kernel, csrc/tc_forward_h.cu, for
+ * K <= 256; tc_h_gemm_kernel<0> above); mode 2: the same product through tc_h_gemm_kernel<0> for every K, the
+ * reference mode 0 is compared against bit for bit; mode 1 (dgrad form, K = 256): C = A[M,256] . B[256,256].  amax: device float holding
  * max|A| (or max|Z|), NULL = no operand scaling.  work: >= 512*K floats (packed fp16 weight tiles: forward + dgrad pack). */
 int rb200_tc_gemm_h(const float* A, const float* B, float* C, int64_t M, int K, int mode, const float* amax,
                     float* work, rb200_stream_t stream);

@@ -540,6 +540,11 @@ int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, 
   int e;
   const bool l0_tc = layer0_on_tc(idx, in_dim);
   rb::tch::GemmLaunch g[2];
+  // tc_h_fwd_kernel for K <= 256; tc_h_gemm_kernel<0> is the tensor-core path for wider observations
+  auto gemm = [&](int K) {
+    return K <= rb::tc::BN ? rb::tch::forward(g, nt, n, K, rb::tc::EPI_BIAS_TANH, st)
+                           : rb::tch::launch(g, nt, n, K, rb::tc::EPI_BIAS_TANH, 0, st);
+  };
   if (l0_tc) {
     if (x_amax_in) {
       cudaError_t ce = cudaMemcpyAsync(x_amax, x_amax_in, sizeof(float) * x_amax_floats(in_dim), cudaMemcpyDeviceToDevice, st);
@@ -548,15 +553,15 @@ int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, 
       return e;
     }
     for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{X, t[i].wh.w0f, nullptr, t[i].H1, t[i].w.b0, nullptr, nullptr, nullptr, nullptr, x_amax};
-    if ((e = rb::tch::launch(g, nt, n, in_dim, rb::tc::EPI_BIAS_TANH, 0, st))) return e;
+    if ((e = gemm(in_dim))) return e;
   } else {
     for (int i = 0; i < nt; ++i)
       if ((e = layer_forward(X, idx, n, in_dim, t[i].w.w0, t[i].w.b0, t[i].H1, st))) return e;
   }
   for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{t[i].H1, t[i].wh.w1f, nullptr, t[i].H2, t[i].w.b1, nullptr, nullptr, nullptr, nullptr};
-  if ((e = rb::tch::launch(g, nt, n, kH, rb::tc::EPI_BIAS_TANH, 0, st))) return e;
+  if ((e = gemm(kH))) return e;
   for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{t[i].H2, t[i].wh.w2f, nullptr, t[i].H3, t[i].w.b2, nullptr, nullptr, nullptr, nullptr};
-  return rb::tch::launch(g, nt, n, kH, rb::tc::EPI_BIAS_TANH, 0, st);
+  return gemm(kH);
 }
 
 // Row chunks of the SIMT layer-0 weight gradient: a function of n and the device only, so the chunk-order sum is the

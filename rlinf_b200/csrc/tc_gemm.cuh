@@ -49,6 +49,9 @@ struct SplitSpec {
 
 // epi: rb::tc::Epi.  b_mn = 0: C = epi(A . W^T) (forward, W [256,K]);  b_mn = 1: C = epi(A . W) (dgrad, W [256,256]).
 int launch(const GemmLaunch* groups, int ngroups, int64_t M, int K, int epi, int b_mn, cudaStream_t st);
+// The forward C = epi(A . W^T) for K <= 256 (tc_forward_h.cu): epi EPI_STORE or EPI_BIAS_TANH, the forward packs'
+// weights resident in shared memory; bit-identical to launch(..., b_mn = 0), which stays the path for K > 256.
+int forward(const GemmLaunch* groups, int ngroups, int64_t M, int K, int epi, cudaStream_t st);
 int wgrad(const WgradLaunch* groups, int ngroups, int64_t n, int IN, cudaStream_t st);
 struct BackwardLaunch {    // one group of the backward through a square hidden layer (tc_backward_h.cu)
   const float* z;          // [n,256] dZ_L

@@ -25,7 +25,8 @@ using rb::tc::BK;
 using rb::tc::BM;
 using rb::tc::BN;
 
-// Forward / dgrad kernel (persistent, one CTA per SM): a producer warp fills a ring of stages (fp32 landing tile of the
+// Forward / dgrad kernel (persistent, one CTA per SM; the towers' forward runs tc_h_fwd_kernel of tc_forward_h.cu for
+// K <= 256 and this kernel for wider layer-0 inputs): a producer warp fills a ring of stages (fp32 landing tile of the
 // streamed operand, [128 rows x 32 k] TMA SWIZZLE_128B, + the packed weight tile of the k-block, one 32 KB bulk copy);
 // warpgroups 0 / 1 own rows 0-63 / 64-127 of the 128 x 256 output tile, split their fp32 rows into fp16 hi / lo wgmma A
 // fragments in registers and keep the fp32 accumulator in registers through the epilogue.
@@ -42,23 +43,6 @@ constexpr int kRingBytes = kStages * kStageBytes;  // 192 KB
 constexpr int kThreads = 384;
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file");
-
-__device__ __forceinline__ float tanh_fast(float x) {
-  const float t = __expf(-2.0f * fabsf(x));
-  return copysignf(__fdividef(1.0f - t, 1.0f + t), x);
-}
-
-// wgmma A fragment (m64k16, this thread's rows r0 / r0 + 8, k columns c0 + 2t + {0, 1, 8, 9}) of a row-major fp32
-// [rows x 32] SWIZZLE_128B landing tile, scaled and split into fp16 hi / lo
-__device__ __forceinline__ void a_frag_rows(const uint8_t* tile, int r0, int c0, float scale, uint32_t (&hi)[4],
-                                            uint32_t (&lo)[4]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = r0 + (i & 1) * 8, c = c0 + (i >> 1) * 8;
-    const float2 x = *reinterpret_cast<const float2*>(tile + r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4);
-    split2(x.x * scale, x.y * scale, hi[i], lo[i]);
-  }
-}
 
 struct __align__(16) Barriers {
   uint64_t full[kStages];   // landing tile + weight tile arrived (tx bytes)
@@ -634,22 +618,26 @@ extern "C" int rb200_debug_set_flags(int flags) {
 }
 
 // ---- unit-test entries (tests/test_gpu_tc_gemm.py) --------------------------------------------------------------------
-// C[M,256] = A[M,K] . B[256,K]^T (mode 0, forward) or A[M,256] . B[256,256] (mode 1, dgrad form: B is [out=K, in=N]);
-// work: >= 256*K floats (fp16 hi/lo copies of B).  amax (device float, nullable) exercises the gradient scaling.
+// C[M,256] = A[M,K] . B[256,K]^T (mode 0: the shipped forward, tc_h_fwd_kernel for K <= 256, tc_h_gemm_kernel<0> above;
+// mode 2: tc_h_gemm_kernel<0> for every K, the reference of the bit-identity tests) or A[M,256] . B[256,256] (mode 1,
+// dgrad form: B is [out=K, in=N]); work: >= 256*K floats (fp16 hi/lo copies of B).  amax (device float, nullable)
+// exercises the gradient scaling.
 extern "C" int rb200_tc_gemm_h(const float* A, const float* B, float* C, int64_t M, int K, int mode, const float* amax,
                                float* work, rb200_stream_t stream) {
   if (!A || !B || !C || !work) return RB200_E_NULL;
-  if (M <= 0 || K <= 0 || K % rb::tc::BK != 0) return RB200_E_SHAPE;
+  if (M <= 0 || K <= 0 || K % rb::tc::BK != 0 || mode < 0 || mode > 2) return RB200_E_SHAPE;
   cudaStream_t st = rb::as_stream(stream);
   const int64_t nb = (int64_t)rb::tc::BN * K;
-  if (mode && K != rb::tc::BN) return RB200_E_SHAPE;
+  const bool dgrad = mode == 1;
+  if (dgrad && K != rb::tc::BN) return RB200_E_SHAPE;
   // forward pack always; the dgrad pack (square matrices only) behind it
-  rb::tch::SplitSpec sp{B, work, mode ? work + nb : nullptr, nb};
+  rb::tch::SplitSpec sp{B, work, dgrad ? work + nb : nullptr, nb};
   int e = rb::tch::split_weights(&sp, 1, st);
   if (e) return e;
   rb::tch::GemmLaunch l{};
-  l.a = A; l.b_hi = mode ? sp.lo : sp.hi; l.b_lo = nullptr; l.c = C; l.amax_in = amax;
-  return rb::tch::launch(&l, 1, M, K, rb::tc::EPI_STORE, mode ? 1 : 0, st);
+  l.a = A; l.b_hi = dgrad ? sp.lo : sp.hi; l.b_lo = nullptr; l.c = C; l.amax_in = amax;
+  if (mode == 0 && K <= rb::tc::BN) return rb::tch::forward(&l, 1, M, K, rb::tc::EPI_STORE, st);
+  return rb::tch::launch(&l, 1, M, K, rb::tc::EPI_STORE, dgrad ? 1 : 0, st);
 }
 
 extern "C" int rb200_tc_wgrad_h(const float* Z, const float* H, float* dW, int64_t n, int IN, const float* amax,

@@ -1,5 +1,5 @@
-// Device helpers shared by the fp16-split wgmma kernels of the PPO update (tc_gemm_h.cu, tc_backward_h.cu): operand
-// scaling, the fp32 -> fp16 (hi, lo) split, bulk copies and ring-slot release.
+// Device helpers shared by the fp16-split wgmma kernels of the PPO update (tc_gemm_h.cu, tc_forward_h.cu,
+// tc_backward_h.cu): operand scaling, the fp32 -> fp16 (hi, lo) split, bulk copies and ring-slot release.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -55,6 +55,24 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
   const __half2 ll = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
   hi = *reinterpret_cast<const uint32_t*>(&hh);
   lo = *reinterpret_cast<const uint32_t*>(&ll);
+}
+
+// wgmma A fragment (m64k16, this thread's rows r0 / r0 + 8, k columns c0 + 2t + {0, 1, 8, 9}) of a row-major fp32
+// [rows x 32] SWIZZLE_128B landing tile, scaled and split into fp16 hi / lo
+__device__ __forceinline__ void a_frag_rows(const uint8_t* tile, int r0, int c0, float scale, uint32_t (&hi)[4],
+                                            uint32_t (&lo)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = r0 + (i & 1) * 8, c = c0 + (i >> 1) * 8;
+    const float2 x = *reinterpret_cast<const float2*>(tile + r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4);
+    split2(x.x * scale, x.y * scale, hi[i], lo[i]);
+  }
+}
+
+// the forward epilogue's tanh (MUFU exp, 3e-7 absolute)
+__device__ __forceinline__ float tanh_fast(float x) {
+  const float t = __expf(-2.0f * fabsf(x));
+  return copysignf(__fdividef(1.0f - t, 1.0f + t), x);
 }
 
 // One split item = (row r, 8 floats cp of its 32): the two 16-byte chunks of fp32 row r (SWIZZLE_128B, 128-B rows) ->
