@@ -294,17 +294,17 @@ int64_t rb200_mlp_fwd_scratch_floats(const rb200_mlp_layout* L, int64_t n);
 
 /* Tensor-core operand cache: packed fp16 (hi, lo) tiles of the hidden-layer weights (forward and dgrad packs).
  * rb200_mlp_wsplit_floats() floats; refresh with rb200_mlp_prepare_weights() after every parameter update.
- * Passing wsplit == NULL to the calls below selects the fp32 SIMT GEMMs for every layer. */
+ * Every MLP call below requires it: wsplit == NULL returns RB200_E_NULL. */
 int64_t rb200_mlp_wsplit_floats(const rb200_mlp_layout* L);
 int rb200_mlp_prepare_weights(const rb200_mlp_layout* L, const float* params, float* wsplit,
                               rb200_stream_t stream);
 
 /* Forward for training: states [n,obs] (row i at idx?idx[i]:i), action [n,act] (same gather).
  * Writes logprobs [n,act], entropy [n,act] (NULL ok), values [n,value_dim] (NULL ok) and keeps
- * the activations needed by backward in `acts`. Hidden layers run on wgmma (2-way fp16 split) when wsplit is given
- * and the layer's K is a multiple of 32 (layer 1 additionally needs idx == NULL). Activations are plain fp32; the
- * tensor-core kernels split them into fp16 (hi, lo) operands.  (The 3xTF32 entries of earlier versions -
- * rb200_tc_gemm, rb200_tc_wgrad, rb200_split_tf32 - and the two probe hooks are gone.) */
+ * the activations needed by backward in `acts`. Hidden layers run on wgmma (2-way fp16 split); layer 0 does too when
+ * obs is a multiple of 32 and idx == NULL (its weight gradient only for obs <= 256), and runs on the fp32 SIMT GEMM
+ * otherwise. Activations are plain fp32; the
+ * tensor-core kernels split them into fp16 (hi, lo) operands. */
 int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params, const float* wsplit,
                       const float* states, const float* action, const int64_t* idx, int64_t n,
                       float* logprobs, float* entropy, float* values, float* acts, float* work,
@@ -508,7 +508,7 @@ int rb200_counter_add(uint64_t* counter_dev, uint64_t inc, rb200_stream_t stream
 /* Eval-mode inference, _generate_actions(mode="eval") (mlp_policy.py:256-293): actor tower and mean head only,
  * action [n,act] = mean; logprobs [n,act] = Normal(mean, exp(logstd)).log_prob(mean) (NULL = not computed);
  * values [n,value_dim] = ValueHead(states) (NULL = value tower skipped).  No sampling, no RNG.
- * work: rb200_mlp_fwd_scratch_floats(L, n) floats; wsplit as for rb200_mlp_sample (NULL = fp32 SIMT GEMMs). */
+ * work: rb200_mlp_fwd_scratch_floats(L, n) floats; wsplit as for rb200_mlp_sample. */
 int rb200_mlp_mean(const rb200_mlp_layout* L, const float* params, const float* wsplit, const float* states,
                    int64_t n, float* action, float* logprobs, float* values, float* work, rb200_stream_t stream);
 /* Episode statistics of one chunk step of an evaluation rollout, one thread per env (ManiskillEnv._record_metrics /

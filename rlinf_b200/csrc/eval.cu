@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(kReduceThreads) episode_stats_reduce_kernel(co
 extern "C" int rb200_mlp_mean(const rb200_mlp_layout* L, const float* params, const float* wsplit,
                               const float* states, int64_t n, float* action, float* logprobs, float* values,
                               float* work, rb200_stream_t stream) {
-  if (!L || !params || !states || !action || !work) return RB200_E_NULL;
+  if (!L || !params || !wsplit || !states || !action || !work) return RB200_E_NULL;
   if (n <= 0) return RB200_E_SHAPE;
   if (values && L->value_dim == 0) return RB200_E_SHAPE;
   return rb::mlp_mean_forward(L, params, wsplit, states, n, action, logprobs, values, work, rb::as_stream(stream));

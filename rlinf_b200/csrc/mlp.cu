@@ -4,9 +4,10 @@
 // ValueHead, rlinf/models/embodiment/modules/value_head.py:18-67 (3x256 tanh MLP -> value_dim, last layer
 // without bias); backward = what autograd derives from them.
 //
-// Hidden-layer GEMMs run on the tensor cores whenever the operand shapes allow TMA (K % 32 == 0, no row gather): the
-// fp16-split kernels (tc_gemm_h.cu: wgmma, a = a_hi + a_lo in fp16, three MMAs per product, fp32-level accuracy, both
-// towers per launch); the fp32 SIMT GEMM (sgemm.cuh) covers the remaining shapes and callers without a weight cache.
+// Hidden-layer GEMMs run on the fp16-split tensor-core kernels (tc_gemm_h.cu: wgmma, a = a_hi + a_lo in fp16, three
+// MMAs per product, fp32-level accuracy, both towers per launch), which read the weight cache (wsplit) every entry
+// requires.  Layer 0 runs on them too when the operand shapes allow TMA (obs % 32 == 0, no row gather); the fp32 SIMT
+// GEMM (sgemm.cuh) covers its remaining shapes.
 // Activations and activation-gradients are stored once, as plain fp32 [n,256] (6 tanh outputs per forward,
 // tanh' = 1 - h^2); the tensor-core kernels split them into (hi, lo) pairs on the fly.
 // The heads (256 -> act mean, 256 -> value) are fused with the Normal log-prob / entropy epilogue and their backward.
@@ -19,25 +20,6 @@
 namespace {
 
 using namespace rb::gemm;
-
-// out[n] += sum_m Z[m][n]   (bias gradients); Z is [M, N] with N <= 1024
-__global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ Z, float* __restrict__ out, int64_t M, int N,
-                                                     int64_t rows_per_block) {
-  const int64_t r0 = (int64_t)blockIdx.x * rows_per_block;
-  const int64_t r1 = (r0 + rows_per_block < M) ? r0 + rows_per_block : M;
-  for (int n = threadIdx.x; n < N; n += blockDim.x) {
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    int64_t r = r0;
-    for (; r + 3 < r1; r += 4) {
-      s0 += Z[r * N + n];
-      s1 += Z[(r + 1) * N + n];
-      s2 += Z[(r + 2) * N + n];
-      s3 += Z[(r + 3) * N + n];
-    }
-    for (; r < r1; ++r) s0 += Z[r * N + n];
-    atomicAdd(&out[n], (s0 + s1) + (s2 + s3));
-  }
-}
 
 // max|x| of a row-major [rows, 4 * cols4] matrix: out[0] = max(out[0], max |x|) and, with cols, out[4 + c] =
 // max(out[4 + c], max over rows |x[:, c]|).  Non-negative floats order like their bit patterns, so the results do not
@@ -422,65 +404,16 @@ int head_grid(int64_t n) {
 // ---------------------------------------------------------------------------------------------------------
 // Towers.  Activation / gradient tensors are plain fp32 [n,256].
 // ---------------------------------------------------------------------------------------------------------
-struct TowerW {           // fp32 weights (SIMT path)
+struct TowerW {  // fp32 weights and biases
   const float *w0, *b0, *w1, *b1, *w2, *b2;
 };
-// one hidden layer forward: out = tanh(in . W^T + b)
+// layer 0 forward on the SIMT GEMM (shapes the tensor-core kernels do not take): out = tanh(in[idx] . W^T + b)
 int layer_forward(const float* in, const int64_t* idx, int64_t n, int in_dim, const float* w, const float* b,
                   float* out, cudaStream_t st) {
   GemmArgs g{};
   g.M = n; g.N = kH; g.ldc = kH; g.k_per_split = 1 << 30;
   g.A = in; g.lda = in_dim; g.a_rows = idx; g.B = w; g.ldb = in_dim; g.K = in_dim; g.bias = b; g.C = out;
   return launch_gemm<A_KCONTIG, B_KCONTIG, EPI_BIAS_TANH>(g, 1, st);
-}
-
-// X -> H1 -> H2 -> H3 (each [n,256]), fp32 SIMT
-int tower_forward(const float* X, const int64_t* idx, int64_t n, int in_dim, const TowerW& w, float* H1, float* H2,
-                  float* H3, cudaStream_t st) {
-  int e = layer_forward(X, idx, n, in_dim, w.w0, w.b0, H1, st);
-  if (e) return e;
-  e = layer_forward(H1, nullptr, n, kH, w.w1, w.b1, H2, st);
-  if (e) return e;
-  return layer_forward(H2, nullptr, n, kH, w.w2, w.b2, H3, st);
-}
-
-// backward through the three hidden layers of one tower, given dZ3 (fp32 SIMT). tmpA/tmpB: [n,256] scratch.
-int tower_backward(const float* X, const int64_t* idx, int64_t n, int in_dim, const TowerW& w, const float* H1, const float* H2, const float* dZ3, float* tmpA, float* tmpB, float* g_w0,
-                   float* g_b0, float* g_w1, float* g_b1, float* g_w2, float* g_b2, cudaStream_t st) {
-  const int64_t rows_per_split = 4096;
-  const int splits = (int)((n + rows_per_split - 1) / rows_per_split);
-  const int64_t cs_rows = 128;
-  const int cs_blocks = (int)((n + cs_rows - 1) / cs_rows);
-  int e;
-  auto colsum = [&](const float* dZ, float* gb) -> int {
-    colsum_kernel<<<cs_blocks, 256, 0, st>>>(dZ, gb, n, kH, cs_rows);
-    rb::count_launch();
-    cudaError_t ce = cudaPeekAtLastError();
-    return ce == cudaSuccess ? 0 : (int)ce;
-  };
-  auto wgrad = [&](const float* dZ, const float* Hin, const int64_t* in_rows, int in_ld, float* gw, float* gb,
-                   bool need_colsum) -> int {
-    // gw[256, in_ld] += dZ^T [256, n] . Hin [n, in_ld]
-    // split over samples, atomics
-    GemmArgs g{};
-    g.A = dZ; g.lda = kH; g.B = Hin; g.ldb = in_ld; g.b_rows = in_rows; g.C = gw;
-    g.ldc = in_ld; g.M = kH; g.N = in_ld; g.K = n; g.k_per_split = rows_per_split;
-    const int ee = launch_gemm<A_MCONTIG, B_NCONTIG, EPI_ATOMIC>(g, splits, st);
-    if (ee || !need_colsum) return ee;
-    return colsum(dZ, gb);
-  };
-  auto dgrad = [&](const float* dZ, const float* W, const float* Hprev, float* out) -> int {
-    // out = (dZ . W) * (1 - Hprev^2)
-    GemmArgs g{};
-    g.A = dZ; g.lda = kH; g.B = W; g.ldb = kH; g.C = out; g.ldc = kH; g.aux = Hprev;
-    g.ldaux = kH; g.M = n; g.N = kH; g.K = kH; g.k_per_split = 1 << 30;
-    return launch_gemm<A_KCONTIG, B_NCONTIG, EPI_TANHGRAD>(g, 1, st);
-  };
-  if ((e = wgrad(dZ3, H2, nullptr, kH, g_w2, g_b2, false))) return e;  // g_b2: head_bwd_kernel
-  if ((e = dgrad(dZ3, w.w2, H2, tmpA))) return e;  // dZ2
-  if ((e = wgrad(tmpA, H1, nullptr, kH, g_w1, g_b1, true))) return e;
-  if ((e = dgrad(tmpA, w.w1, H1, tmpB))) return e;  // dZ1
-  return wgrad(tmpB, X, idx, in_dim, g_w0, g_b0, true);
 }
 
 // ---- fp16-split tensor-core path (tc_gemm_h.cu), both towers per launch ------------------------------------------------
@@ -552,15 +485,15 @@ int towers_forward_h(const float* X, const int64_t* idx, int64_t n, int in_dim, 
     } else if ((e = publish_absmax(X, n, in_dim, x_amax, st))) {
       return e;
     }
-    for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{X, t[i].wh.w0f, nullptr, t[i].H1, t[i].w.b0, nullptr, nullptr, nullptr, nullptr, x_amax};
+    for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{X, t[i].wh.w0f, t[i].H1, t[i].w.b0, nullptr, nullptr, nullptr, nullptr, x_amax};
     if ((e = gemm(in_dim))) return e;
   } else {
     for (int i = 0; i < nt; ++i)
       if ((e = layer_forward(X, idx, n, in_dim, t[i].w.w0, t[i].w.b0, t[i].H1, st))) return e;
   }
-  for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{t[i].H1, t[i].wh.w1f, nullptr, t[i].H2, t[i].w.b1, nullptr, nullptr, nullptr, nullptr};
+  for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{t[i].H1, t[i].wh.w1f, t[i].H2, t[i].w.b1, nullptr, nullptr, nullptr, nullptr};
   if ((e = gemm(kH))) return e;
-  for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{t[i].H2, t[i].wh.w2f, nullptr, t[i].H3, t[i].w.b2, nullptr, nullptr, nullptr, nullptr};
+  for (int i = 0; i < nt; ++i) g[i] = rb::tch::GemmLaunch{t[i].H2, t[i].wh.w2f, t[i].H3, t[i].w.b2, nullptr, nullptr, nullptr, nullptr};
   return gemm(kH);
 }
 
@@ -652,8 +585,9 @@ extern "C" int rb200_mlp_layout_init(rb200_mlp_layout* L, int obs_dim, int act_d
   return RB200_OK;
 }
 
-// acts layout (floats): H1 H2 H3 G1 G2 G3, each [n,256] | mean [n,act]
-// work layout: 6 gradient tensors of [n,256]
+// acts layout (floats): H1 H2 H3 G1 G2 G3, each [n,256] (backbone, value tower) | mean [n,act] | x_amax slot; the
+// inference entries lay out their `work` the same way
+// backward work layout: 6 gradient tensors of [n,256] | 8 floats of gradient maxima
 static inline int64_t act_floats(int64_t n) { return n * kH; }
 
 extern "C" int64_t rb200_mlp_fwd_scratch_floats(const rb200_mlp_layout* L, int64_t n) {
@@ -698,6 +632,42 @@ TowerWH tower_wh(const rb200_mlp_layout* L, const float* ws, bool value) {
   t.w2d = b + n0 + 3 * nn;
   return t;
 }
+
+// The backbone (value = false) or the value tower with its activations H1 H2 H3 at h, h + n*256, h + 2*n*256.
+TowerIO tower_io(const rb200_mlp_layout* L, const float* P, const float* wsplit, bool value, float* h, int64_t n) {
+  TowerIO t{};
+  t.w = tower_w(L, P, value);
+  t.wh = tower_wh(L, wsplit, value);
+  t.H1 = h;
+  t.H2 = h + act_floats(n);
+  t.H3 = h + 2 * act_floats(n);
+  return t;
+}
+
+// Forward of the backbone (policy) and of the value tower (value) into buf, laid out as acts.  x_amax_in as for
+// towers_forward_h.
+int forward_towers(const rb200_mlp_layout* L, const float* P, const float* wsplit, const float* states,
+                   const int64_t* idx, int64_t n, bool policy, bool value, float* buf, const float* x_amax_in,
+                   cudaStream_t st) {
+  TowerIO t[2];
+  int nt = 0;
+  if (policy) t[nt++] = tower_io(L, P, wsplit, false, buf, n);
+  if (value) t[nt++] = tower_io(L, P, wsplit, true, buf + 3 * act_floats(n), n);
+  return towers_forward_h(states, idx, n, L->obs_dim, t, nt, x_amax_slot(L, buf, n), x_amax_in, st);
+}
+
+// head_fwd_kernel on the tower outputs in buf (laid out as acts; the value tower's is read when values != NULL).
+// h holds the fields of the mode: sample_mode with its inputs and outputs.
+int head_forward(const rb200_mlp_layout* L, const float* P, const float* buf, int64_t n, float* values, HeadFwdArgs h,
+                 cudaStream_t st) {
+  h.h3 = buf + 2 * act_floats(n); h.g3 = values ? buf + 5 * act_floats(n) : nullptr;
+  h.mw = P + L->mw; h.mb = P + L->mb; h.logstd = P + L->logstd; h.vw3 = P + L->vw3;
+  h.values = values; h.n = n; h.act = L->act_dim; h.vdim = L->value_dim;
+  const size_t smem = sizeof(float) * (size_t)(L->act_dim + (values ? L->value_dim : 0)) * kH;
+  head_fwd_kernel<<<head_grid(n), 256, smem, st>>>(h);
+  rb::count_launch();
+  RB_RETURN_LAUNCH();
+}
 }  // namespace
 
 // Refresh the weight copies the tensor-core GEMMs read: packed fp16 (hi, lo) tiles of w * 2^10 for all hidden matrices,
@@ -728,31 +698,15 @@ extern "C" int rb200_mlp_forward(const rb200_mlp_layout* L, const float* params,
                                  const float* states_amax, rb200_stream_t stream) {
   int e = check_layout(L);
   if (e) return e;
-  if (!params || !states || !action || !logprobs || !acts || !work) return RB200_E_NULL;
+  if (!params || !wsplit || !states || !action || !logprobs || !acts || !work) return RB200_E_NULL;
   if (n <= 0) return RB200_E_SHAPE;
   if (values && L->value_dim == 0) return RB200_E_SHAPE;
   cudaStream_t st = rb::as_stream(stream);
-  const int64_t PF = act_floats(n);
-  float *H1 = acts, *H2 = H1 + PF, *H3 = H2 + PF, *G1 = H3 + PF, *G2 = G1 + PF, *G3 = G2 + PF;
-  float* mean = G3 + PF;
-  const float* P = params;
-  if (wsplit) {
-    TowerIO t[2] = {};
-    t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
-    t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
-    if ((e = towers_forward_h(states, idx, n, L->obs_dim, t, values ? 2 : 1, x_amax_slot(L, acts, n), states_amax, st))) return e;
-  } else {
-    if ((e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
-    if (values && (e = tower_forward(states, idx, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
-  }
+  if ((e = forward_towers(L, params, wsplit, states, idx, n, true, values != nullptr, acts, states_amax, st))) return e;
   HeadFwdArgs h{};
-  h.h3 = H3; h.g3 = values ? G3 : nullptr; h.mw = P + L->mw; h.mb = P + L->mb;
-  h.logstd = P + L->logstd; h.vw3 = P + L->vw3; h.action = action; h.idx = idx; h.sample_mode = 0; h.mean_out = mean;
-  h.logprobs = logprobs; h.entropy = entropy; h.values = values; h.n = n; h.act = L->act_dim; h.vdim = L->value_dim;
-  const size_t smem = sizeof(float) * (size_t)(L->act_dim + L->value_dim) * kH;
-  head_fwd_kernel<<<head_grid(n), 256, smem, st>>>(h);
-  rb::count_launch();
-  RB_RETURN_LAUNCH();
+  h.action = action; h.idx = idx; h.sample_mode = 0; h.mean_out = acts + 6 * act_floats(n); h.logprobs = logprobs;
+  h.entropy = entropy;
+  return head_forward(L, params, acts, n, values, h, st);
 }
 
 extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params, const float* wsplit,
@@ -761,12 +715,11 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params
                                   const float* acts, float* work, float* grads, rb200_stream_t stream) {
   int e = check_layout(L);
   if (e) return e;
-  if (!params || !states || !action || !d_logprobs || !acts || !work || !grads) return RB200_E_NULL;
+  if (!params || !wsplit || !states || !action || !d_logprobs || !acts || !work || !grads) return RB200_E_NULL;
   if (n <= 0) return RB200_E_SHAPE;
   cudaStream_t st = rb::as_stream(stream);
   const int64_t PF = act_floats(n);
-  const float *H1 = acts, *H2 = H1 + PF, *H3 = H2 + PF, *G1 = H3 + PF, *G2 = G1 + PF, *G3 = G2 + PF;
-  const float* mean = G3 + PF;
+  const float *H3 = acts + 2 * PF, *G3 = acts + 5 * PF, *mean = acts + 6 * PF;
   float *dZ3 = work, *tA = dZ3 + PF, *tB = tA + PF, *dY3 = tB + PF, *uA = dY3 + PF, *uB = uA + PF;
   const float* P = params;
   float* G = grads;
@@ -777,14 +730,13 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params
   h.g_mw = G + L->mw; h.g_mb = G + L->mb; h.g_logstd = G + L->logstd; h.g_vw3 = G + L->vw3;
   h.g_b2 = G + L->bb2; h.g_vb2 = G + L->vb2;
   h.n = n; h.act = L->act_dim; h.vdim = L->value_dim;
-  const bool use_h = wsplit != nullptr;
   float* amax = work + 6 * PF;  // 8 floats of the scratch tail: max|dZ3|,|dZ2|,|dZ1| of the policy tower, then the value tower
-  if (use_h) {
+  {
     cudaError_t ce = cudaMemsetAsync(amax, 0, 8 * sizeof(float), st);
     if (ce != cudaSuccess) return (int)ce;
-    h.amax_dz3 = amax;
-    h.amax_dy3 = amax + 3;
   }
+  h.amax_dz3 = amax;
+  h.amax_dy3 = amax + 3;
   const int acc_len = (L->act_dim + L->value_dim) * kH + 64 + 2 * kH, w_len = (L->act_dim + L->value_dim) * kH;
   int nw = (232448 / 4 - w_len) / acc_len;  // warps per block: one accumulator copy each
   nw = nw > 8 ? 8 : nw;
@@ -825,28 +777,15 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_layout* L, const float* params
     }
     if ((e = rb::tch::sum_slots(ss, st))) return e;
   }
-  if (use_h) {
-    TowerIO t[2] = {};
-    t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false);
-    t[0].H1 = const_cast<float*>(H1); t[0].H2 = const_cast<float*>(H2); t[0].dZ3 = dZ3; t[0].tA = tA; t[0].tB = tB;
-    t[0].g_w0 = G + L->bw0; t[0].g_b0 = G + L->bb0; t[0].g_w1 = G + L->bw1; t[0].g_b1 = G + L->bb1;
-    t[0].g_w2 = G + L->bw2; t[0].g_b2 = G + L->bb2; t[0].amax = amax;
-    t[1].w = tower_w(L, P, true); t[1].wh = tower_wh(L, wsplit, true);
-    t[1].H1 = const_cast<float*>(G1); t[1].H2 = const_cast<float*>(G2); t[1].dZ3 = dY3; t[1].tA = uA; t[1].tB = uB;
-    t[1].g_w0 = G + L->vw0; t[1].g_b0 = G + L->vb0; t[1].g_w1 = G + L->vw1; t[1].g_b1 = G + L->vb1;
-    t[1].g_w2 = G + L->vw2; t[1].g_b2 = G + L->vb2; t[1].amax = amax + 3;
-    return towers_backward_h(states, idx, n, L->obs_dim, t, d_values ? 2 : 1, x_amax_slot(L, const_cast<float*>(acts), n),
-                             st);
-  }
-  if ((e = tower_backward(states, idx, n, L->obs_dim, tower_w(L, P, false), H1, H2,
-                          dZ3, tA, tB, G + L->bw0, G + L->bb0, G + L->bw1, G + L->bb1, G + L->bw2, G + L->bb2, st)))
-    return e;
-  if (d_values &&
-      (e = tower_backward(states, idx, n, L->obs_dim, tower_w(L, P, true), G1, G2,
-                          dY3, uA, uB,
-                          G + L->vw0, G + L->vb0, G + L->vw1, G + L->vb1, G + L->vw2, G + L->vb2, st)))
-    return e;
-  return RB200_OK;
+  float* act_buf = const_cast<float*>(acts);
+  TowerIO t[2] = {tower_io(L, P, wsplit, false, act_buf, n), tower_io(L, P, wsplit, true, act_buf + 3 * PF, n)};
+  t[0].dZ3 = dZ3; t[0].tA = tA; t[0].tB = tB; t[0].amax = amax;
+  t[0].g_w0 = G + L->bw0; t[0].g_b0 = G + L->bb0; t[0].g_w1 = G + L->bw1; t[0].g_b1 = G + L->bb1;
+  t[0].g_w2 = G + L->bw2; t[0].g_b2 = G + L->bb2;
+  t[1].dZ3 = dY3; t[1].tA = uA; t[1].tB = uB; t[1].amax = amax + 3;
+  t[1].g_w0 = G + L->vw0; t[1].g_b0 = G + L->vb0; t[1].g_w1 = G + L->vw1; t[1].g_b1 = G + L->vb1;
+  t[1].g_w2 = G + L->vw2; t[1].g_b2 = G + L->vb2;
+  return towers_backward_h(states, idx, n, L->obs_dim, t, d_values ? 2 : 1, x_amax_slot(L, act_buf, n), st);
 }
 
 // work: 6 activation tensors; rb200_mlp_fwd_scratch_floats(L, n) floats is always enough
@@ -856,30 +795,14 @@ extern "C" int rb200_mlp_sample(const rb200_mlp_layout* L, const float* params, 
                                 float* work, rb200_stream_t stream) {
   int e = check_layout(L);
   if (e) return e;
-  if (!params || !states || !action || !logprobs || !work) return RB200_E_NULL;
+  if (!params || !wsplit || !states || !action || !logprobs || !work) return RB200_E_NULL;
   if (n <= 0) return RB200_E_SHAPE;
   cudaStream_t st = rb::as_stream(stream);
-  const int64_t PF = act_floats(n);
-  float *H1 = work, *H2 = H1 + PF, *H3 = H2 + PF, *G1 = H3 + PF, *G2 = G1 + PF, *G3 = G2 + PF;
-  const float* P = params;
-  if (wsplit) {  // both towers in one grouped launch per layer
-    TowerIO t[2] = {};
-    t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
-    t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
-    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, x_amax_slot(L, work, n), nullptr, st))) return e;
-  } else {
-    if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
-    if (values && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
-  }
+  if ((e = forward_towers(L, params, wsplit, states, nullptr, n, true, values != nullptr, work, nullptr, st))) return e;
   HeadFwdArgs h{};
-  h.h3 = H3; h.g3 = values ? G3 : nullptr; h.mw = P + L->mw; h.mb = P + L->mb;
-  h.logstd = P + L->logstd; h.vw3 = P + L->vw3; h.noise = noise; h.seed = seed; h.offset = offset;
-  h.counter = counter_dev; h.sample_mode = 1; h.action_out = action; h.logprobs = logprobs; h.values = values; h.n = n;
-  h.act = L->act_dim; h.vdim = L->value_dim;
-  const size_t smem = sizeof(float) * (size_t)(L->act_dim + L->value_dim) * kH;
-  head_fwd_kernel<<<head_grid(n), 256, smem, st>>>(h);
-  rb::count_launch();
-  RB_RETURN_LAUNCH();
+  h.noise = noise; h.seed = seed; h.offset = offset; h.counter = counter_dev; h.sample_mode = 1; h.action_out = action;
+  h.logprobs = logprobs;
+  return head_forward(L, params, work, n, values, h, st);
 }
 
 // Eval-mode inference (rb200_mlp_mean in eval.cu): actor tower (+ value tower when values != null) and the head with
@@ -889,26 +812,10 @@ int mlp_mean_forward(const rb200_mlp_layout* L, const float* params, const float
                      int64_t n, float* action, float* logprobs, float* values, float* work, cudaStream_t st) {
   int e = check_layout(L);
   if (e) return e;
-  const int64_t PF = act_floats(n);
-  float *H1 = work, *H2 = H1 + PF, *H3 = H2 + PF, *G1 = H3 + PF, *G2 = G1 + PF, *G3 = G2 + PF;
-  const float* P = params;
-  if (wsplit) {
-    TowerIO t[2] = {};
-    t[0].w = tower_w(L, P, false); t[0].wh = tower_wh(L, wsplit, false); t[0].H1 = H1; t[0].H2 = H2; t[0].H3 = H3;
-    t[1].w = tower_w(L, P, true);  t[1].wh = tower_wh(L, wsplit, true);  t[1].H1 = G1; t[1].H2 = G2; t[1].H3 = G3;
-    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, values ? 2 : 1, x_amax_slot(L, work, n), nullptr, st))) return e;
-  } else {
-    if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, false), H1, H2, H3, st))) return e;
-    if (values && (e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, P, true), G1, G2, G3, st))) return e;
-  }
+  if ((e = forward_towers(L, params, wsplit, states, nullptr, n, true, values != nullptr, work, nullptr, st))) return e;
   HeadFwdArgs h{};
-  h.h3 = H3; h.g3 = values ? G3 : nullptr; h.mw = P + L->mw; h.mb = P + L->mb;
-  h.logstd = P + L->logstd; h.vw3 = P + L->vw3; h.sample_mode = 2; h.action_out = action; h.logprobs = logprobs;
-  h.values = values; h.n = n; h.act = L->act_dim; h.vdim = L->value_dim;
-  const size_t smem = sizeof(float) * (size_t)(L->act_dim + (values ? L->value_dim : 0)) * kH;
-  head_fwd_kernel<<<head_grid(n), 256, smem, st>>>(h);
-  rb::count_launch();
-  RB_RETURN_LAUNCH();
+  h.sample_mode = 2; h.action_out = action; h.logprobs = logprobs;
+  return head_forward(L, params, work, n, values, h, st);
 }
 }  // namespace rb
 
@@ -940,24 +847,16 @@ __global__ void __launch_bounds__(256) value_head_kernel(const float* __restrict
 }
 }  // namespace
 
-// work: rb200_mlp_fwd_scratch_floats(L, n) floats (3 activation tensors and the max|X| slot behind the 6 of the header)
+// work: rb200_mlp_fwd_scratch_floats(L, n) floats, laid out as acts (the value tower's activations and the x_amax slot)
 extern "C" int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, const float* wsplit,
                                const float* states, int64_t n, float* values, float* work, rb200_stream_t stream) {
   int e = check_layout(L);
   if (e) return e;
-  if (!params || !states || !values || !work) return RB200_E_NULL;
+  if (!params || !wsplit || !states || !values || !work) return RB200_E_NULL;
   if (n <= 0 || L->value_dim <= 0) return RB200_E_SHAPE;
   cudaStream_t st = rb::as_stream(stream);
-  const int64_t PF = act_floats(n);
-  float *G1 = work, *G2 = G1 + PF, *G3 = G2 + PF;
-  if (wsplit) {
-    TowerIO t[1] = {};
-    t[0].w = tower_w(L, params, true); t[0].wh = tower_wh(L, wsplit, true); t[0].H1 = G1; t[0].H2 = G2; t[0].H3 = G3;
-    if ((e = towers_forward_h(states, nullptr, n, L->obs_dim, t, 1, x_amax_slot(L, work, n), nullptr, st))) return e;
-  } else if ((e = tower_forward(states, nullptr, n, L->obs_dim, tower_w(L, params, true), G1, G2, G3, st))) {
-    return e;
-  }
-  value_head_kernel<<<head_grid(n), 256, 0, st>>>(G3, params + L->vw3, values, n, L->value_dim);
+  if ((e = forward_towers(L, params, wsplit, states, nullptr, n, false, true, work, nullptr, st))) return e;
+  value_head_kernel<<<head_grid(n), 256, 0, st>>>(work + 5 * act_floats(n), params + L->vw3, values, n, L->value_dim);
   rb::count_launch();
   RB_RETURN_LAUNCH();
 }

@@ -1,8 +1,9 @@
-// fp32 SIMT GEMM used by the MLP towers and the synthetic env (exact fp32 FMA accumulation).
+// fp32 SIMT GEMM (exact fp32 FMA accumulation) for the MLP towers' layer 0 where the tensor-core kernels do not take
+// the shape (row gather, obs % 32 != 0, obs > 256 in the weight gradient) and for the synthetic env.
 // C[M,N] = epilogue( sum_k A(m,k) * B(k,n) ), 128x128x8 tiles, 256 threads, 8x8 micro-tile per thread,
 // register-prefetched double-buffered shared memory.  Operand layouts are template parameters so the same
-// kernel serves forward (X.W^T), dgrad (dZ.W) and wgrad (dZ^T.H, split over the sample axis: atomics, or one stored
-// partial per split that the caller sums in split order).
+// kernel serves the forward (X.W^T) and the weight gradient (dZ^T.X, split over the sample axis: one stored partial per
+// split that the caller sums in split order).
 #pragma once
 #include "common.cuh"
 
@@ -13,21 +14,17 @@ constexpr int BM = 128, BN = 128, BK = 8, NT = 256;
 
 enum AMode { A_KCONTIG = 0, A_MCONTIG = 1 };  // A(m,k) stored [M,K] (k fastest) or [K,M] (m fastest)
 enum BMode { B_KCONTIG = 0, B_NCONTIG = 1 };  // B(k,n) stored [N,K] (k fastest) or [K,N] (n fastest)
-enum Epi { EPI_BIAS_TANH = 0, EPI_TANHGRAD = 1, EPI_ATOMIC = 2, EPI_STORE = 3 };
+enum Epi { EPI_BIAS_TANH = 0, EPI_STORE = 1 };
 
 struct GemmArgs {
   const float* A;
   const float* B;
-  const float* A2;  // optional second addend of the A operand (hi/lo split storage): A := A + A2, same layout
-  const float* B2;  // optional second addend of the B operand
   float* C;
-  const int64_t* a_rows;  // optional row gather for A (A_KCONTIG) or for B rows r (wgrad layer 1: B_NCONTIG rows)
+  const int64_t* a_rows;  // optional row gather for A (A_KCONTIG) or for B rows r (wgrad layer 0: B_NCONTIG rows)
   const int64_t* b_rows;
   const float* bias;  // [N]          (EPI_BIAS_TANH)
-  const float* aux;   // [M, ldaux]   (EPI_TANHGRAD: previous activation h, out = acc * (1 - h^2))
-  const float* aux2;  // optional second addend of aux (hi/lo split storage)
   int64_t M;          // rows of C; for the wgrad form this is N_out and K is the (huge) reduction over samples
-  int N, lda, ldb, ldc, ldaux;
+  int N, lda, ldb, ldc;
   int64_t K;
   int64_t k_per_split;  // reduction range per blockIdx.z
   int64_t c_split_stride;  // EPI_STORE: split z writes its partial to C + z * c_split_stride (0: all splits share C)
@@ -43,8 +40,6 @@ __device__ __forceinline__ float4 ld4(const float* p, bool vec, int valid) {
   if (valid > 3) r.w = p[3];
   return r;
 }
-
-__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
 
 template <int AM, int BMODE, int EPI>
 __global__ void __launch_bounds__(NT) sgemm_kernel(GemmArgs p) {
@@ -65,31 +60,22 @@ __global__ void __launch_bounds__(NT) sgemm_kernel(GemmArgs p) {
   const int b_col = (BMODE == B_KCONTIG) ? (tid >> 1) : ((tid & 31) * 4);
   const int b_k = (BMODE == B_KCONTIG) ? ((tid & 1) * 4) : (tid >> 5);
 
-  const bool a_vec_ok = ((p.lda & 3) == 0) && (((reinterpret_cast<uintptr_t>(p.A) | reinterpret_cast<uintptr_t>(p.A2)) & 15) == 0);
-  const bool b_vec_ok = ((p.ldb & 3) == 0) && (((reinterpret_cast<uintptr_t>(p.B) | reinterpret_cast<uintptr_t>(p.B2)) & 15) == 0);
+  const bool a_vec_ok = ((p.lda & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.A) & 15) == 0);
+  const bool b_vec_ok = ((p.ldb & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.B) & 15) == 0);
 
   const float* a_ptr = nullptr;  // A_KCONTIG: row base pointer (fixed over k)
-  const float* a_ptr2 = nullptr;
   bool a_row_ok = false;
   if (AM == A_KCONTIG) {
     const int64_t m = m0 + a_row;
     a_row_ok = m < p.M;
-    if (a_row_ok) {
-      const int64_t src = p.a_rows ? p.a_rows[m] : m;
-      a_ptr = p.A + src * p.lda;
-      if (p.A2) a_ptr2 = p.A2 + src * p.lda;
-    }
+    if (a_row_ok) a_ptr = p.A + (p.a_rows ? p.a_rows[m] : m) * p.lda;
   }
   const float* b_ptr = nullptr;
-  const float* b_ptr2 = nullptr;
   bool b_col_ok = false;
   if (BMODE == B_KCONTIG) {
     const int n = n0 + b_col;
     b_col_ok = n < p.N;
-    if (b_col_ok) {
-      b_ptr = p.B + (int64_t)n * p.ldb;
-      if (p.B2) b_ptr2 = p.B2 + (int64_t)n * p.ldb;
-    }
+    if (b_col_ok) b_ptr = p.B + (int64_t)n * p.ldb;
   }
 
   auto load_a = [&](int64_t k0) -> float4 {
@@ -97,18 +83,14 @@ __global__ void __launch_bounds__(NT) sgemm_kernel(GemmArgs p) {
       const int64_t k = k0 + a_k;
       if (!a_row_ok || k >= kend) return make_float4(0.f, 0.f, 0.f, 0.f);
       const int valid = (int)((kend - k) < 4 ? (kend - k) : 4);
-      float4 v = ld4(a_ptr + k, a_vec_ok && valid == 4, valid);
-      if (a_ptr2) v = add4(v, ld4(a_ptr2 + k, a_vec_ok && valid == 4, valid));
-      return v;
+      return ld4(a_ptr + k, a_vec_ok && valid == 4, valid);
     } else {  // A(m,k) = A[k*lda + m], m fastest. k is the reduction index (sample row for wgrad)
       const int64_t k = k0 + a_k;
       const int64_t m = m0 + a_row;
       if (k >= kend || m >= p.M) return make_float4(0.f, 0.f, 0.f, 0.f);
       const int64_t src = p.a_rows ? p.a_rows[k] : k;
       const int valid = (int)((p.M - m) < 4 ? (p.M - m) : 4);
-      float4 v = ld4(p.A + src * p.lda + m, a_vec_ok && valid == 4, valid);
-      if (p.A2) v = add4(v, ld4(p.A2 + src * p.lda + m, a_vec_ok && valid == 4, valid));
-      return v;
+      return ld4(p.A + src * p.lda + m, a_vec_ok && valid == 4, valid);
     }
   };
   auto load_b = [&](int64_t k0) -> float4 {
@@ -116,18 +98,14 @@ __global__ void __launch_bounds__(NT) sgemm_kernel(GemmArgs p) {
       const int64_t k = k0 + b_k;
       if (!b_col_ok || k >= kend) return make_float4(0.f, 0.f, 0.f, 0.f);
       const int valid = (int)((kend - k) < 4 ? (kend - k) : 4);
-      float4 v = ld4(b_ptr + k, b_vec_ok && valid == 4, valid);
-      if (b_ptr2) v = add4(v, ld4(b_ptr2 + k, b_vec_ok && valid == 4, valid));
-      return v;
+      return ld4(b_ptr + k, b_vec_ok && valid == 4, valid);
     } else {  // B(k,n) = B[k*ldb + n]
       const int64_t k = k0 + b_k;
       const int n = n0 + b_col;
       if (k >= kend || n >= p.N) return make_float4(0.f, 0.f, 0.f, 0.f);
       const int64_t src = p.b_rows ? p.b_rows[k] : k;
       const int valid = (p.N - n) < 4 ? (p.N - n) : 4;
-      float4 v = ld4(p.B + src * p.ldb + n, b_vec_ok && valid == 4, valid);
-      if (p.B2) v = add4(v, ld4(p.B2 + src * p.ldb + n, b_vec_ok && valid == 4, valid));
-      return v;
+      return ld4(p.B + src * p.ldb + n, b_vec_ok && valid == 4, valid);
     }
   };
   auto store_a = [&](int buf, float4 v) {
@@ -200,19 +178,8 @@ __global__ void __launch_bounds__(NT) sgemm_kernel(GemmArgs p) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         if (n + j >= p.N) continue;
-        float v = acc[i][jh * 4 + j];
-        float* dst = p.C + blockIdx.z * p.c_split_stride + m * p.ldc + n + j;
-        if (EPI == EPI_BIAS_TANH) {
-          v = tanhf(v + p.bias[n + j]);
-          *dst = v;
-        } else if (EPI == EPI_TANHGRAD) {
-          const float h = p.aux[m * p.ldaux + n + j] + (p.aux2 ? p.aux2[m * p.ldaux + n + j] : 0.f);
-          *dst = v * (1.0f - h * h);
-        } else if (EPI == EPI_ATOMIC) {
-          atomicAdd(dst, v);
-        } else {
-          *dst = v;
-        }
+        const float v = acc[i][jh * 4 + j];
+        p.C[blockIdx.z * p.c_split_stride + m * p.ldc + n + j] = EPI == EPI_BIAS_TANH ? tanhf(v + p.bias[n + j]) : v;
       }
     }
   }

@@ -387,7 +387,7 @@ int dgrad_wgrad(const BackwardLaunch* L, int ngroups, int64_t n, cudaStream_t st
   GemmLaunch d[2];
   for (int g = 0; g < ngroups; ++g) {
     w[g] = WgradLaunch{L[g].z, L[g].h, L[g].dW, L[g].amax_in};
-    d[g] = GemmLaunch{L[g].z, L[g].wpack, nullptr, L[g].dzprev, nullptr, L[g].h, L[g].colsum, L[g].amax_in, L[g].amax_out};
+    d[g] = GemmLaunch{L[g].z, L[g].wpack, L[g].dzprev, nullptr, L[g].h, L[g].colsum, L[g].amax_in, L[g].amax_out};
   }
   int e = wgrad(w, ngroups, n, BN, st);
   return e ? e : launch(d, ngroups, n, BN, rb::tc::EPI_TANHGRAD, 1, st);

@@ -23,7 +23,6 @@ struct GemmLaunch {        // one group (tower) of a forward / dgrad launch
   const float* b_hi;       // PACKED fp16 weight tiles of w * 2^10 for this launch's mode (pack_weights): per k-block of 32
                            // one contiguous 32 KB block = hi tile | lo tile, pre-swizzled as the MMA reads them; b_mn = 0
                            // takes the forward pack, b_mn = 1 the dgrad pack
-  const float* b_lo;       // unused (kept for the aggregate initialisers)
   float* c;                // [M,256] fp32 result
   const float* bias;       // EPI_BIAS_TANH
   const float* h;          // EPI_TANHGRAD: previous activation [M,256]

@@ -635,7 +635,7 @@ extern "C" int rb200_tc_gemm_h(const float* A, const float* B, float* C, int64_t
   int e = rb::tch::split_weights(&sp, 1, st);
   if (e) return e;
   rb::tch::GemmLaunch l{};
-  l.a = A; l.b_hi = dgrad ? sp.lo : sp.hi; l.b_lo = nullptr; l.c = C; l.amax_in = amax;
+  l.a = A; l.b_hi = dgrad ? sp.lo : sp.hi; l.c = C; l.amax_in = amax;
   if (mode == 0 && K <= rb::tc::BN) return rb::tch::forward(&l, 1, M, K, rb::tc::EPI_STORE, st);
   return rb::tch::launch(&l, 1, M, K, rb::tc::EPI_STORE, dgrad ? 1 : 0, st);
 }

@@ -400,6 +400,44 @@ def test_tc_gemm_h_forward_long_k(K, grad_like):
     assert err < 2e-6, err
 
 
+def test_mlp_entries_require_the_weight_cache():
+    """Every MLP entry returns RB200_E_NULL for wsplit = NULL: the towers run only with the tensor-core weight cache.
+    The buffers are real and sized as the entries require (the same calls with the cache succeed), so an entry that
+    lacks the check launches on valid memory and fails the assertion instead."""
+    import ctypes as C
+
+    from rlinf_b200 import _lib as L
+
+    lib = L.load()
+    pol = _policy(42, "8/2")
+    n = 129
+    lay = C.byref(pol.layout)
+    nscr = lib.rb200_mlp_fwd_scratch_floats(lay, n)
+
+    def zeros(*shape):
+        return torch.zeros(*shape, device="cuda")
+
+    states, action, noise = zeros(n, pol.obs_dim), zeros(n, pol.act_dim), zeros(n, pol.act_dim)
+    logp, ent, vals = zeros(n, pol.act_dim), zeros(n, pol.act_dim), zeros(n, pol.value_dim)
+    acts, work = zeros(nscr), zeros(nscr)
+    P, G, st = L.ptr(pol.flat_params), L.ptr(pol.flat_grads), L.stream_ptr()
+    X, A, lp, en, v = L.ptr(states), L.ptr(action), L.ptr(logp), L.ptr(ent), L.ptr(vals)
+    calls = {  # in this order with the cache: the backward reads the forward's activations
+        "forward": lambda ws: lib.rb200_mlp_forward(lay, P, ws, X, A, None, n, lp, en, v, L.ptr(acts), L.ptr(work), None,
+                                                    st),
+        "backward": lambda ws: lib.rb200_mlp_backward(lay, P, ws, X, A, None, n, lp, en, v, L.ptr(acts), L.ptr(work), G,
+                                                      st),
+        "sample": lambda ws: lib.rb200_mlp_sample(lay, P, ws, X, L.ptr(noise), 0, 0, None, n, A, lp, v, L.ptr(work), st),
+        "value": lambda ws: lib.rb200_mlp_value(lay, P, ws, X, n, v, L.ptr(work), st),
+        "mean": lambda ws: lib.rb200_mlp_mean(lay, P, ws, X, n, A, lp, v, L.ptr(work), st),
+    }
+    for name, call in calls.items():
+        assert call(None) == -1, f"rb200_mlp_{name} with wsplit = NULL"  # RB200_E_NULL
+    for name, call in calls.items():
+        assert call(pol._ws()) == 0, f"rb200_mlp_{name} with the weight cache"
+    torch.cuda.synchronize()
+
+
 def test_runner_update_is_bit_reproducible_simt_layer0():
     """obs 42 keeps layer 0 on the SIMT kernels; one micro-batch of 16384 rows.  Two identical runners must end one
     iteration with identical parameters and Adam moments.  clip_grad is far above the gradient norm, so the clip
