@@ -459,6 +459,27 @@ int rb200_logits_logprob_entropy_bwd(const void* logits, int dtype, const int64_
                                      const float* grad_logprob, const float* grad_entropy, void* dlogits,
                                      int64_t d_batch_stride, int64_t d_row_stride, rb200_stream_t stream);
 
+/* The same log-probabilities and entropies fused into the LM-head GEMM (csrc/lmhead.cu): z = (X . W^T) * inv_T from
+ * the last hidden states X (bf16, row r at hidden + (r / L) * batch_stride + (r % L) * row_stride, strides multiples of
+ * 8 elements) and the LM-head weight W [V, H] (bf16 row-major, no bias), H % 64 == 0, 64 <= H <= 8192; the logits are
+ * never stored.  Window, temperature, target handling and outputs as in rb200_logits_logprob_entropy_*.
+ * workspace: device memory of workspace_bytes (16-byte aligned).  rb200_lmhead_workspace_bytes() returns what the
+ * forward and a backward with vocabulary chunks of vocab_chunk columns (<= 0: the whole window) need, or -1 for an
+ * unsupported shape.  The backward derives its chunk from workspace_bytes: the whole window when its bf16 dZ [N, window]
+ * fits, else what fits after an fp32 [N, H] dX accumulator, in multiples of 256 columns (RB200_E_ARG below 256).
+ * Backward: d_hidden [N, H] and d_weight [V, H] bf16, contiguous, either nullable (not computed); d_weight rows outside
+ * the window are 0.  Deterministic: a fixed order, no atomics, nothing depends on the SM count. */
+int64_t rb200_lmhead_workspace_bytes(int64_t N, int64_t L, int H, int V, int v_lo, int v_hi, int64_t vocab_chunk);
+int rb200_lmhead_logprob_entropy_fwd(const void* hidden, const void* weight, const int64_t* target, int64_t N, int64_t L,
+                                     int64_t batch_stride, int64_t row_stride, int H, int V, int v_lo, int v_hi,
+                                     double inv_temperature, float* logprob, float* entropy, float* lse,
+                                     void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
+int rb200_lmhead_logprob_entropy_bwd(const void* hidden, const void* weight, const int64_t* target, int64_t N, int64_t L,
+                                     int64_t batch_stride, int64_t row_stride, int H, int V, int v_lo, int v_hi,
+                                     double inv_temperature, const float* lse, const float* entropy,
+                                     const float* grad_logprob, const float* grad_entropy, void* d_hidden,
+                                     void* d_weight, void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
+
 /* Value tower only: values [n,value_dim] = ValueHead(states). Used for the bootstrap value of
  * final observations (get_bootstrap_values, workers/rollout/hf/huggingface_worker.py:612-627). */
 int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, const float* wsplit,

@@ -85,4 +85,22 @@ int encode_f16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
 }
 }  // namespace tch
 
+namespace lmh {
+// bf16 [d2, d1, d0] with element strides (1, s1, s2) given in bytes, box [1, box1, box0 = 64] (one 128-byte SWIZZLE_128B
+// span); a 2-D matrix is d2 = 1.  Out-of-bounds parts of a box are zero-filled.
+int encode_bf16_sw128(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1_bytes,
+                      uint64_t s2_bytes, uint32_t box0, uint32_t box1) {
+  auto enc = get_encode();
+  if (!enc) return -1;
+  cuuint64_t gdim[3] = {d0, d1, d2};
+  cuuint64_t gstride[2] = {s1_bytes, s2_bytes};
+  cuuint32_t box[3] = {box0, box1, 1u};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstride, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+}  // namespace lmh
+
 }  // namespace rb

@@ -1,6 +1,6 @@
 // sm_90a wgmma wrappers: D[64 x N] (+)= A[64 x 16] . B[16 x N], fp16 in, fp32 accumulators in registers.  Mma: A from
 // registers (the m64k16 fragment of the PTX ISA), B from a descriptor (TB = 1: MN-major).  MmaSS: both from descriptors
-// (TA / TB = 1: MN-major; K-major by default).
+// (TA / TB = 1: MN-major; K-major by default); its element type E is f16 (default) or bf16.
 // Accumulator fragment: for each 8-column block j, d[4j + {0,1}] = (row g, cols 8j + 2t + {0,1}) and d[4j + {2,3}] =
 // (row g + 8, same cols), rows relative to 16 * (warp % 4), g = lane / 4, t = lane % 4.
 #pragma once
@@ -39,9 +39,12 @@ __device__ __forceinline__ uint64_t desc(uint32_t saddr, uint32_t lbo, uint32_t 
 #define RB_WG_D16(i) RB_WG_D4(i), RB_WG_D4(i + 4), RB_WG_D4(i + 8), RB_WG_D4(i + 12)
 #define RB_WG_D64(i) RB_WG_D16(i), RB_WG_D16(i + 16), RB_WG_D16(i + 32), RB_WG_D16(i + 48)
 
+struct f16;   // element-type tags of MmaSS
+struct bf16;
+
 template <int N, int TB>
 struct Mma;
-template <int N, int TA = 0, int TB = 0>
+template <int N, int TA = 0, int TB = 0, typename E = f16>
 struct MmaSS;
 
 template <int TB>
@@ -73,7 +76,7 @@ struct Mma<256, TB> {
 };
 
 template <int TA, int TB>
-struct MmaSS<32, TA, TB> {
+struct MmaSS<32, TA, TB, f16> {
   __device__ __forceinline__ static void run(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {"
@@ -85,7 +88,7 @@ struct MmaSS<32, TA, TB> {
 };
 
 template <int TA, int TB>
-struct MmaSS<64, TA, TB> {
+struct MmaSS<64, TA, TB, f16> {
   __device__ __forceinline__ static void run(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
@@ -97,10 +100,23 @@ struct MmaSS<64, TA, TB> {
 };
 
 template <int TA, int TB>
-struct MmaSS<128, TA, TB> {
+struct MmaSS<128, TA, TB, f16> {
   __device__ __forceinline__ static void run(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+                 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+                 "}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+                 : RB_WG_D64(0)
+                 : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
+
+template <int TA, int TB>
+struct MmaSS<128, TA, TB, bf16> {
+  __device__ __forceinline__ static void run(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
                  "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
                  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
                  "}, %64, %65, p, 1, 1, %67, %68;\n}\n"

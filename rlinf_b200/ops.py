@@ -464,3 +464,120 @@ def compute_entropy_from_logits(logits, dim: int = -1):
         raise ValueError("compute_entropy_from_logits: only the last (vocabulary) dimension is supported")
     tgt = torch.zeros(logits.shape[:-1], dtype=torch.int64, device=logits.device)
     return logprobs_entropy_from_logits(logits, tgt, compute_entropy=True)[1]
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The same, fused into the LM-head GEMM: hidden states and lm_head.weight in, no logits tensor (csrc/lmhead.cu)
+# ---------------------------------------------------------------------------------------------------------------
+LMHEAD_DZ_BUDGET = 1 << 30  # bytes of the backward's bf16 dZ chunk [N, Vc]
+
+
+def _lmhead_check(hidden: torch.Tensor, weight: torch.Tensor):
+    if hidden.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16:
+        raise ValueError(f"linear_logprobs_entropy: hidden and weight must be bfloat16, got {hidden.dtype} / {weight.dtype}")
+    if weight.dim() != 2:
+        raise ValueError(f"linear_logprobs_entropy: weight must be [V, H], got shape {tuple(weight.shape)}")
+    H = weight.shape[1]
+    if hidden.shape[-1] != H:
+        raise ValueError(f"linear_logprobs_entropy: hidden size {hidden.shape[-1]} != weight's {H}")
+    if H % 64 != 0 or not 64 <= H <= 8192:
+        raise ValueError(f"linear_logprobs_entropy: needs H % 64 == 0 and 64 <= H <= 8192, got H = {H}")
+    if not (hidden.is_cuda and weight.is_cuda):
+        raise L.Rb200Error("rlinf_b200 kernels take CUDA tensors; move inputs with to_device() first")
+
+
+def _lmhead_geometry(hidden: torch.Tensor):
+    """(tensor, N, L, batch_stride, row_stride) of [N, H] or [bsz, L, H] hidden states: addressed in place when the last
+    dim is contiguous, the other strides are multiples of 8 elements and the base is 16-byte aligned (e.g. the slice
+    `hidden[:, -L-1:-1, :]`); anything else is made contiguous first."""
+    H = hidden.shape[-1]
+    if hidden.dim() in (2, 3) and hidden.stride(-1) == 1 and hidden.data_ptr() % 16 == 0:
+        if hidden.dim() == 2 and hidden.stride(0) % 8 == 0 and hidden.stride(0) >= H:
+            return hidden, hidden.shape[0], hidden.shape[0], hidden.shape[0] * hidden.stride(0), hidden.stride(0)
+        if hidden.dim() == 3 and hidden.stride(1) % 8 == 0 and hidden.stride(1) >= H and hidden.stride(0) % 8 == 0:
+            bsz, Lr, _ = hidden.shape
+            return hidden, bsz * Lr, Lr, hidden.stride(0), hidden.stride(1)
+    x = hidden.reshape(-1, H).contiguous()
+    return x, x.shape[0], x.shape[0], x.shape[0] * H, H
+
+
+def lmhead_workspace_bytes(N: int, L_rows: int, H: int, V: int, lo: int, hi: int, vocab_chunk: int = 0) -> int:
+    """Workspace of the fused LM-head log-prob kernels (forward, and a backward in chunks of vocab_chunk columns;
+    0 = the whole window)."""
+    n = L.load().rb200_lmhead_workspace_bytes(N, L_rows, H, V, lo, hi, vocab_chunk)
+    if n < 0:
+        raise ValueError(f"linear_logprobs_entropy: unsupported shape N={N} L={L_rows} H={H} V={V} window=[{lo}, {hi})")
+    return int(n)
+
+
+def _lmhead_chunk(N: int, lo: int, hi: int) -> int:
+    """dZ chunk width under LMHEAD_DZ_BUDGET: the whole window if it fits, multiples of 256 columns otherwise."""
+    whole = -(-(hi - lo) // 256) * 256
+    fit = max(256, LMHEAD_DZ_BUDGET // (2 * N) // 256 * 256)
+    return min(whole, fit)
+
+
+class _LinearLogprobEntropy(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, hidden, weight, target, temperature, window, want_entropy):
+        _lmhead_check(hidden, weight)
+        lib = L.load()
+        x, N, Lr, bs, rs = _lmhead_geometry(hidden)
+        w = weight.contiguous()
+        V, H = w.shape
+        tgt = L.to_device(target, x.device, torch.int64).reshape(-1).contiguous()
+        if tgt.numel() != N:
+            raise ValueError(f"target has {tgt.numel()} entries for {N} hidden rows")
+        lo, hi = (0, V) if window is None else (int(window[0]), int(window[1]))
+        if not 0 <= lo < hi <= V:
+            raise ValueError(f"linear_logprobs_entropy: window [{lo}, {hi}) must lie inside [0, {V}) and be non-empty")
+        vc = _lmhead_chunk(N, lo, hi)
+        wsb = lmhead_workspace_bytes(N, Lr, H, V, lo, hi, vc)
+        ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+        lp = torch.empty(N, dtype=torch.float32, device=x.device)
+        ent = torch.empty(N, dtype=torch.float32, device=x.device) if want_entropy else None
+        lse = torch.empty(N, dtype=torch.float32, device=x.device)
+        L.check(lib.rb200_lmhead_logprob_entropy_fwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo, hi,
+                                                     1.0 / float(temperature), L.ptr(lp), L.ptr(ent), L.ptr(lse),
+                                                     L.ptr(ws), wsb, L.stream_ptr(x.device)),
+                "lmhead_logprob_entropy_fwd")
+        del ws
+        ctx.save_for_backward(x, w, tgt, lse, ent if want_entropy else lse)
+        ctx.meta = (N, Lr, bs, rs, H, V, lo, hi, vc, float(temperature), want_entropy, tuple(hidden.shape))
+        shape = hidden.shape[:-1]
+        if want_entropy:
+            return lp.view(shape), ent.view(shape)
+        none = lp.new_zeros(())
+        ctx.mark_non_differentiable(none)
+        return lp.view(shape), none
+
+    @staticmethod
+    def backward(ctx, g_lp, g_ent):
+        lib = L.load()
+        x, w, tgt, lse, ent = ctx.saved_tensors
+        N, Lr, bs, rs, H, V, lo, hi, vc, temp, want_entropy, shape = ctx.meta
+        need_x, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (need_x or need_w):
+            return None, None, None, None, None, None
+        glp = g_lp.reshape(-1).float().contiguous() if g_lp is not None else None
+        gh = g_ent.reshape(-1).float().contiguous() if (want_entropy and g_ent is not None) else None
+        dx = torch.empty((N, H), dtype=torch.bfloat16, device=x.device) if need_x else None
+        dw = torch.empty((V, H), dtype=torch.bfloat16, device=x.device) if need_w else None
+        wsb = lmhead_workspace_bytes(N, Lr, H, V, lo, hi, vc)
+        ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+        L.check(lib.rb200_lmhead_logprob_entropy_bwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo, hi,
+                                                     1.0 / temp, L.ptr(lse), L.ptr(ent) if gh is not None else None,
+                                                     L.ptr(glp), L.ptr(gh), L.ptr(dx), L.ptr(dw), L.ptr(ws), wsb,
+                                                     L.stream_ptr(x.device)),
+                "lmhead_logprob_entropy_bwd")
+        return (dx.view(shape) if need_x else None), dw, None, None, None, None
+
+
+def linear_logprobs_entropy(hidden, weight, target, temperature: float = 1.0, window=None, compute_entropy: bool = True):
+    """logprobs_entropy_from_logits(hidden @ weight.T, ...) without the logits tensor: `hidden` [N, H] or [bsz, L, H]
+    (e.g. the last hidden state's `[:, -L-1:-1, :]` slice, read in place) and `weight` = lm_head.weight [V, H], both
+    bf16, H % 64 == 0.  Temperature and the vocabulary window [lo, hi) act as in logprobs_entropy_from_logits.
+    Differentiable w.r.t. hidden and weight (only the gradients whose inputs require them are computed).
+    Returns (logprobs [...], entropy [...] or None), fp32."""
+    lp, ent = _LinearLogprobEntropy.apply(hidden, weight, target, temperature, window, bool(compute_entropy))
+    return lp, (ent if compute_entropy else None)
