@@ -480,6 +480,45 @@ int rb200_lmhead_logprob_entropy_bwd(const void* hidden, const void* weight, con
                                      const float* grad_logprob, const float* grad_entropy, void* d_hidden,
                                      void* d_weight, void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
 
+/* Vocabulary-parallel (tensor-parallel) variants of the two ops above (csrc/vocab_parallel.cu, lmhead.cu, logits.cu).
+ * Equal shards (Megatron's VocabUtility; the vocabulary is padded so that P divides it): rank k of P owns the global
+ * vocabulary columns [vocab_start, vocab_start + Vs), vocab_start = k * Vs; its weight shard is W[k*Vs:(k+1)*Vs] [Vs, H],
+ * its logits shard [..., Vs].  target holds global ids; [v_lo, v_hi) is the global window, 0 <= v_lo < v_hi <= P * Vs,
+ * and each rank uses its intersection with the shard.
+ * Record: each rank writes one 16-byte record per row, float4 {m, s, t, z_t} [N, 4] (16-byte aligned): the softmax
+ * statistics of softmax_acc.cuh over the rank's part of the window (max m, s = sum e^(z-m), t = sum e^(z-m) (z-m)),
+ * and z_t = the scaled logit of the target column if the rank owns it and it lies in the window, else 0.  A rank whose
+ * shard misses the window writes {-inf, 0, 0, 0} and launches no row pass.
+ * rb200_vp_combine: the gathered records [n_ranks, N, 4] (rank-major, rank 0 first) -> logprob / entropy / lse [N] as
+ * the single-GPU ops write them (entropy, lse nullable).  Rows are merged in rank order and z_t comes from rank
+ * target / Vs, so every rank that combines the same records gets the same bits; with one rank the results are
+ * bit-identical to rb200_lmhead_logprob_entropy_fwd / rb200_logits_logprob_entropy_fwd.
+ * rb200_lmhead_vp_logprob_entropy_bwd: the single-GPU backward on the shard, given the global lse / entropy of the
+ * combine: d_weight_shard [Vs, H] bf16 (rows outside the window 0) and d_hidden_partial [N, H] **fp32**, the rank's
+ * share of dX for the caller to sum over ranks (so the sum rounds once, in the caller's final bf16 cast); either
+ * nullable.  Its vocabulary chunk comes from workspace_bytes as in rb200_lmhead_logprob_entropy_bwd, with no fp32
+ * accumulator (d_hidden_partial is it).  rb200_lmhead_vp_workspace_bytes() sizes the workspace of both lmhead entries
+ * (vocab_chunk 0: the shard's whole part of the window in one chunk; < 0: the forward's workspace only).
+ * The logits-level backward is rb200_logits_logprob_entropy_bwd on the shard with the global lse / entropy, the local
+ * window and the shard-local target (target - vocab_start; values outside [0, Vs) get no target term). */
+int64_t rb200_lmhead_vp_workspace_bytes(int64_t N, int64_t L, int H, int Vs, int64_t vocab_start, int v_lo, int v_hi,
+                                        int64_t vocab_chunk);
+int rb200_lmhead_vp_partials_fwd(const void* hidden, const void* weight_shard, const int64_t* target, int64_t N,
+                                 int64_t L, int64_t batch_stride, int64_t row_stride, int H, int Vs,
+                                 int64_t vocab_start, int v_lo, int v_hi, double inv_temperature, float* record,
+                                 void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
+int rb200_lmhead_vp_logprob_entropy_bwd(const void* hidden, const void* weight_shard, const int64_t* target,
+                                        int64_t N, int64_t L, int64_t batch_stride, int64_t row_stride, int H, int Vs,
+                                        int64_t vocab_start, int v_lo, int v_hi, double inv_temperature,
+                                        const float* lse, const float* entropy, const float* grad_logprob,
+                                        const float* grad_entropy, float* d_hidden_partial, void* d_weight_shard,
+                                        void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
+int rb200_logits_vp_partials_fwd(const void* logits, int dtype, const int64_t* target, int64_t N, int64_t L,
+                                 int64_t batch_stride, int64_t row_stride, int Vs, int64_t vocab_start, int v_lo,
+                                 int v_hi, double inv_temperature, float* record, rb200_stream_t stream);
+int rb200_vp_combine(const float* records, int n_ranks, int64_t N, const int64_t* target, int vocab_shard, int v_lo,
+                     int v_hi, float* logprob, float* entropy, float* lse, rb200_stream_t stream);
+
 /* Value tower only: values [n,value_dim] = ValueHead(states). Used for the bootstrap value of
  * final observations (get_bootstrap_values, workers/rollout/hf/huggingface_worker.py:612-627). */
 int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, const float* wsplit,

@@ -453,7 +453,101 @@ int check_ptrs(const void* hidden, const void* weight, const void* target, const
   return RB200_OK;
 }
 
+// the FWD pass over [g.v_lo, g.v_hi): per-range partials at P.part, the target's z at P.zt (workspace)
+int fwd_partials(Params& P, const Geo& g, const void* hidden, const void* weight, const int64_t* target,
+                 double inv_temperature, void* workspace, cudaStream_t st) {
+  P = Params{};
+  base_params(P, g, inv_temperature);
+  if (x_map(&P.a, hidden, g, BM) || w_map(&P.b, weight, g, BN)) return RB200_E_UNSUPPORTED;
+  P.n_kb = g.H / BK;
+  P.n_ranges = g.n_ranges; P.tiles_per_range = g.tiles_per_range; P.n_vtiles = g.n_vtiles;
+  P.target = target;
+  P.part = static_cast<float*>(workspace);
+  P.zt = P.part + (size_t)g.n_ranges * g.N * 3;
+  return launch<FWD>(P, (int)(g.row_tiles * g.n_ranges), st);
+}
+
+// vocabulary chunk of the backward from the workspace: the whole window if its dZ fits, else what is left after an
+// fp32 [N, H] dX accumulator (dx_acc_bytes), in whole 256-column tiles; 0 when not even one tile fits
+int64_t bwd_chunk(const Geo& g, int64_t workspace_bytes, int64_t dx_acc_bytes) {
+  const int64_t whole = cdiv(g.v_hi - g.v_lo, BN) * BN;
+  if (workspace_bytes >= dz_ws_bytes(g, whole)) return whole;
+  const int64_t vc = (workspace_bytes - dx_acc_bytes) / (2 * g.N) / BN * BN;
+  return vc < BN ? 0 : vc;
+}
+
+// The backward over [g.v_lo, g.v_hi) in chunks of vc columns.  dX is summed in fp32 in dx_acc over the chunks; with dx
+// the last chunk writes it there in bf16 instead, without dx it stays in dx_acc.
+int bwd_chunks(const Geo& g, const void* hidden, const void* weight, const int64_t* target, double inv_temperature,
+               const float* lse, const float* entropy, const float* grad_logprob, const float* grad_entropy, int64_t vc,
+               __nv_bfloat16* dz, float* dx_acc, __nv_bfloat16* dx, __nv_bfloat16* dw, cudaStream_t st) {
+  const int H = g.H, V = g.V, v_lo = g.v_lo, v_hi = g.v_hi;
+  if (dw) {  // rows outside the window get no gradient
+    if (v_lo > 0) RB_CHECK_CUDA(cudaMemsetAsync(dw, 0, (size_t)v_lo * H * 2, st));
+    if (v_hi < V) RB_CHECK_CUDA(cudaMemsetAsync(dw + (size_t)v_hi * H, 0, (size_t)(V - v_hi) * H * 2, st));
+  }
+  const int n_ntiles = (int)cdiv(H, BN);
+  int e;
+  for (int64_t c0 = v_lo; c0 < v_hi; c0 += vc) {
+    const int width = (int)((v_hi - c0) < vc ? (v_hi - c0) : vc);
+    Params P{};
+    base_params(P, g, inv_temperature);
+    P.c0 = (int)c0; P.width = width; P.ld = (int)vc;
+    P.target = target; P.lse = lse; P.h_in = entropy; P.g_lp = grad_logprob; P.g_h = grad_entropy;
+    P.dz = dz; P.dx_acc = dx_acc; P.dx = dx; P.dw = dw;
+    P.n_ntiles = n_ntiles;
+    P.first = c0 == v_lo;
+    P.last = dx && c0 + width >= v_hi;
+    // (a) dZ of the chunk
+    Params A = P;
+    if (x_map(&A.a, hidden, g, BM) || w_map(&A.b, weight, g, BN)) return RB200_E_UNSUPPORTED;
+    A.n_kb = H / BK;
+    split_ranges(g.row_tiles, width, A.n_vtiles, A.n_ranges, A.tiles_per_range);
+    if ((e = launch<DZ>(A, (int)(g.row_tiles * A.n_ranges), st))) return e;
+    // (b) dW[c0 : c0 + width] = dZ^T . X over all rows
+    if (dw) {
+      Params B = P;
+      if (dz_map(&B.a, dz, g, width, vc, 64, 64) || x_map(&B.b, hidden, g, 64)) return RB200_E_UNSUPPORTED;
+      B.kpb = (int)cdiv(g.L, BK);
+      B.n_kb = (int)(g.bsz * B.kpb);
+      if ((e = launch<DW>(B, (int)(cdiv(width, BM) * n_ntiles), st))) return e;
+    }
+    // (c) dX (+)= dZ . W[c0 : c0 + width]
+    if (dx_acc || dx) {
+      Params C = P;
+      if (dz_map(&C.a, dz, g, width, vc, 64, BM) || w_map(&C.b, weight, g, 64)) return RB200_E_UNSUPPORTED;
+      C.n_kb = (int)cdiv(width, BK);
+      if ((e = launch<DX>(C, (int)(g.row_tiles * n_ntiles), st))) return e;
+    }
+  }
+  return RB200_OK;
+}
+
+// ---- vocabulary-parallel shard (rank k owns global columns [vocab_start, vocab_start + Vs)) ----
+// the shard's part of the global window [v_lo, v_hi), in shard columns; lo >= hi when the shard misses the window
+void shard_window(int64_t vocab_start, int Vs, int v_lo, int v_hi, int& lo, int& hi) {
+  const int64_t l = v_lo - vocab_start, h = v_hi - vocab_start;
+  lo = (int)(l < 0 ? 0 : (l > Vs ? Vs : l));
+  hi = (int)(h < 0 ? 0 : (h > Vs ? Vs : h));
+}
+// the shard-local targets (target - vocab_start) head the workspace; the kernels' own workspace follows
+int64_t vp_target_bytes(int64_t N) { return cdiv(N * 8, 256) * 256; }
+
+int vp_check(int Vs, int64_t vocab_start, int v_lo, int v_hi, double inv_temperature) {
+  if (Vs <= 0 || vocab_start < 0 || vocab_start % Vs != 0 || v_lo < 0 || v_lo >= v_hi) return RB200_E_SHAPE;
+  if (!(inv_temperature > 0.0)) return RB200_E_ARG;
+  return RB200_OK;
+}
+
 }  // namespace
+
+namespace rb {
+namespace vp {
+int shift_target(const int64_t* target, int64_t N, int64_t vocab_start, int64_t* out, cudaStream_t st);
+int range_record(const float* part, const float* zt, const int64_t* local_target, int64_t N, int n_ranges, int lo,
+                 int hi, float* rec, cudaStream_t st);
+}  // namespace vp
+}  // namespace rb
 
 extern "C" int64_t rb200_lmhead_workspace_bytes(int64_t N, int64_t L, int H, int V, int v_lo, int v_hi,
                                                 int64_t vocab_chunk) {
@@ -479,16 +573,8 @@ extern "C" int rb200_lmhead_logprob_entropy_fwd(const void* hidden, const void* 
   if ((e = make_geo(g, N, L, batch_stride, row_stride, H, V, v_lo, v_hi))) return e;
   if (workspace_bytes < fwd_ws_bytes(g)) return RB200_E_ARG;
   cudaStream_t st = rb::as_stream(stream);
-  Params P{};
-  base_params(P, g, inv_temperature);
-  if (x_map(&P.a, hidden, g, BM) || w_map(&P.b, weight, g, BN)) return RB200_E_UNSUPPORTED;
-  P.n_kb = H / BK;
-  P.n_ranges = g.n_ranges; P.tiles_per_range = g.tiles_per_range; P.n_vtiles = g.n_vtiles;
-  P.target = target;
-  P.part = static_cast<float*>(workspace);
-  P.zt = P.part + (size_t)g.n_ranges * N * 3;
-  e = launch<FWD>(P, (int)(g.row_tiles * g.n_ranges), st);
-  if (e) return e;
+  Params P;
+  if ((e = fwd_partials(P, g, hidden, weight, target, inv_temperature, workspace, st))) return e;
   combine_kernel<<<(unsigned)cdiv(N, 256), 256, 0, st>>>(P.part, P.zt, target, N, g.n_ranges, v_lo, v_hi, logprob,
                                                           entropy, lse);
   rb::count_launch();
@@ -509,56 +595,90 @@ extern "C" int rb200_lmhead_logprob_entropy_bwd(const void* hidden, const void* 
   Geo g;
   if ((e = make_geo(g, N, L, batch_stride, row_stride, H, V, v_lo, v_hi))) return e;
   if (!d_hidden && !d_weight) return RB200_OK;
-  // vocabulary chunk from the workspace: the whole window if its dZ fits, else what is left after the fp32 dX
-  // accumulator, in whole 256-column tiles
-  const int64_t whole = cdiv(v_hi - v_lo, BN) * BN;
-  int64_t vc;
-  if (workspace_bytes >= dz_ws_bytes(g, whole)) {
-    vc = whole;
-  } else {
-    vc = (workspace_bytes - (int64_t)N * H * 4) / (2 * N) / BN * BN;
-    if (vc < BN) return RB200_E_ARG;
-  }
-  cudaStream_t st = rb::as_stream(stream);
+  const int64_t vc = bwd_chunk(g, workspace_bytes, (int64_t)N * H * 4);
+  if (vc == 0) return RB200_E_ARG;
   __nv_bfloat16* dz = static_cast<__nv_bfloat16*>(workspace);
   float* dx_acc = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + dz_ws_bytes(g, vc));
-  __nv_bfloat16* dw = static_cast<__nv_bfloat16*>(d_weight);
-  if (dw) {  // rows outside the window get no gradient
-    if (v_lo > 0) RB_CHECK_CUDA(cudaMemsetAsync(dw, 0, (size_t)v_lo * H * 2, st));
-    if (v_hi < V) RB_CHECK_CUDA(cudaMemsetAsync(dw + (size_t)v_hi * H, 0, (size_t)(V - v_hi) * H * 2, st));
+  return bwd_chunks(g, hidden, weight, target, inv_temperature, lse, entropy, grad_logprob, grad_entropy, vc, dz,
+                    d_hidden ? dx_acc : nullptr, static_cast<__nv_bfloat16*>(d_hidden),
+                    static_cast<__nv_bfloat16*>(d_weight), rb::as_stream(stream));
+}
+
+extern "C" int64_t rb200_lmhead_vp_workspace_bytes(int64_t N, int64_t L, int H, int Vs, int64_t vocab_start, int v_lo,
+                                                   int v_hi, int64_t vocab_chunk) {
+  if (vp_check(Vs, vocab_start, v_lo, v_hi, 1.0)) return -1;
+  int lo, hi;
+  shard_window(vocab_start, Vs, v_lo, v_hi, lo, hi);
+  if (lo >= hi) {  // no mainloop: only the shape checks of a full shard
+    Geo g;
+    return make_geo(g, N, L, L * H, H, H, Vs, 0, Vs) != RB200_OK ? -1 : vp_target_bytes(N);
   }
-  const int n_ntiles = (int)cdiv(H, BN);
-  for (int64_t c0 = v_lo; c0 < v_hi; c0 += vc) {
-    const int width = (int)((v_hi - c0) < vc ? (v_hi - c0) : vc);
-    Params P{};
-    base_params(P, g, inv_temperature);
-    P.c0 = (int)c0; P.width = width; P.ld = (int)vc;
-    P.target = target; P.lse = lse; P.h_in = entropy; P.g_lp = grad_logprob; P.g_h = grad_entropy;
-    P.dz = dz; P.dx_acc = dx_acc; P.dx = static_cast<__nv_bfloat16*>(d_hidden); P.dw = dw;
-    P.n_ntiles = n_ntiles;
-    P.first = c0 == v_lo;
-    P.last = c0 + width >= v_hi;
-    // (a) dZ of the chunk
-    Params A = P;
-    if (x_map(&A.a, hidden, g, BM) || w_map(&A.b, weight, g, BN)) return RB200_E_UNSUPPORTED;
-    A.n_kb = H / BK;
-    split_ranges(g.row_tiles, width, A.n_vtiles, A.n_ranges, A.tiles_per_range);
-    if ((e = launch<DZ>(A, (int)(g.row_tiles * A.n_ranges), st))) return e;
-    // (b) dW[c0 : c0 + width] = dZ^T . X over all rows
-    if (dw) {
-      Params B = P;
-      if (dz_map(&B.a, dz, g, width, vc, 64, 64) || x_map(&B.b, hidden, g, 64)) return RB200_E_UNSUPPORTED;
-      B.kpb = (int)cdiv(g.L, BK);
-      B.n_kb = (int)(g.bsz * B.kpb);
-      if ((e = launch<DW>(B, (int)(cdiv(width, BM) * n_ntiles), st))) return e;
-    }
-    // (c) dX (+)= dZ . W[c0 : c0 + width]
-    if (d_hidden) {
-      Params C = P;
-      if (dz_map(&C.a, dz, g, width, vc, 64, BM) || w_map(&C.b, weight, g, 64)) return RB200_E_UNSUPPORTED;
-      C.n_kb = (int)cdiv(width, BK);
-      if ((e = launch<DX>(C, (int)(g.row_tiles * n_ntiles), st))) return e;
-    }
+  Geo g;
+  if (make_geo(g, N, L, L * H, H, H, Vs, lo, hi) != RB200_OK) return -1;
+  const int64_t f = fwd_ws_bytes(g);
+  if (vocab_chunk < 0) return vp_target_bytes(N) + f;
+  const int64_t whole = cdiv(hi - lo, BN) * BN;
+  int64_t vc = vocab_chunk == 0 ? whole : cdiv(vocab_chunk, BN) * BN;
+  if (vc > whole) vc = whole;
+  const int64_t b = dz_ws_bytes(g, vc);  // the backward's dX sum is the caller's fp32 output
+  return vp_target_bytes(N) + (f > b ? f : b);
+}
+
+extern "C" int rb200_lmhead_vp_partials_fwd(const void* hidden, const void* weight_shard, const int64_t* target,
+                                            int64_t N, int64_t L, int64_t batch_stride, int64_t row_stride, int H,
+                                            int Vs, int64_t vocab_start, int v_lo, int v_hi, double inv_temperature,
+                                            float* record, void* workspace, int64_t workspace_bytes,
+                                            rb200_stream_t stream) {
+  int e = check_ptrs(hidden, weight_shard, target, workspace);
+  if (e) return e;
+  if (!record || !workspace) return RB200_E_NULL;
+  if ((reinterpret_cast<uintptr_t>(record) & 15) != 0) return RB200_E_ALIGN;
+  if ((e = vp_check(Vs, vocab_start, v_lo, v_hi, inv_temperature))) return e;
+  int lo, hi;
+  shard_window(vocab_start, Vs, v_lo, v_hi, lo, hi);
+  Geo g;
+  if ((e = make_geo(g, N, L, batch_stride, row_stride, H, Vs, lo < hi ? lo : 0, lo < hi ? hi : Vs))) return e;
+  cudaStream_t st = rb::as_stream(stream);
+  if (lo >= hi) return rb::vp::range_record(nullptr, nullptr, nullptr, N, 0, 0, 0, record, st);
+  if (workspace_bytes < vp_target_bytes(N) + fwd_ws_bytes(g)) return RB200_E_ARG;
+  int64_t* local_target = static_cast<int64_t*>(workspace);
+  if ((e = rb::vp::shift_target(target, N, vocab_start, local_target, st))) return e;
+  Params P;
+  if ((e = fwd_partials(P, g, hidden, weight_shard, local_target, inv_temperature,
+                        static_cast<uint8_t*>(workspace) + vp_target_bytes(N), st)))
+    return e;
+  return rb::vp::range_record(P.part, P.zt, local_target, N, g.n_ranges, lo, hi, record, st);
+}
+
+extern "C" int rb200_lmhead_vp_logprob_entropy_bwd(const void* hidden, const void* weight_shard, const int64_t* target,
+                                                   int64_t N, int64_t L, int64_t batch_stride, int64_t row_stride,
+                                                   int H, int Vs, int64_t vocab_start, int v_lo, int v_hi,
+                                                   double inv_temperature, const float* lse, const float* entropy,
+                                                   const float* grad_logprob, const float* grad_entropy,
+                                                   float* d_hidden_partial, void* d_weight_shard, void* workspace,
+                                                   int64_t workspace_bytes, rb200_stream_t stream) {
+  int e = check_ptrs(hidden, weight_shard, target, workspace);
+  if (e) return e;
+  if (!lse || !workspace || (grad_entropy && !entropy)) return RB200_E_NULL;
+  if (((reinterpret_cast<uintptr_t>(d_hidden_partial) | reinterpret_cast<uintptr_t>(d_weight_shard)) & 7) != 0)
+    return RB200_E_ALIGN;
+  if ((e = vp_check(Vs, vocab_start, v_lo, v_hi, inv_temperature))) return e;
+  int lo, hi;
+  shard_window(vocab_start, Vs, v_lo, v_hi, lo, hi);
+  Geo g;
+  if ((e = make_geo(g, N, L, batch_stride, row_stride, H, Vs, lo < hi ? lo : 0, lo < hi ? hi : Vs))) return e;
+  if (!d_hidden_partial && !d_weight_shard) return RB200_OK;
+  cudaStream_t st = rb::as_stream(stream);
+  if (lo >= hi) {  // the shard misses the window: no gradient
+    if (d_hidden_partial) RB_CHECK_CUDA(cudaMemsetAsync(d_hidden_partial, 0, (size_t)N * H * 4, st));
+    if (d_weight_shard) RB_CHECK_CUDA(cudaMemsetAsync(d_weight_shard, 0, (size_t)Vs * H * 2, st));
+    return RB200_OK;
   }
-  return RB200_OK;
+  const int64_t vc = bwd_chunk(g, workspace_bytes - vp_target_bytes(N), 0);
+  if (vc == 0) return RB200_E_ARG;
+  int64_t* local_target = static_cast<int64_t*>(workspace);
+  if ((e = rb::vp::shift_target(target, N, vocab_start, local_target, st))) return e;
+  return bwd_chunks(g, hidden, weight_shard, local_target, inv_temperature, lse, entropy, grad_logprob, grad_entropy,
+                    vc, reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(workspace) + vp_target_bytes(N)),
+                    d_hidden_partial, nullptr, static_cast<__nv_bfloat16*>(d_weight_shard), st);
 }

@@ -170,6 +170,45 @@ __global__ void __launch_bounds__(kThreads) fwd_warp_kernel(LArgs a) {
   }
 }
 
+// ---- vocabulary-parallel forward: the same row pass over the shard's part of the window, ending in the rank's
+// record {m, s, t, z_t} (vocab_parallel.cu) instead of the row finish; a.target holds global ids ----
+template <typename T>
+__global__ void __launch_bounds__(kThreads) vp_block_kernel(LArgs a, int64_t vocab_start, float4* rec) {
+  __shared__ Acc part[kThreads / 32];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  for (int64_t r = blockIdx.x; r < a.N; r += gridDim.x) {
+    const T* x = row_ptr<T>(a, r);
+    Acc acc = warp_merge(row_reduce<T, kThreads>(x, a.v_lo, a.v_hi, a.inv_t, t));
+    if (lane == 0) part[warp] = acc;
+    __syncthreads();
+    if (warp == 0) {
+      Acc b;
+      if (lane < kThreads / 32) b = part[lane];
+      else acc_init(b);
+      b = warp_merge(b);
+      if (lane == 0) {
+        const int64_t tg = a.target[r] - vocab_start;
+        rec[r] = make_float4(b.m, b.s, b.t, (tg >= a.v_lo && tg < a.v_hi) ? load1(x + tg) * a.inv_t : 0.f);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) vp_warp_kernel(LArgs a, int64_t vocab_start, float4* rec) {
+  const int lane = threadIdx.x & 31;
+  const int64_t w0 = (int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5);
+  for (int64_t r = w0; r < a.N; r += (int64_t)gridDim.x * (kThreads / 32)) {
+    const T* x = row_ptr<T>(a, r);
+    const Acc acc = warp_merge(row_reduce<T, 32>(x, a.v_lo, a.v_hi, a.inv_t, lane));
+    if (lane == 0) {
+      const int64_t tg = a.target[r] - vocab_start;
+      rec[r] = make_float4(acc.m, acc.s, acc.t, (tg >= a.v_lo && tg < a.v_hi) ? load1(x + tg) * a.inv_t : 0.f);
+    }
+  }
+}
+
 // ---- backward: elementwise over the row given lse (and H), NT threads per row ----
 template <typename T, int NT>
 __device__ __forceinline__ void row_backward(const LArgs& a, int64_t r, int t) {
@@ -291,6 +330,36 @@ extern "C" int rb200_logits_logprob_entropy_bwd(const void* logits, int dtype, c
   } else {
     if (dtype == 0) bwd_warp_kernel<float><<<grid_for(kThreads / 32, N), kThreads, 0, st>>>(a);
     else bwd_warp_kernel<__nv_bfloat16><<<grid_for(kThreads / 32, N), kThreads, 0, st>>>(a);
+  }
+  rb::count_launch();
+  RB_RETURN_LAUNCH();
+}
+
+extern "C" int rb200_logits_vp_partials_fwd(const void* logits, int dtype, const int64_t* target, int64_t N, int64_t L,
+                                            int64_t batch_stride, int64_t row_stride, int Vs, int64_t vocab_start,
+                                            int v_lo, int v_hi, double inv_temperature, float* record,
+                                            rb200_stream_t stream) {
+  if (!record) return RB200_E_NULL;
+  if ((reinterpret_cast<uintptr_t>(record) & 15) != 0) return RB200_E_ALIGN;
+  if (Vs <= 0 || vocab_start < 0 || vocab_start % Vs != 0 || v_lo < 0 || v_lo >= v_hi) return RB200_E_SHAPE;
+  // the shard's part of the global window, in shard columns (empty: the rank's record is {-inf, 0, 0, 0})
+  const int64_t l = v_lo - vocab_start, h = v_hi - vocab_start;
+  const int lo = (int)(l < 0 ? 0 : (l > Vs ? Vs : l)), hi = (int)(h < 0 ? 0 : (h > Vs ? Vs : h));
+  LArgs a{};
+  a.logits = logits; a.target = target; a.N = N; a.L = L; a.batch_stride = batch_stride; a.row_stride = row_stride;
+  a.V = Vs; a.v_lo = 0; a.v_hi = Vs; a.inv_t = (float)inv_temperature;
+  int e = check(a, dtype);
+  if (e) return e;
+  a.v_lo = lo;
+  a.v_hi = hi;
+  cudaStream_t st = rb::as_stream(stream);
+  float4* rec = reinterpret_cast<float4*>(record);
+  if (hi - lo > 2048) {
+    if (dtype == 0) vp_block_kernel<float><<<grid_for(1, N), kThreads, 0, st>>>(a, vocab_start, rec);
+    else vp_block_kernel<__nv_bfloat16><<<grid_for(1, N), kThreads, 0, st>>>(a, vocab_start, rec);
+  } else {
+    if (dtype == 0) vp_warp_kernel<float><<<grid_for(kThreads / 32, N), kThreads, 0, st>>>(a, vocab_start, rec);
+    else vp_warp_kernel<__nv_bfloat16><<<grid_for(kThreads / 32, N), kThreads, 0, st>>>(a, vocab_start, rec);
   }
   rb::count_launch();
   RB_RETURN_LAUNCH();

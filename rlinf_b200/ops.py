@@ -581,3 +581,308 @@ def linear_logprobs_entropy(hidden, weight, target, temperature: float = 1.0, wi
     Returns (logprobs [...], entropy [...] or None), fp32."""
     lp, ent = _LinearLogprobEntropy.apply(hidden, weight, target, temperature, window, bool(compute_entropy))
     return lp, (ent if compute_entropy else None)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Vocabulary-parallel (tensor-parallel) variants: each rank holds one equal shard of the vocabulary (Megatron's
+# VocabUtility, parallel_output=True), reduces it to one 16-byte record per row, and ONE all-gather of the records
+# gives every rank the rows' log-probs / entropies (csrc/vocab_parallel.cu)
+# ---------------------------------------------------------------------------------------------------------------
+def _vp_group(group, what: str):
+    """(group, P, rank) of the tensor-parallel group the vocabulary is split over.  group=None resolves to Megatron's
+    tensor-parallel group when megatron.core's model parallelism is initialised (as the reference's functions use), to
+    one rank when torch.distributed is not initialised or its world has one rank, and is an error otherwise: the world
+    group of a data- or pipeline-parallel job is not the group the vocabulary is split over."""
+    import torch.distributed as dist
+
+    if not (dist.is_available() and dist.is_initialized()):
+        return None, 1, 0
+    if group is None:
+        try:
+            from megatron.core import parallel_state
+        except ImportError:
+            parallel_state = None
+        if parallel_state is not None and parallel_state.model_parallel_is_initialized():
+            group = parallel_state.get_tensor_model_parallel_group()
+        elif dist.get_world_size() > 1:
+            raise ValueError(f"{what}: torch.distributed has {dist.get_world_size()} ranks and Megatron's model "
+                             "parallelism is not initialised; pass the tensor-parallel group as group=")
+    return group, dist.get_world_size(group), dist.get_rank(group)
+
+
+def _vp_window(window, Vs: int, world_size: int, what: str, vocab_size=None):
+    V = Vs * world_size
+    if vocab_size is not None and int(vocab_size) != V:
+        raise ValueError(f"{what}: shards must be equal, but vocab_size {vocab_size} != P * Vs = {world_size} * {Vs}")
+    lo, hi = (0, V) if window is None else (int(window[0]), int(window[1]))
+    if not 0 <= lo < hi <= V:
+        raise ValueError(f"{what}: window [{lo}, {hi}) must lie inside [0, {V}) (P = {world_size} shards of {Vs}) "
+                         "and be non-empty")
+    return lo, hi
+
+
+def _vp_rank(rank: int, world_size: int, what: str):
+    if not 0 <= rank < world_size:
+        raise ValueError(f"{what}: rank {rank} outside [0, {world_size})")
+
+
+def _vp_target(target, device, N: int):
+    tgt = L.to_device(target, device, torch.int64).reshape(-1).contiguous()
+    if tgt.numel() != N:
+        raise ValueError(f"target has {tgt.numel()} entries for {N} rows")
+    return tgt
+
+
+def lmhead_vp_workspace_bytes(N: int, L_rows: int, H: int, Vs: int, vocab_start: int, lo: int, hi: int,
+                              vocab_chunk: int = 0) -> int:
+    """Workspace of the shard's fused forward and of a backward in chunks of vocab_chunk columns (0 = the shard's
+    whole part of the window; < 0 = the forward only)."""
+    n = L.load().rb200_lmhead_vp_workspace_bytes(N, L_rows, H, Vs, vocab_start, lo, hi, vocab_chunk)
+    if n < 0:
+        raise ValueError(f"vocab_parallel_linear_logprobs_entropy: unsupported shape N={N} L={L_rows} H={H} Vs={Vs} "
+                         f"vocab_start={vocab_start} window=[{lo}, {hi})")
+    return int(n)
+
+
+def _lmhead_vp_fwd(x, N, Lr, bs, rs, w, tgt, rank, lo, hi, temperature):
+    Vs, H = w.shape
+    vs = rank * Vs
+    wsb = lmhead_vp_workspace_bytes(N, Lr, H, Vs, vs, lo, hi, -1)  # the forward's workspace only
+    ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+    rec = torch.empty(N, 4, dtype=torch.float32, device=x.device)
+    L.check(L.load().rb200_lmhead_vp_partials_fwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, Vs, vs, lo, hi,
+                                                  1.0 / float(temperature), L.ptr(rec), L.ptr(ws), wsb,
+                                                  L.stream_ptr(x.device)), "lmhead_vp_partials_fwd")
+    return rec
+
+
+def _lmhead_vp_bwd(x, N, Lr, bs, rs, w, tgt, rank, lo, hi, temperature, lse, ent, glp, gh, need_x, need_w):
+    Vs, H = w.shape
+    vs = rank * Vs
+    slo, shi = min(max(lo - vs, 0), Vs), min(max(hi - vs, 0), Vs)
+    vc = _lmhead_chunk(N, slo, shi) if slo < shi else 0
+    wsb = lmhead_vp_workspace_bytes(N, Lr, H, Vs, vs, lo, hi, vc)
+    ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+    dx = torch.empty((N, H), dtype=torch.float32, device=x.device) if need_x else None
+    dw = torch.empty((Vs, H), dtype=torch.bfloat16, device=x.device) if need_w else None
+    L.check(L.load().rb200_lmhead_vp_logprob_entropy_bwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, Vs, vs,
+                                                         lo, hi, 1.0 / float(temperature), L.ptr(lse),
+                                                         L.ptr(ent) if gh is not None else None, L.ptr(glp), L.ptr(gh),
+                                                         L.ptr(dx), L.ptr(dw), L.ptr(ws), wsb, L.stream_ptr(x.device)),
+            "lmhead_vp_logprob_entropy_bwd")
+    return dx, dw
+
+
+def lmhead_vp_partials(hidden, weight_shard, target, rank: int, world_size: int, temperature: float = 1.0,
+                       window=None, vocab_size=None) -> torch.Tensor:
+    """Rank `rank`'s records [N, 4] fp32 {m, s, t, z_t} of hidden @ weight_shard.T, weight_shard = rows
+    [rank * Vs, (rank + 1) * Vs) of lm_head.weight; global targets and window.  No communication: with vp_combine
+    this emulates `world_size` ranks on one device.  vocab_size, when given, must be world_size * Vs."""
+    what = "vocab_parallel_linear_logprobs_entropy"
+    _vp_rank(rank, world_size, what)
+    lo, hi = _vp_window(window, weight_shard.shape[0], world_size, what, vocab_size)
+    _lmhead_check(hidden, weight_shard)
+    x, N, Lr, bs, rs = _lmhead_geometry(hidden)
+    w = weight_shard.contiguous()
+    return _lmhead_vp_fwd(x, N, Lr, bs, rs, w, _vp_target(target, x.device, N), rank, lo, hi, temperature)
+
+
+def lmhead_vp_backward(hidden, weight_shard, target, rank: int, world_size: int, lse, entropy, grad_logprob,
+                       grad_entropy, temperature: float = 1.0, window=None, need_hidden=True, need_weight=True):
+    """Rank `rank`'s share of the backward given the combined lse / entropy: (dX partial [N, H] fp32 to be summed over
+    ranks, or None; d_weight_shard [Vs, H] bf16, or None)."""
+    what = "vocab_parallel_linear_logprobs_entropy"
+    _vp_rank(rank, world_size, what)
+    lo, hi = _vp_window(window, weight_shard.shape[0], world_size, what)
+    _lmhead_check(hidden, weight_shard)
+    x, N, Lr, bs, rs = _lmhead_geometry(hidden)
+    w = weight_shard.contiguous()
+    glp = grad_logprob.reshape(-1).float().contiguous() if grad_logprob is not None else None
+    gh = grad_entropy.reshape(-1).float().contiguous() if grad_entropy is not None else None
+    return _lmhead_vp_bwd(x, N, Lr, bs, rs, w, _vp_target(target, x.device, N), rank, lo, hi, temperature,
+                          lse.contiguous(), entropy.contiguous() if entropy is not None else None, glp, gh,
+                          need_hidden, need_weight)
+
+
+def logits_vp_partials(logits_shard, target, rank: int, world_size: int, temperature: float = 1.0,
+                       window=None, vocab_size=None) -> torch.Tensor:
+    """Rank `rank`'s records [N, 4] fp32 {m, s, t, z_t} of a [..., Vs] logits shard (fp32 or bf16, the `[:, -L-1:-1, :]`
+    slice read in place), global targets and window."""
+    what = "vocab_parallel_entropy_and_log_probs"
+    if logits_shard.dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"{what}: logits must be float32 or bfloat16, got {logits_shard.dtype}")
+    _vp_rank(rank, world_size, what)
+    lo, hi = _vp_window(window, logits_shard.shape[-1], world_size, what, vocab_size)
+    x, N, Lr, bs, rs, Vs = _logits_geometry(logits_shard)
+    tgt = _vp_target(target, x.device, N)
+    rec = torch.empty(N, 4, dtype=torch.float32, device=x.device)
+    L.check(L.load().rb200_logits_vp_partials_fwd(_raw_ptr(x), 0 if x.dtype == torch.float32 else 1, L.ptr(tgt), N, Lr,
+                                                  bs, rs, Vs, rank * Vs, lo, hi, 1.0 / float(temperature), L.ptr(rec),
+                                                  L.stream_ptr(x.device)), "logits_vp_partials_fwd")
+    return rec
+
+
+def vp_combine(records, target, vocab_shard: int, window=None, compute_entropy: bool = True):
+    """records [P, N, 4] gathered in rank order -> (logprob [N], entropy [N] or None, lse [N]), fp32."""
+    P, N = records.shape[0], records.shape[1]
+    if records.dtype != torch.float32 or records.shape[2] != 4:
+        raise ValueError(f"vp_combine: records must be [P, N, 4] float32, got {tuple(records.shape)} {records.dtype}")
+    rec = records.contiguous()
+    lo, hi = _vp_window(window, vocab_shard, P, "vp_combine")
+    tgt = _vp_target(target, rec.device, N)
+    lp = torch.empty(N, dtype=torch.float32, device=rec.device)
+    ent = torch.empty(N, dtype=torch.float32, device=rec.device) if compute_entropy else None
+    lse = torch.empty(N, dtype=torch.float32, device=rec.device)
+    L.check(L.load().rb200_vp_combine(L.ptr(rec), P, N, L.ptr(tgt), vocab_shard, lo, hi, L.ptr(lp), L.ptr(ent),
+                                      L.ptr(lse), L.stream_ptr(rec.device)), "vp_combine")
+    return lp, ent, lse
+
+
+def _vp_gather(rec: torch.Tensor, group, P: int) -> torch.Tensor:
+    """[N, 4] -> [P, N, 4]: the one collective of the forward."""
+    if P == 1:
+        return rec[None]
+    import torch.distributed as dist
+
+    out = torch.empty((P, *rec.shape), dtype=rec.dtype, device=rec.device)
+    dist.all_gather_into_tensor(out, rec, group=group)
+    return out
+
+
+class _VPLinearLogprobEntropy(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, hidden, weight_shard, target, group, temperature, window, want_entropy, reduce_hidden_grad,
+                vocab_size):
+        what = "vocab_parallel_linear_logprobs_entropy"
+        group, P, k = _vp_group(group, what)
+        Vs = weight_shard.shape[0]
+        lo, hi = _vp_window(window, Vs, P, what, vocab_size)
+        _lmhead_check(hidden, weight_shard)
+        x, N, Lr, bs, rs = _lmhead_geometry(hidden)
+        w = weight_shard.contiguous()
+        tgt = _vp_target(target, x.device, N)
+        rec = _lmhead_vp_fwd(x, N, Lr, bs, rs, w, tgt, k, lo, hi, temperature)
+        lp, ent, lse = vp_combine(_vp_gather(rec, group, P), tgt, Vs, (lo, hi), want_entropy)
+        ctx.save_for_backward(x, w, tgt, lse, ent if want_entropy else lse)
+        ctx.meta = (group, P, k, N, Lr, bs, rs, lo, hi, float(temperature), want_entropy, reduce_hidden_grad,
+                    tuple(hidden.shape))
+        shape = hidden.shape[:-1]
+        if want_entropy:
+            return lp.view(shape), ent.view(shape)
+        none = lp.new_zeros(())
+        ctx.mark_non_differentiable(none)
+        return lp.view(shape), none
+
+    @staticmethod
+    def backward(ctx, g_lp, g_ent):
+        x, w, tgt, lse, ent = ctx.saved_tensors
+        group, P, k, N, Lr, bs, rs, lo, hi, temp, want_entropy, reduce_hidden_grad, shape = ctx.meta
+        need_x, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (need_x or need_w):
+            return (None,) * 9
+        glp = g_lp.reshape(-1).float().contiguous() if g_lp is not None else None
+        gh = g_ent.reshape(-1).float().contiguous() if (want_entropy and g_ent is not None) else None
+        dx32, dw = _lmhead_vp_bwd(x, N, Lr, bs, rs, w, tgt, k, lo, hi, temp, lse, ent, glp, gh, need_x, need_w)
+        dx = None
+        if need_x:
+            if P > 1 and reduce_hidden_grad:
+                import torch.distributed as dist
+
+                dist.all_reduce(dx32, group=group)  # fp32: the rank sum rounds to bf16 once, below
+            dx = dx32.to(torch.bfloat16).view(shape)
+        return dx, dw, None, None, None, None, None, None, None
+
+
+def vocab_parallel_linear_logprobs_entropy(hidden, weight_shard, target, group=None, temperature: float = 1.0,
+                                           window=None, compute_entropy: bool = True, reduce_hidden_grad: bool = True,
+                                           vocab_size=None):
+    """linear_logprobs_entropy with the vocabulary split over the ranks of `group` (tensor parallelism): rank k holds
+    weight_shard = lm_head.weight[k * Vs:(k + 1) * Vs] (equal shards, as Megatron pads the vocabulary), `hidden` is the
+    full [N, H] / [bsz, L, H] input on every rank, `target` and `window` are global.  `group` is the tensor-parallel group; None resolves to Megatron's
+    tensor-parallel group when megatron.core's model parallelism is initialised, to one rank without torch.distributed
+    (or with a one-rank world), and raises ValueError in any other multi-rank job.
+    The forward does one all-gather of N x 16 bytes and returns the same log-probs / entropies on every rank; the
+    backward returns d_weight_shard and all-reduces dX in fp32 (reduce_hidden_grad=False leaves the rank's fp32 share
+    un-summed, cast to bf16, for callers that reduce-scatter it themselves).  Shard widths are not compared across
+    ranks (that would cost a collective per call): vocab_size, when given, is checked against P * Vs and is the only
+    guard against unequal shards.  Without an initialised torch.distributed, P = 1 and the results are bit-identical
+    to linear_logprobs_entropy.  Returns (logprobs [...], entropy [...] or None), fp32."""
+    lp, ent = _VPLinearLogprobEntropy.apply(hidden, weight_shard, target, group, temperature, window,
+                                            bool(compute_entropy), bool(reduce_hidden_grad), vocab_size)
+    return lp, (ent if compute_entropy else None)
+
+
+class _VPLogitsLogprobEntropy(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, target, group, want_entropy, entropy_grad):
+        what = "vocab_parallel_entropy_and_log_probs"
+        if logits.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"{what}: logits must be float32 or bfloat16, got {logits.dtype}")
+        group, P, k = _vp_group(group, what)
+        x, N, Lr, bs, rs, Vs = _logits_geometry(logits)
+        tgt = _vp_target(target, x.device, N)
+        rec = torch.empty(N, 4, dtype=torch.float32, device=x.device)
+        L.check(L.load().rb200_logits_vp_partials_fwd(_raw_ptr(x), 0 if x.dtype == torch.float32 else 1, L.ptr(tgt),
+                                                      N, Lr, bs, rs, Vs, k * Vs, 0, P * Vs, 1.0, L.ptr(rec),
+                                                      L.stream_ptr(x.device)), "logits_vp_partials_fwd")
+        lp, ent, lse = vp_combine(_vp_gather(rec, group, P), tgt, Vs, None, want_entropy)
+        ctx.save_for_backward(x, tgt - k * Vs, lse, ent if want_entropy else lse)  # shard-local targets
+        ctx.meta = (N, Lr, bs, rs, Vs, entropy_grad, tuple(logits.shape))
+        shape = logits.shape[:-1]
+        ent = ent.view(shape) if want_entropy else lp.new_zeros(())
+        if not entropy_grad:
+            ctx.mark_non_differentiable(ent)
+        return lp.view(shape), ent
+
+    @staticmethod
+    def backward(ctx, g_lp, g_ent):
+        x, tgt_local, lse, ent = ctx.saved_tensors
+        N, Lr, bs, rs, Vs, entropy_grad, shape = ctx.meta
+        glp = g_lp.reshape(-1).float().contiguous() if g_lp is not None else None
+        gh = g_ent.reshape(-1).float().contiguous() if (entropy_grad and g_ent is not None) else None
+        return _logits_vp_bwd(x, N, Lr, bs, rs, Vs, tgt_local, lse, ent, glp, gh).view(shape), None, None, None, None
+
+
+def _logits_vp_bwd(x, N, Lr, bs, rs, Vs, tgt_local, lse, ent, glp, gh):
+    """dlogits [N, Vs] of the shard: the single-GPU backward with the global lse / entropy and shard-local targets
+    (ids outside [0, Vs) get no target term)."""
+    dx = torch.empty((N, Vs), dtype=x.dtype, device=x.device)
+    L.check(L.load().rb200_logits_logprob_entropy_bwd(_raw_ptr(x), 0 if x.dtype == torch.float32 else 1,
+                                                      L.ptr(tgt_local), N, Lr, bs, rs, Vs, 0, Vs, 1.0, L.ptr(lse),
+                                                      L.ptr(ent) if gh is not None else None, L.ptr(glp), L.ptr(gh),
+                                                      L.ptr(dx), Lr * Vs, Vs, L.stream_ptr(x.device)),
+            "logits_logprob_entropy_bwd")
+    return dx
+
+
+def logits_vp_backward(logits_shard, target, rank: int, lse, entropy, grad_logprob, grad_entropy) -> torch.Tensor:
+    """Rank `rank`'s dlogits [N, Vs] (the shard's dtype) given the combined lse / entropy and global targets."""
+    x, N, Lr, bs, rs, Vs = _logits_geometry(logits_shard)
+    tgt = _vp_target(target, x.device, N) - rank * Vs
+    glp = grad_logprob.reshape(-1).float().contiguous() if grad_logprob is not None else None
+    gh = grad_entropy.reshape(-1).float().contiguous() if grad_entropy is not None else None
+    return _logits_vp_bwd(x, N, Lr, bs, rs, Vs, tgt, lse.contiguous(),
+                          entropy.contiguous() if entropy is not None else None, glp, gh)
+
+
+def vocab_parallel_entropy_and_log_probs(vocab_parallel_logits, target, label_smoothing: float = 0.0,
+                                         calculate_entropy_loss: bool = True, group=None):
+    """Drop-in for rlinf.utils.distributed.vocab_parallel_entropy_and_log_probs (:1230-1242): the rank's logits shard
+    [..., Vs] (fp32 or bf16, Megatron's parallel_output=True; its padded vocabulary makes the shards equal), global
+    targets, over the ranks of `group`.  `group` is the tensor-parallel group; None resolves to Megatron's
+    tensor-parallel group when megatron.core's model parallelism is initialised, to one rank without torch.distributed
+    (or with a one-rank world), and raises ValueError in any other multi-rank job.  One all-gather of N x 16 bytes
+    per call; nothing [N, Vs] is saved for the backward beyond the logits themselves.  Returns (entropy, log_probs),
+    fp32.  The entropy gradient is the mathematical one, which the reference's is not (DESIGN.md §2); with
+    calculate_entropy_loss=False the entropy is returned without a gradient, as in the reference."""
+    if label_smoothing != 0.0:
+        raise ValueError("vocab_parallel_entropy_and_log_probs: label_smoothing != 0 is not supported")
+    lp, ent = _VPLogitsLogprobEntropy.apply(vocab_parallel_logits, target, group, True, bool(calculate_entropy_loss))
+    return ent, lp
+
+
+def vocab_parallel_log_probs_from_logits(logits, labels, group=None):
+    """Drop-in for rlinf.utils.distributed.vocab_parallel_log_probs_from_logits (:1245-1250, = -Megatron's
+    vocab_parallel_cross_entropy) from the rank's logits shard; fp32 log-probs.  `group` as in
+    vocab_parallel_entropy_and_log_probs."""
+    return _VPLogitsLogprobEntropy.apply(logits, labels, group, False, False)[0]
