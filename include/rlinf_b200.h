@@ -236,6 +236,76 @@ int rb200_opd_loss(const float* logprobs, const float* advantages, const uint8_t
                    double loss_scale, double* workspace, float* loss /*[1] or NULL*/,
                    float* metrics /*[RB200_NUM_METRICS]*/, float* d_logprobs /*or NULL*/, rb200_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Token-level PPO-clip actor loss of the reasoning workers (csrc/token_loss.cu): the loss block of
+ *   FSDPActor.training_step (workers/actor/fsdp_actor_worker.py:700-780) and of the Megatron loss_func
+ *   (megatron_actor_worker.py:194-293) for token log-probs [bsz, L]:
+ *     advantages *= min(exp(recomputed - rollout), importance_sampling_clip)   (importance_sampling_fix)
+ *     policy = compute_ppo_actor_loss (losses.py:170-312) aggregated with `agg`, fast_path_zero_loss_mask honoured
+ *     entropy_loss = agg(entropy, mask);  kl_loss = agg(kl_penalty(x, y, kl_mode), mask)
+ *     loss = policy - entropy_bonus * entropy_loss + kl_beta * kl_loss
+ *   and the gradients of `loss` for a unit upstream gradient.  No host sync, no floating-point atomics: two identical
+ *   calls give the same bits on any SM count.
+ * Row i, token j of each input is at ptr[i * <name>_stride + j] (strides in elements, >= L), so slices such as
+ *   log_probs[:, -L-1:-1] are read in place.  loss_mask is uint8 / bool; every other input is fp32.
+ * Optional inputs (NULL = absent): entropy (the entropy term; its loss is reported even when entropy_bonus is 0),
+ *   ref_logprobs (the KL term, added when kl_beta > 0), rollout_logprobs + recomputed_logprobs (the IS fix when
+ *   importance_sampling_fix != 0, and RB200_TM_ROLLOUT_TRAIN_KL = masked_mean(|recomputed - rollout|)).
+ * kl_order 0: kl_penalty(logprobs, ref_logprobs) (Megatron), 1: kl_penalty(ref_logprobs, logprobs) (FSDP).
+ * fast_path_zero_loss_mask: if the FIRST row's mask is empty, the policy part and its metrics are 0 (decided on the
+ *   device).  agg RB200_AGG_SEQ_MEAN_TOKEN_MEAN divides by each row's own count, so an empty row makes the loss NaN,
+ *   as in the reference.
+ * Outputs: loss [1], metrics [RB200_TM_NUM] (RB200_TM_*), d_logprobs / d_entropy [bsz, L] contiguous or NULL
+ *   (d_entropy is zero unless entropy_bonus > 0).  workspace: rb200_token_loss_workspace_bytes(bsz, L) bytes,
+ *   16-byte aligned, no initialisation needed (-1 = unsupported shape: bsz > 65535 or a non-positive dimension).
+ * ---------------------------------------------------------------------------------------- */
+enum { RB200_AGG_TOKEN_MEAN = 0, RB200_AGG_SEQ_MEAN_TOKEN_SUM = 1, RB200_AGG_SEQ_MEAN_TOKEN_MEAN = 2 };
+enum {
+  RB200_TM_POLICY_LOSS = 0,         /* actor/policy_loss        */
+  RB200_TM_POLICY_LOSS_ABS = 1,     /* actor/policy_loss_abs    */
+  RB200_TM_RATIO = 2,               /* actor/ratio              */
+  RB200_TM_RATIO_ABS = 3,           /* actor/ratio_abs          */
+  RB200_TM_CLIPPED_RATIO = 4,       /* actor/clipped_ratio      */
+  RB200_TM_DUAL_CLIPPED_RATIO = 5,  /* actor/dual_cliped_ratio  */
+  RB200_TM_APPROX_KL = 6,           /* actor/approx_kl          */
+  RB200_TM_CLIP_FRACTION = 7,       /* actor/clip_fraction      */
+  RB200_TM_ENTROPY_LOSS = 8,        /* actor/entropy_loss       */
+  RB200_TM_KL_LOSS = 9,             /* actor/kl_loss            */
+  RB200_TM_FINAL_LOSS = 10,         /* actor/final_loss (= loss[0]) */
+  RB200_TM_ROLLOUT_TRAIN_KL = 11,   /* actor/rollout_train_kl   */
+  RB200_TM_NUM = 16
+};
+typedef struct rb200_token_loss_args {
+  int64_t bsz, L;
+  const float* logprobs;            int64_t logprobs_stride;
+  const float* old_logprobs;        int64_t old_logprobs_stride;
+  const float* advantages;          int64_t advantages_stride;
+  const uint8_t* loss_mask;         int64_t loss_mask_stride;
+  const float* entropy;             int64_t entropy_stride;
+  const float* ref_logprobs;        int64_t ref_logprobs_stride;
+  const float* rollout_logprobs;    int64_t rollout_logprobs_stride;
+  const float* recomputed_logprobs; int64_t recomputed_logprobs_stride;
+  double clip_ratio_low, clip_ratio_high;
+  double clip_ratio_c;              /* <= 0: no dual clip; else must be > 1 */
+  double clip_log_ratio_min, clip_log_ratio_max;
+  double entropy_bonus, kl_beta, importance_sampling_clip;
+  int32_t has_clip_log_ratio_min, has_clip_log_ratio_max;
+  int32_t agg;                      /* RB200_AGG_* */
+  int32_t kl_mode;                  /* 0 k1/kl, 1 abs, 2 k2/mse, 3 k3/low_var_kl */
+  int32_t kl_order;
+  int32_t importance_sampling_fix;
+  int32_t fast_path_zero_loss_mask;
+  int32_t reserved;
+  void* workspace;
+  int64_t workspace_bytes;
+  float* loss;
+  float* metrics;
+  float* d_logprobs;
+  float* d_entropy;
+} rb200_token_loss_args;
+int64_t rb200_token_loss_workspace_bytes(int64_t bsz, int64_t L);
+int rb200_token_ppo_loss(const rb200_token_loss_args* args, rb200_stream_t stream);
+
 /* x[i] *= s (device scalar-free helper for autograd's upstream scalar). */
 int rb200_scale(float* x, int64_t n, float s, rb200_stream_t stream);
 /* x[i] *= *s_dev  (the scalar lives on the device: no host sync in autograd's backward). */

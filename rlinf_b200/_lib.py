@@ -90,6 +90,29 @@ DM_KEYS = {
 DM_ENTROPY = 20  # RB200_DM_ENTROPY: actor/entropy_loss of the decoupled loss
 
 
+# reasoning token loss (mirror of RB200_AGG_* / RB200_TM_* / rb200_token_loss_args)
+AGG_MODES = {"token-mean": 0, "seq-mean-token-sum": 1, "seq-mean-token-mean": 2}
+TM_NUM = 16
+TM_KEYS = {
+    0: "actor/policy_loss", 1: "actor/policy_loss_abs", 2: "actor/ratio", 3: "actor/ratio_abs",
+    4: "actor/clipped_ratio", 5: "actor/dual_cliped_ratio", 6: "actor/approx_kl", 7: "actor/clip_fraction",
+    8: "actor/entropy_loss", 9: "actor/kl_loss", 10: "actor/final_loss", 11: "actor/rollout_train_kl",
+}
+
+
+class TokenLossArgs(C.Structure):
+    _fields_ = [("bsz", c_int64), ("L", c_int64)] + [
+        f for name in ("logprobs", "old_logprobs", "advantages", "loss_mask", "entropy", "ref_logprobs",
+                       "rollout_logprobs", "recomputed_logprobs") for f in ((name, c_void_p), (name + "_stride", c_int64))
+    ] + [(n, c_double) for n in ("clip_ratio_low", "clip_ratio_high", "clip_ratio_c", "clip_log_ratio_min",
+                                  "clip_log_ratio_max", "entropy_bonus", "kl_beta", "importance_sampling_clip")] + [
+        (n, C.c_int32) for n in ("has_clip_log_ratio_min", "has_clip_log_ratio_max", "agg", "kl_mode", "kl_order",
+                                 "importance_sampling_fix", "fast_path_zero_loss_mask", "reserved")] + [
+        ("workspace", c_void_p), ("workspace_bytes", c_int64),
+        ("loss", c_void_p), ("metrics", c_void_p), ("d_logprobs", c_void_p), ("d_entropy", c_void_p),
+    ]
+
+
 class MlpLayout(C.Structure):
     _fields_ = [
         ("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("value_dim", C.c_int32), ("hidden", C.c_int32),
@@ -117,6 +140,8 @@ SIGNATURES = {
     "rb200_decoupled_ppo_loss": (c_int, [C.POINTER(DppoArgs), c_void_p]),
     "rb200_decoupled_ppo_loss_scalar_version": (c_int, [C.POINTER(DppoScalarVersionArgs), c_void_p]),
     "rb200_opd_loss": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_double] + [c_void_p] * 5),
+    "rb200_token_loss_workspace_bytes": (c_int64, [c_int64, c_int64]),
+    "rb200_token_ppo_loss": (c_int, [C.POINTER(TokenLossArgs), c_void_p]),
     "rb200_scale": (c_int, [c_void_p, c_int64, c_float, c_void_p]),
     "rb200_scale_by": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "rb200_grad_sqnorm": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),

@@ -323,6 +323,78 @@ def compute_decoupled_ppo_actor_critic_loss(**kwargs) -> tuple[torch.Tensor, dic
     return loss, metrics
 
 
+# loss_agg_func of the reasoning workers (get_loss_agg_func, rlinf/utils/utils.py:359-381), matched by function name
+_AGG_BY_NAME = {"masked_mean": "token-mean", "seq_mean_token_sum": "seq-mean-token-sum",
+                "seq_mean_token_mean": "seq-mean-token-mean"}
+
+
+def loss_agg_mode(loss_agg_func) -> str:
+    """The aggregation a reasoning worker's loss_agg_func selects: None or masked_mean -> "token-mean", the reference's
+    seq_mean_token_sum / seq_mean_token_mean by name; a string is one of get_loss_agg_func's names.  Any other callable
+    raises ValueError naming what is supported."""
+    if loss_agg_func is None:
+        return "token-mean"
+    if isinstance(loss_agg_func, str):
+        if loss_agg_func not in L.AGG_MODES:
+            raise ValueError(f"Unsupported loss aggregation method: {loss_agg_func}")
+        return loss_agg_func
+    mode = _AGG_BY_NAME.get(getattr(loss_agg_func, "__name__", None))
+    if mode is None:
+        raise ValueError(f"loss_agg_func {loss_agg_func!r} is not supported: pass masked_mean, seq_mean_token_sum or "
+                         f"seq_mean_token_mean (rlinf.utils.utils.get_loss_agg_func)")
+    return mode
+
+
+def token_level_actor_loss(**kwargs) -> tuple[torch.Tensor, dict]:
+    """policy_loss(task_type != "embodied", loss_type="actor") with a seq-mean loss_agg_func: compute_ppo_actor_loss
+    (losses.py:170-312) on [bsz, L] token log-probs through the token-level kernel, fast_path_zero_loss_mask honoured.
+    Metrics: the eight actor/* keys as 0-dim device tensors."""
+    if kwargs.get("critic_warmup"):
+        raise ValueError("critic_warmup is not supported with a seq-mean loss_agg_func")
+    loss, metrics = ops.token_policy_loss(
+        kwargs["logprobs"], kwargs["old_logprobs"], kwargs["advantages"], kwargs.get("loss_mask"),
+        loss_agg=loss_agg_mode(kwargs.get("loss_agg_func")), clip_ratio_low=kwargs["clip_ratio_low"],
+        clip_ratio_high=kwargs["clip_ratio_high"], clip_ratio_c=kwargs.get("clip_ratio_c"),
+        clip_log_ratio_min=kwargs.get("clip_log_ratio_min"), clip_log_ratio_max=kwargs.get("clip_log_ratio_max"),
+        fast_path_zero_loss_mask=bool(kwargs.get("fast_path_zero_loss_mask", False)))
+    return loss, {k: metrics[k] for k in (L.TM_KEYS[s] for s in L.ACTOR_SLOTS)}
+
+
+def reasoning_actor_loss(logprobs, advantages, loss_mask, *, old_logprobs=None, recomputed_logprobs=None,
+                         rollout_logprobs=None, ref_logprobs=None, entropy=None, loss_agg_func=None,
+                         clip_ratio_low: float = 0.2, clip_ratio_high: float = 0.2, clip_ratio_c: Optional[float] = 3.0,
+                         clip_log_ratio_min: Optional[float] = None, clip_log_ratio_max: Optional[float] = None,
+                         entropy_bonus: float = 0.0, kl_beta: float = 0.0, kl_penalty_type: str = "kl",
+                         kl_order: str = "fsdp", importance_sampling_fix: bool = False,
+                         importance_sampling_clip: Optional[float] = None,
+                         fast_path_zero_loss_mask: bool = True) -> tuple[torch.Tensor, dict]:
+    """The whole loss block of the reasoning actor in one device pass: FSDPActor.training_step
+    (workers/actor/fsdp_actor_worker.py:700-780, kl_order="fsdp") or the Megatron loss_func
+    (megatron_actor_worker.py:194-293, kl_order="megatron"), with the worker's own variables.
+
+    old_logprobs defaults to recomputed_logprobs, else rollout_logprobs (the workers' choice).  loss_agg_func is the
+    worker's self.loss_agg_func (or a get_loss_agg_func name).  entropy: pass it when the worker has calculate_entropy
+    (actor/entropy_loss is then reported); entropy_bonus > 0 adds the term to the loss (calculate_entropy_loss).
+    ref_logprobs with kl_beta > 0 adds kl_beta * kl_loss.  rollout and recomputed log-probs also give
+    actor/rollout_train_kl (compute_rollout_train_kl, fsdp_actor_worker.py:75-93).
+
+    Returns (loss, metrics): loss before 1/gradient_accumulation (and before Megatron's early-stop and valid-token
+    scales, which stay with the caller), differentiable w.r.t. logprobs and entropy; metrics are 0-dim device tensors
+    under the workers' keys, actor/final_loss, actor/entropy_loss and actor/kl_loss included.  No host sync."""
+    if old_logprobs is None:
+        old_logprobs = recomputed_logprobs if recomputed_logprobs is not None else rollout_logprobs
+    if old_logprobs is None:
+        raise ValueError("reasoning_actor_loss needs old_logprobs, recomputed_logprobs or rollout_logprobs")
+    return ops.token_policy_loss(
+        logprobs, old_logprobs, advantages, loss_mask, entropy=entropy, ref_logprobs=ref_logprobs,
+        rollout_logprobs=rollout_logprobs, recomputed_logprobs=recomputed_logprobs,
+        loss_agg=loss_agg_mode(loss_agg_func), clip_ratio_low=clip_ratio_low, clip_ratio_high=clip_ratio_high,
+        clip_ratio_c=clip_ratio_c, clip_log_ratio_min=clip_log_ratio_min, clip_log_ratio_max=clip_log_ratio_max,
+        entropy_bonus=entropy_bonus, kl_beta=kl_beta, kl_penalty=kl_penalty_type, kl_order=kl_order,
+        importance_sampling_fix=importance_sampling_fix, importance_sampling_clip=importance_sampling_clip,
+        fast_path_zero_loss_mask=fast_path_zero_loss_mask)
+
+
 class _FusedOpdLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logprobs, cfg):

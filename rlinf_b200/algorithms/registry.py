@@ -75,6 +75,16 @@ def policy_loss(**kwargs) -> tuple[torch.Tensor, dict]:
     fused = getattr(loss_fn, "_rb200_fused_embodied", None)
     if task_type == "embodied" and fused is not None:
         return fused(**kwargs)
+    if task_type != "embodied" and fused is not None:
+        # the reasoning workers pass loss_agg_func (fsdp_actor_worker.py:737-751, megatron_actor_worker.py:225-243);
+        # the built-in kernels aggregate as masked_mean, the token-level kernel also as the two seq-mean variants
+        mode = losses.loss_agg_mode(kwargs.get("loss_agg_func"))
+        ratio_agg = all(kwargs.get(k) is not None for k in ("max_episode_steps", "loss_mask_sum", "loss_mask"))
+        if mode != "token-mean" and not ratio_agg:  # masked_mean_ratio overrides loss_agg_func (losses.py:221-227)
+            if loss_type != "actor":
+                raise ValueError(f"loss_agg_func {mode!r} is supported with loss_type='actor' only; "
+                                 f"{loss_type!r} aggregates as token-mean (masked_mean)")
+            return losses.token_level_actor_loss(**kwargs)
     if task_type == "embodied":
         kwargs = losses.preprocess_loss_inputs(**kwargs)
     loss, metrics_data = loss_fn(**kwargs)

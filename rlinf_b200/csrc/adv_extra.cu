@@ -4,6 +4,7 @@
 // normalize_from_stats :957-965.
 // Layout everywhere: step-major [L, B] (B fastest), loss_mask as uint8 0/1 (NULL = all valid).
 #include "common.cuh"
+#include "kl_unit.cuh"
 
 namespace {
 
@@ -136,15 +137,8 @@ __global__ void __launch_bounds__(kCols* kRowsPar) raw_adv_kernel(const float* _
 // The cumulative sum follows torch's CPU cumsum: sequential from the last row, accumulated in fp64 (acc_type of float
 // on CPU), each prefix rounded to fp32.  kl terms: mode as rb200_kl_penalty (k1 / abs / k2 / k3).
 __device__ __forceinline__ float kl_term(float a, float b, int mode) {
-  if (mode == 0) return __fsub_rn(a, b);
-  if (mode == 1) return fabsf(__fsub_rn(a, b));
-  if (mode == 2) {
-    const float d = __fsub_rn(a, b);
-    return __fmul_rn(0.5f, __fmul_rn(d, d));
-  }
-  const float kl = fminf(fmaxf(__fsub_rn(b, a), -20.0f), 20.0f);
-  const float kld = __fsub_rn(__fsub_rn(expf(kl), kl), 1.0f);
-  return fminf(fmaxf(kld, -10.0f), 10.0f);
+  float g;
+  return rb::kl_penalty_unit(a, b, mode, g);
 }
 
 __global__ void __launch_bounds__(128) reinpp_scan_kernel(const float* __restrict__ rewards,

@@ -1,5 +1,6 @@
 // Small path kernels: reward filter (a10), kl_penalty (a18), masked statistics for rollout metrics (a24).
 #include "common.cuh"
+#include "kl_unit.cuh"
 
 namespace {
 
@@ -50,28 +51,8 @@ __global__ void __launch_bounds__(256) kl_penalty_kernel(const float* __restrict
                                                          int mode) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const float a = lp[i], b = ref[i];
-    float v, g;
-    if (mode == 0) {
-      v = __fsub_rn(a, b);
-      g = 1.0f;
-    } else if (mode == 1) {
-      const float d = __fsub_rn(a, b);
-      v = fabsf(d);
-      g = d > 0.f ? 1.0f : (d < 0.f ? -1.0f : 0.0f);
-    } else if (mode == 2) {
-      const float d = __fsub_rn(a, b);
-      v = __fmul_rn(0.5f, __fmul_rn(d, d));
-      g = d;
-    } else {
-      const float raw = __fsub_rn(b, a);
-      const float kl = fminf(fmaxf(raw, -20.0f), 20.0f);
-      const float ratio = expf(kl);
-      const float kld = __fsub_rn(__fsub_rn(ratio, kl), 1.0f);
-      v = fminf(fmaxf(kld, -10.0f), 10.0f);
-      const bool pass = (raw >= -20.0f && raw <= 20.0f) && (kld >= -10.0f && kld <= 10.0f);
-      g = pass ? -(ratio - 1.0f) : 0.0f;  // d kld / d lp = (ratio - 1) * d kl / d lp, d kl / d lp = -1
-    }
+    float g;
+    const float v = rb::kl_penalty_unit(lp[i], ref[i], mode, g);
     out[i] = v;
     if (dlp) dlp[i] = g;
   }

@@ -270,6 +270,172 @@ def kl_penalty_raw(logprob, ref_logprob, kind, want_grad=False):
     return out, g
 
 
+# ---------------------------------------------------------------------------------------------------------------
+# Token-level PPO-clip actor loss of the reasoning workers (csrc/token_loss.cu)
+_KL_ORDERS = {"megatron": 0, "fsdp": 1}
+
+
+def _rows(t, name, shape, dev, dtype=torch.float32):
+    """A [bsz, L] input as (tensor, row stride): read in place when its tokens are contiguous."""
+    if t is None:
+        return None, 0
+    if tuple(t.shape) != shape:
+        raise ValueError(f"token_policy_loss: {name} has shape {tuple(t.shape)}, expected {shape} (that of logprobs)")
+    if t.dtype != dtype:
+        raise ValueError(f"token_policy_loss: {name} must be {dtype}, got {t.dtype}")
+    if t.device != dev:
+        raise ValueError(f"token_policy_loss: {name} is on {t.device}, logprobs on {dev}")
+    if t.stride(1) != 1 or t.stride(0) < shape[1]:
+        t = t.contiguous()
+    return t, t.stride(0)
+
+
+def _token_loss_cfg(logprobs, old_logprobs, advantages, loss_mask, entropy, ref_logprobs, rollout_logprobs,
+                    recomputed_logprobs, loss_agg, clip_ratio_low, clip_ratio_high, clip_ratio_c, clip_log_ratio_min,
+                    clip_log_ratio_max, entropy_bonus, kl_beta, kl_penalty, kl_order, importance_sampling_fix,
+                    importance_sampling_clip, fast_path_zero_loss_mask):
+    """Validate the arguments of token_policy_loss (before anything touches the device) -> the ABI struct's fields."""
+    for name, t in (("logprobs", logprobs), ("old_logprobs", old_logprobs), ("advantages", advantages)):
+        assert t.dtype == torch.float32, f"{name} must be float32 to keep numerical stability"  # losses.py:232-240
+    if logprobs.dim() != 2:
+        raise ValueError(f"token_policy_loss: logprobs must be [bsz, L], got {tuple(logprobs.shape)}")
+    if loss_agg not in L.AGG_MODES:
+        raise ValueError(f"Unsupported loss aggregation method: {loss_agg}; supported: {sorted(L.AGG_MODES)}")
+    if clip_ratio_c is not None:
+        assert clip_ratio_c > 1.0, "clip_ratio_c must be greater than 1.0"  # losses.py:260
+    if kl_penalty == "full":
+        raise NotImplementedError("kl_penalty 'full' needs the whole vocabulary's log-probs (utils.py:60-62)")
+    if kl_penalty not in _KL_MODES:
+        raise ValueError(f"unknown kl_penalty {kl_penalty!r}; supported: {sorted(_KL_MODES)}")
+    if kl_order not in _KL_ORDERS:
+        raise ValueError(f"kl_order must be one of {sorted(_KL_ORDERS)}, got {kl_order!r}")
+    if importance_sampling_fix:
+        if rollout_logprobs is None or recomputed_logprobs is None:
+            raise ValueError("importance_sampling_fix requires both rollout_logprobs and recomputed_logprobs")
+        if importance_sampling_clip is None:
+            raise ValueError("importance_sampling_fix requires importance_sampling_clip")
+    shape, dev = tuple(logprobs.shape), logprobs.device
+    if loss_mask is None or tuple(loss_mask.shape) != shape:
+        raise ValueError(f"token_policy_loss: loss_mask has shape {None if loss_mask is None else tuple(loss_mask.shape)}"
+                         f", expected {shape} (that of logprobs)")
+    if loss_mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"token_policy_loss: loss_mask must be bool or uint8, got {loss_mask.dtype}")
+    if 0 in shape:
+        raise ValueError(f"token_policy_loss: empty logprobs {shape}")
+    named = dict(logprobs=logprobs, old_logprobs=old_logprobs, advantages=advantages,
+                 loss_mask=loss_mask.view(torch.uint8) if loss_mask.dtype == torch.bool else loss_mask,
+                 entropy=entropy, ref_logprobs=ref_logprobs, rollout_logprobs=rollout_logprobs,
+                 recomputed_logprobs=recomputed_logprobs)
+    ins = {k: _rows(t, k, shape, dev, torch.uint8 if k == "loss_mask" else torch.float32) for k, t in named.items()}
+    hp = dict(clip_ratio_low=float(clip_ratio_low), clip_ratio_high=float(clip_ratio_high),
+              clip_ratio_c=float(clip_ratio_c) if clip_ratio_c is not None else 0.0,
+              has_clip_log_ratio_min=int(clip_log_ratio_min is not None),
+              has_clip_log_ratio_max=int(clip_log_ratio_max is not None),
+              clip_log_ratio_min=float(clip_log_ratio_min or 0.0), clip_log_ratio_max=float(clip_log_ratio_max or 0.0),
+              entropy_bonus=float(entropy_bonus or 0.0), kl_beta=float(kl_beta or 0.0),
+              importance_sampling_clip=float(importance_sampling_clip or 0.0), agg=L.AGG_MODES[loss_agg],
+              kl_mode=_KL_MODES[kl_penalty], kl_order=_KL_ORDERS[kl_order],
+              importance_sampling_fix=int(bool(importance_sampling_fix)),
+              fast_path_zero_loss_mask=int(bool(fast_path_zero_loss_mask)))
+    return ins, hp
+
+
+def _token_loss_launch(lp, ent, ins, hp, want_d_lp, want_d_ent):
+    if not lp.is_cuda:
+        raise L.Rb200Error("token_policy_loss takes CUDA tensors; there is no CPU path")
+    lib = L.load()
+    dev = lp.device
+    bsz, Ln = lp.shape
+    a = L.TokenLossArgs()
+    a.bsz, a.L = bsz, Ln
+    keep = []
+    for name, (t, stride) in ins.items():
+        if name == "logprobs":
+            t, stride = lp, lp.stride(0)
+        elif name == "entropy":
+            t, stride = ent, (ent.stride(0) if ent is not None else 0)
+        keep.append(t)
+        setattr(a, name, None if t is None else C.c_void_p(t.data_ptr()))
+        setattr(a, name + "_stride", stride)
+    for k, v in hp.items():
+        setattr(a, k, v)
+    wsb = L.load().rb200_token_loss_workspace_bytes(bsz, Ln)
+    if wsb < 0:
+        raise ValueError(f"token_policy_loss: unsupported shape bsz={bsz} L={Ln} (bsz <= 65535)")
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+    loss = torch.empty(1, dtype=torch.float32, device=dev)
+    metrics = torch.empty(L.TM_NUM, dtype=torch.float32, device=dev)
+    d_lp = torch.empty((bsz, Ln), dtype=torch.float32, device=dev) if want_d_lp else None
+    d_ent = torch.empty((bsz, Ln), dtype=torch.float32, device=dev) if want_d_ent else None
+    a.workspace, a.workspace_bytes = L.ptr(ws), wsb
+    a.loss, a.metrics, a.d_logprobs, a.d_entropy = L.ptr(loss), L.ptr(metrics), L.ptr(d_lp), L.ptr(d_ent)
+    L.check(lib.rb200_token_ppo_loss(C.byref(a), L.stream_ptr(dev)), "token_ppo_loss")
+    return loss.reshape(()), metrics, d_lp, d_ent
+
+
+class _TokenPolicyLoss(torch.autograd.Function):
+    """forward: one launch group writes the loss, the metrics and the gradients that are needed; backward: those
+    gradients times the upstream scalar, read on the device."""
+
+    @staticmethod
+    def forward(ctx, logprobs, entropy, ins, hp):
+        want_d_ent = entropy is not None and ctx.needs_input_grad[1] and hp["entropy_bonus"] > 0.0
+        loss, metrics, d_lp, d_ent = _token_loss_launch(logprobs.detach(), None if entropy is None else entropy.detach(),
+                                                        ins, hp, ctx.needs_input_grad[0], want_d_ent)
+        ctx.grads = (d_lp, d_ent)
+        ctx.mark_non_differentiable(metrics)
+        return loss, metrics
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_metrics):
+        d_lp, d_ent = ctx.grads
+        ctx.grads = None
+        if d_lp is not None:
+            scale_by_(d_lp, g_loss)
+        if d_ent is not None:
+            scale_by_(d_ent, g_loss)
+        return d_lp, d_ent, None, None
+
+
+def token_policy_loss(logprobs, old_logprobs, advantages, loss_mask, *, entropy=None, ref_logprobs=None,
+                      rollout_logprobs=None, recomputed_logprobs=None, loss_agg: str = "token-mean",
+                      clip_ratio_low: float = 0.2, clip_ratio_high: float = 0.2, clip_ratio_c: Optional[float] = None,
+                      clip_log_ratio_min: Optional[float] = None, clip_log_ratio_max: Optional[float] = None,
+                      entropy_bonus: float = 0.0, kl_beta: float = 0.0, kl_penalty: str = "kl", kl_order: str = "fsdp",
+                      importance_sampling_fix: bool = False, importance_sampling_clip: Optional[float] = None,
+                      fast_path_zero_loss_mask: bool = False):
+    """Token-level PPO-clip actor loss of the reasoning workers, with its entropy and KL terms, in one device pass.
+
+    logprobs, old_logprobs, advantages, loss_mask (bool / uint8) and the optional entropy, ref_logprobs,
+    rollout_logprobs, recomputed_logprobs are [bsz, L] CUDA tensors (fp32 but the mask); slices whose tokens are
+    contiguous, e.g. log_probs[:, -L-1:-1], are read in place.  loss_agg: "token-mean", "seq-mean-token-sum" or
+    "seq-mean-token-mean" (get_loss_agg_func's names), applied to the policy loss, policy_loss_abs, the entropy and
+    the KL term.  kl_order "fsdp" computes kl_penalty(ref_logprobs, logprobs), "megatron" kl_penalty(logprobs,
+    ref_logprobs); the KL term is added when kl_beta > 0.  importance_sampling_fix multiplies the advantages by
+    min(exp(recomputed - rollout), importance_sampling_clip).  fast_path_zero_loss_mask: an empty first row zeroes the
+    policy part and its metrics, decided on the device.
+
+    Returns (loss, metrics): loss = policy - entropy_bonus * entropy_loss + kl_beta * kl_loss as a 0-dim tensor,
+    differentiable w.r.t. logprobs and entropy (only the gradients that are needed are computed); metrics maps the
+    workers' keys (actor/policy_loss ... actor/clip_fraction, actor/entropy_loss, actor/kl_loss, actor/final_loss,
+    and actor/rollout_train_kl when both rollout and recomputed log-probs are given) to 0-dim device tensors.  No host sync.
+    """
+    ins, hp = _token_loss_cfg(logprobs, old_logprobs, advantages, loss_mask, entropy, ref_logprobs, rollout_logprobs,
+                              recomputed_logprobs, loss_agg, clip_ratio_low, clip_ratio_high, clip_ratio_c,
+                              clip_log_ratio_min, clip_log_ratio_max, entropy_bonus, kl_beta, kl_penalty, kl_order,
+                              importance_sampling_fix, importance_sampling_clip, fast_path_zero_loss_mask)
+    lp, _ = ins["logprobs"]
+    ent, _ = ins["entropy"]
+    needs = torch.is_grad_enabled() and (logprobs.requires_grad or (entropy is not None and entropy.requires_grad))
+    if needs:
+        loss, metrics = _TokenPolicyLoss.apply(lp, ent, ins, hp)
+    else:
+        loss, metrics, _, _ = _token_loss_launch(lp, ent, ins, hp, False, False)
+    with_rr = rollout_logprobs is not None and recomputed_logprobs is not None
+    keys = {s: k for s, k in L.TM_KEYS.items() if k != "actor/rollout_train_kl" or with_rr}
+    return loss, {k: metrics[s] for s, k in keys.items()}
+
+
 def masked_stats(x, mask=None, mask_div=1):
     """{count, sum, min, max} (float64[4], device) of x over mask (mask index = flat index // mask_div)."""
     lib = L.load()
