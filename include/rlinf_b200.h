@@ -589,6 +589,36 @@ int rb200_logits_vp_partials_fwd(const void* logits, int dtype, const int64_t* t
 int rb200_vp_combine(const float* records, int n_ranks, int64_t N, const int64_t* target, int vocab_shard, int v_lo,
                      int v_hi, float* logprob, float* entropy, float* lse, rb200_stream_t stream);
 
+/* Response-rows plan (csrc/response_rows.cu): the rows of the flattened [T, H] hidden states that the reasoning loss
+ * reads, for one of three batch layouts, as int64 index maps for rb200_gather_rows.  Sequence b: response length
+ * r_b = response_lengths[b] (0 <= r_b <= L), first response row a_b, first row s_b:
+ *   layout 0 (padded, [bsz, S] left-padded prompt, right-padded response): s_b = b S, a_b = b S + S - L; T = bsz S.
+ *   layout 1 (FSDP-packed): len0 = prompt lengths p_b <= S (S = max prompt length), s_b = sum_{i<b} (p_i + r_i),
+ *            a_b = s_b + p_b.
+ *   layout 2 (Megatron THD, cp 1): len0 = cu_seqlens_padded [bsz + 1], len1 = valid tokens n_b, s_b = len0[b],
+ *            a_b = s_b + n_b - r_b.
+ * Sequence b owns n_b = r_b + entropy_shift compact rows (none when r_b = 0), holding hidden rows a_b - 1 + k; compact
+ * row o_b + j predicts response token j, and holds column j's entropy at o_b + j + entropy_shift.  R = sum n_b.
+ * Outputs (sentinel -1: the zero row the caller appends to the gather's source):
+ *   rows [R]: hidden row of each compact row;  targets [R]: the token at row + 1, or -1 (outside every window) where
+ *   the log-prob is not needed;  cell_map [bsz, L]: compact row of the cell's log-prob, or -1;  hidden_map [T]: compact
+ *   row of each hidden row, or -1;  cells [R + 1]: cells[0] = -1, cells[1 + c] = the cell b L + j whose log-prob
+ *   compact row c holds, or -1;  status [2] int64: {R, RB200_RR_* error bits}.
+ * Only the first min(R, capacity) compact rows are written.  The lengths and tokens are device pointers; the checks
+ * run on the device and land in status[1].  bsz <= 8192.  One launch. */
+enum {
+  RB200_RR_RESPONSE = 1,   /* r_b < 0 or r_b > L */
+  RB200_RR_PROMPT = 2,     /* a sequence has no prompt token (a_b - s_b < 1) */
+  RB200_RR_BOUNDS = 4,     /* rows outside [0, T) */
+  RB200_RR_ORDER = 8,      /* sequences overlap or are not ascending (or overrun their padded segment) */
+  RB200_RR_MAX_PROMPT = 16, /* p_b > max prompt length */
+  RB200_RR_CAPACITY = 32   /* R > capacity */
+};
+int rb200_response_rows_plan(int layout, const int64_t* len0, const int64_t* len1, const int64_t* response_lengths,
+                             int64_t bsz, int64_t S, int64_t L, int64_t T, int entropy_shift, const int64_t* tokens,
+                             int64_t capacity, int64_t* rows, int64_t* targets, int64_t* cell_map,
+                             int64_t* hidden_map, int64_t* cells, int64_t* status, rb200_stream_t stream);
+
 /* Value tower only: values [n,value_dim] = ValueHead(states). Used for the bootstrap value of
  * final observations (get_bootstrap_values, workers/rollout/hf/huggingface_worker.py:612-627). */
 int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, const float* wsplit,

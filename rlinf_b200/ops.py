@@ -1052,3 +1052,81 @@ def vocab_parallel_log_probs_from_logits(logits, labels, group=None):
     vocab_parallel_cross_entropy) from the rank's logits shard; fp32 log-probs.  `group` as in
     vocab_parallel_entropy_and_log_probs."""
     return _VPLogitsLogprobEntropy.apply(logits, labels, group, False, False)[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Response rows only: the LM-head log-probs / entropies of the rows a reasoning loss reads, for padded and packed
+# batches, written straight into [bsz, response_len] (response_rows.py, csrc/response_rows.cu)
+# ---------------------------------------------------------------------------------------------------------------
+class _GatherRows(torch.autograd.Function):
+    """hidden [T, H] -> the plan's compact rows [R, H]; the backward scatters dX back through the plan's inverse map
+    (every row written once, zeros outside the responses)."""
+
+    @staticmethod
+    def forward(ctx, x, rows, hidden_map):
+        ctx.save_for_backward(hidden_map)
+        return gather_rows(x, rows)
+
+    @staticmethod
+    def backward(ctx, g):
+        (hidden_map,) = ctx.saved_tensors
+        ext = torch.cat([g.contiguous(), g.new_zeros(1, g.shape[1])])  # row R: the -1 sentinel's zero row
+        return gather_rows(ext, hidden_map), None, None
+
+
+class _ToCells(torch.autograd.Function):
+    """Compact values [R] -> [bsz, L] (zeros past r_b); the backward gathers the cells' gradients back to compact rows.
+    shift 1 reads each cell one compact row later (the FSDP-packed entropy alignment)."""
+
+    @staticmethod
+    def forward(ctx, v, cell_map, back_idx, shift, shape):
+        ctx.save_for_backward(back_idx)
+        ext = torch.cat([v, v.new_zeros(1)])
+        return gather_rows(ext[shift:], cell_map).view(shape)
+
+    @staticmethod
+    def backward(ctx, g):
+        (back_idx,) = ctx.saved_tensors
+        ext = torch.cat([g.reshape(-1).float(), g.new_zeros(1, dtype=torch.float32)])
+        return gather_rows(ext, back_idx), None, None, None, None
+
+
+def response_logprobs_entropy(hidden, weight, tokens, plan, *, temperature: float = 1.0, compute_entropy: bool = True,
+                              group=None):
+    """Log-probabilities and entropies of `hidden @ weight.T / temperature` at the response tokens of a padded or
+    packed batch, computed on the plan's rows only and returned as (logprobs [bsz, response_len], entropy
+    [bsz, response_len] or None), fp32, zeros at j >= r_b - the layout reasoning_actor_loss reads.
+    hidden: [T, H], [1, T, H], [T, 1, H] (Megatron's sequence-first output) or [bsz, S, H], bf16; tokens: the
+    matching token ids (targets are read from them).  plan: a response_rows.padded / fsdp_packed / megatron_thd plan.
+    weight is lm_head.weight [V, H] on one rank, or the rank's vocabulary shard when `group` (resolved as in
+    vocab_parallel_linear_logprobs_entropy) has more than one rank; the all-gather then covers the plan's R rows.
+    Differentiable w.r.t. hidden and weight (only where required); dX is zero on rows outside every response.
+    Host syncs: none with host lengths; one device-to-host copy of R and the plan's verdict with device lengths;
+    none in the backward.  With R = 0 the outputs are constant zeros."""
+    what = "response_logprobs_entropy"
+    if hidden.dim() not in (2, 3):
+        raise ValueError(f"{what}: hidden must be [T, H], [1, T, H], [T, 1, H] or [bsz, S, H], got "
+                         f"{tuple(hidden.shape)}")
+    _lmhead_check(hidden, weight)
+    group, P, _ = _vp_group(group, what)
+    x = hidden.reshape(-1, hidden.shape[-1])
+    T = x.shape[0]
+    tok = L.to_device(tokens, x.device, torch.int64).reshape(-1)
+    if tok.numel() != T:
+        raise ValueError(f"{what}: {tok.numel()} token ids for {T} hidden rows")
+    idx = plan.index(tok, T)
+    shape = (plan.bsz, plan.response_len)
+    if idx.R == 0:
+        z = torch.zeros(shape, dtype=torch.float32, device=x.device)
+        return z, (torch.zeros_like(z) if compute_entropy else None)
+    hc = _GatherRows.apply(x, idx.rows, idx.hidden_map)
+    if P == 1:
+        lp, ent = linear_logprobs_entropy(hc, weight, idx.targets, temperature, None, compute_entropy)
+    else:
+        lp, ent = vocab_parallel_linear_logprobs_entropy(hc, weight, idx.targets, group=group, temperature=temperature,
+                                                         compute_entropy=compute_entropy)
+    s = plan.entropy_shift
+    lp = _ToCells.apply(lp, idx.cell_map, idx.cells[1:], 0, shape)
+    if compute_entropy:
+        ent = _ToCells.apply(ent, idx.cell_map, idx.cells[1 - s:1 - s + idx.R], s, shape)
+    return lp, ent
