@@ -619,6 +619,39 @@ int rb200_response_rows_plan(int layout, const int64_t* len0, const int64_t* len
                              int64_t capacity, int64_t* rows, int64_t* targets, int64_t* cell_map,
                              int64_t* hidden_map, int64_t* cells, int64_t* status, rb200_stream_t stream);
 
+/* Response-rows plan under Megatron sequence (SP) and context (CP) parallelism (csrc/response_rows_mp.cu), for one
+ * rank (tp_rank, cp_rank).  Lengths as rb200_response_rows_plan's layout 2: cu_seqlens_padded [bsz + 1] (N_b = its
+ * differences, multiples of 2 cp when cp > 1), seq_lengths n_b, response_lengths r_b; responses [bsz, L] holds the
+ * targets.  Ownership follows preprocess_packed_seqs: with cp = 1 sequence b sits at CP-local rows cu[b] + p; with
+ * cp > 1, half = N_b / (2 cp), CP rank c holds positions [half c, half (c + 1)) at rows cu[b] / cp + ... and
+ * [N_b - half (c + 1), N_b - half c) at rows cu[b] / cp + half + ...  T_c = rows of the CP-local stream; under SP TP
+ * rank k holds rows [k Ts, (k + 1) Ts), Ts = T_c / tp.  Token j < r_b is predicted at position n_b - r_b - 1 + j.
+ * A CP rank's R_c compact rows are its prediction rows in ascending local row; TP shard k holds cnt_k of them, starting
+ * at off_k.  Rmax_k = max(1, max_k cnt_k) (SP), Rmax_c = max(1, max_c R_c).  Outputs (-1 = pad / zero row):
+ *   rows [R_c]: CP-local row of each compact row;  targets [R_c]: responses[b, j];  cells [R_c]: b L + j;
+ *   unpad [R_c]: row of the TP-gathered [tp, Rmax_k] buffer holding each compact row (SP; identity without);
+ *   send [Rmax_k] (SP): the rank's compact rows as rows of its shard, -1 past cnt_k;
+ *   slot_map [tp * Rmax_k] (SP): the compact row each slot of the reduce-scatter layout carries, or -1;
+ *   cell_map [bsz L]: row of the CP-gathered [cp, Rmax_c] values holding cell (b, j), or -1 for j >= r_b;
+ *   hidden_map [Ts] (SP: the slot of the reduce-scattered [Rmax_k] rows) or [T_c] (no SP: the compact row), or -1;
+ *   status [1 + cp tp]: {RB200_RR_* bits, then cnt of every rank (c, k) in c-major order (R_c in every k without SP)}.
+ * Only entries below capacity_c (R_c) and capacity_k (Rmax_k) are written.  tp * cp <= 64, bsz <= 8192.  One launch. */
+enum {
+  RB200_RR_SHARD = 64,     /* T_c < cu[bsz] / cp, or T_c not divisible by tp under SP */
+  RB200_RR_CP_ALIGN = 128  /* cp > 1 and a padded length N_b (or cu[0]) is not a multiple of 2 cp */
+};
+int rb200_response_rows_mp_plan(const int64_t* cu_seqlens_padded, const int64_t* seq_lengths,
+                                const int64_t* response_lengths, const int64_t* responses, int64_t bsz, int64_t L,
+                                int64_t T_c, int tp_size, int cp_size, int sequence_parallel, int tp_rank, int cp_rank,
+                                int64_t capacity_c, int64_t capacity_k, int64_t* rows, int64_t* send, int64_t* unpad,
+                                int64_t* slot_map, int64_t* targets, int64_t* cell_map, int64_t* cells,
+                                int64_t* hidden_map, int64_t* status, rb200_stream_t stream);
+/* Backward tail: out [n_out, H] bf16 = dx [idx[i], :] fp32 rounded once to nearest even, zero rows where idx[i] < 0.
+ * With the plan's slot_map it writes the [tp, Rmax_k, H] reduce-scatter send layout; with its hidden_map (no SP), dX
+ * of the whole [T_c, H] input.  H % 8 == 0, 16-byte aligned pointers. */
+int rb200_response_rows_mp_pack_grad(const float* dx, const int64_t* idx, void* out, int64_t n_out, int64_t H,
+                                     rb200_stream_t stream);
+
 /* Value tower only: values [n,value_dim] = ValueHead(states). Used for the bootstrap value of
  * final observations (get_bootstrap_values, workers/rollout/hf/huggingface_worker.py:612-627). */
 int rb200_mlp_value(const rb200_mlp_layout* L, const float* params, const float* wsplit,

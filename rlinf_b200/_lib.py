@@ -192,6 +192,9 @@ SIGNATURES = {
     "rb200_vp_combine": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_int] + [c_void_p] * 4),
     "rb200_response_rows_plan": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                          c_int, c_void_p, c_int64] + [c_void_p] * 6 + [c_void_p]),
+    "rb200_response_rows_mp_plan": (c_int, [c_void_p] * 4 + [c_int64] * 3 + [c_int] * 5 + [c_int64] * 2
+                                    + [c_void_p] * 9 + [c_void_p]),
+    "rb200_response_rows_mp_pack_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "rb200_mlp_value":(c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "rb200_synth_env_step": (c_int, [c_void_p] * 13 + [c_int] * 5 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),
     "rb200_synth_env_chunk_step": (c_int, [c_void_p] * 13 + [c_int] * 6 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),

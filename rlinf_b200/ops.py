@@ -1130,3 +1130,213 @@ def response_logprobs_entropy(hidden, weight, tokens, plan, *, temperature: floa
     if compute_entropy:
         ent = _ToCells.apply(ent, idx.cell_map, idx.cells[1 - s:1 - s + idx.R], s, shape)
     return lp, ent
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Response rows under Megatron sequence and context parallelism: each rank passes its hidden-state shard, only the
+# response rows cross the tensor-parallel group (response_rows.megatron_parallel, csrc/response_rows_mp.cu).  The
+# stages below are one rank's work between collectives; megatron_response_logprobs_entropy runs them with
+# torch.distributed, and a test can run them rank by rank with each collective replaced by a concatenation or a sum.
+# ---------------------------------------------------------------------------------------------------------------
+def mp_pack(hidden_shard, idx):
+    """The rank's response rows: [Rmax_k, H] (SP; pad rows repeat a row of the shard and are dropped by mp_unpad),
+    or the CP rank's compact rows [R_c, H] without SP."""
+    x = hidden_shard.reshape(-1, hidden_shard.shape[-1])
+    return gather_rows(x, idx.send if idx.sp else idx.rows)
+
+
+def mp_unpad(gathered, idx):
+    """TP-gathered rows [tp, Rmax_k, H] -> the CP rank's compact rows [R_c, H] (SP)."""
+    return gather_rows(gathered.reshape(-1, gathered.shape[-1]), idx.unpad)
+
+
+def mp_values(logprob, entropy, idx):
+    """Compact log-probs / entropies [R_c] -> the [Rmax_c, 2] fp32 buffer of the CP all-gather (zero pad rows)."""
+    vals = torch.zeros((idx.Rmax_c, 2), dtype=torch.float32, device=idx.cell_map.device)
+    if idx.R:
+        vals[:idx.R, 0] = logprob
+        if entropy is not None:
+            vals[:idx.R, 1] = entropy
+    return vals
+
+
+def mp_to_cells(gathered, idx, shape, compute_entropy=True):
+    """CP-gathered values [cp, Rmax_c, 2] -> (logprobs [bsz, L], entropy [bsz, L] or None), zeros at j >= r_b."""
+    ext = torch.cat([gathered.reshape(-1, 2), gathered.new_zeros(1, 2)])  # row cp * Rmax_c: the -1 sentinel's zeros
+    out = gather_rows(ext, idx.cell_map)
+    lp = out[:, 0].reshape(shape).contiguous()
+    return lp, (out[:, 1].reshape(shape).contiguous() if compute_entropy else None)
+
+
+def mp_cell_grads(grad_logprob, grad_entropy, idx):
+    """Gradients of the [bsz, L] outputs -> the CP rank's compact rows [R_c] (other CP ranks' cells are dropped)."""
+    def one(g):
+        return None if g is None else gather_rows(g.reshape(-1).float().contiguous(), idx.cells)
+    return one(grad_logprob), one(grad_entropy)
+
+
+def mp_pack_grad(dx32, idx):
+    """The rank's fp32 dX share of the compact rows [R_c, H] -> bf16, rounded once: the [tp, Rmax_k, H]
+    reduce-scatter send layout (SP, zero pad rows), or, without SP, dX of the whole [T_c, H] input (zeros off the
+    response rows; dx32 is then already summed over the TP ranks)."""
+    H = dx32.shape[-1]
+    m = idx.slot_map if idx.sp else idx.hidden_map
+    out = torch.empty((m.numel(), H), dtype=torch.bfloat16, device=m.device)
+    if idx.R == 0:  # a rank without prediction rows sends zeros
+        out.zero_()
+    else:
+        L.check(L.load().rb200_response_rows_mp_pack_grad(L.ptr(dx32), L.ptr(m), L.ptr(out), m.numel(), H,
+                                                          L.stream_ptr(m.device)), "response_rows_mp_pack_grad")
+    return out.view(idx.tp, idx.Rmax_k, H) if idx.sp else out
+
+
+def mp_grad_buffer(idx, H: int):
+    """[Rmax_k + 1, H] bf16 receive buffer of the reduce-scatter (SP): rows [:Rmax_k] are written by the collective,
+    the last row is the zero row of the -1 sentinel."""
+    buf = torch.empty((idx.Rmax_k + 1, H), dtype=torch.bfloat16, device=idx.cell_map.device)
+    buf[-1].zero_()
+    return buf
+
+
+def mp_unpack_grad(buf, idx):
+    """Reduce-scattered rows (mp_grad_buffer) -> dX of the rank's hidden shard [T_c / tp, H], zeros elsewhere."""
+    return gather_rows(buf, idx.hidden_map)
+
+
+def _mp_group(group, kind: str, size: int, what: str):
+    """(group, size, rank) of Megatron's tensor- or context-parallel group: group=None resolves to Megatron's group
+    when megatron.core's model parallelism is initialised, to one rank when torch.distributed is not initialised or the
+    plan has one rank along this dimension, and is an error otherwise."""
+    import torch.distributed as dist
+
+    if not (dist.is_available() and dist.is_initialized()):
+        got = (None, 1, 0)
+    else:
+        if group is None:
+            try:
+                from megatron.core import parallel_state
+            except ImportError:
+                parallel_state = None
+            if parallel_state is not None and parallel_state.model_parallel_is_initialized():
+                group = (parallel_state.get_tensor_model_parallel_group() if kind == "tp"
+                         else parallel_state.get_context_parallel_group())
+            elif size > 1:
+                raise ValueError(f"{what}: the plan has {kind}_size {size} and Megatron's model parallelism is not "
+                                 f"initialised; pass the {kind} group as {kind}_group=")
+        got = (None, 1, 0) if group is None else (group, dist.get_world_size(group), dist.get_rank(group))
+    if got[1] != size:
+        raise ValueError(f"{what}: the {kind} group has {got[1]} ranks, the plan {kind}_size {size}")
+    return got
+
+
+class _MegatronResponseRows(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, hidden, weight_shard, idx, tp_group, cp_group, temperature, want_entropy, shape):
+        import torch.distributed as dist
+
+        H = hidden.shape[-1]
+        tp, cp, k = idx.tp, idx.cp, idx.k
+        if idx.sp:
+            send = mp_pack(hidden, idx)
+            if tp > 1:
+                gathered = torch.empty((tp, idx.Rmax_k, H), dtype=send.dtype, device=send.device)
+                dist.all_gather_into_tensor(gathered, send, group=tp_group)
+            else:
+                gathered = send[None]
+            hc = mp_unpad(gathered, idx)
+        else:
+            hc = mp_pack(hidden, idx)
+        w = weight_shard.contiguous()
+        Vs = w.shape[0]
+        if idx.R:
+            rec = _lmhead_vp_fwd(hc, idx.R, idx.R, idx.R * H, H, w, idx.targets, k, 0, tp * Vs, temperature)
+        else:
+            rec = torch.empty((0, 4), dtype=torch.float32, device=hc.device)
+        recs = _vp_gather(rec, tp_group, tp)
+        if idx.R:
+            lp, ent, lse = vp_combine(recs, idx.targets, Vs, None, want_entropy)
+        else:
+            lp = ent = lse = rec[:, 0]
+        vals = mp_values(lp, ent, idx)
+        if cp > 1:
+            allv = torch.empty((cp, *vals.shape), dtype=vals.dtype, device=vals.device)
+            dist.all_gather_into_tensor(allv, vals, group=cp_group)
+        else:
+            allv = vals[None]
+        out_lp, out_ent = mp_to_cells(allv, idx, shape, want_entropy)
+        ctx.save_for_backward(hc, w, lse, ent if want_entropy else lse)
+        ctx.meta = (idx, tp_group, float(temperature), want_entropy, tuple(hidden.shape))
+        if want_entropy:
+            return out_lp, out_ent
+        none = out_lp.new_zeros(())
+        ctx.mark_non_differentiable(none)
+        return out_lp, none
+
+    @staticmethod
+    def backward(ctx, g_lp, g_ent):
+        import torch.distributed as dist
+
+        hc, w, lse, ent = ctx.saved_tensors
+        idx, tp_group, temp, want_entropy, shape = ctx.meta
+        need_x, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (need_x or need_w):
+            return (None,) * 8
+        H, Vs, tp = hc.shape[1], w.shape[0], idx.tp
+        glp, gh = mp_cell_grads(g_lp, g_ent if want_entropy else None, idx)
+        if idx.R:
+            dx32, dw = _lmhead_vp_bwd(hc, idx.R, idx.R, idx.R * H, H, w, idx.targets, idx.k, 0, tp * Vs, temp, lse,
+                                      ent, glp, gh, need_x, need_w)
+        else:
+            dx32 = hc.new_zeros((0, H), dtype=torch.float32) if need_x else None
+            dw = torch.zeros_like(w) if need_w else None
+        dx = None
+        if need_x:
+            if idx.sp:
+                send = mp_pack_grad(dx32, idx)
+                buf = mp_grad_buffer(idx, H)
+                if tp > 1:
+                    dist.reduce_scatter_tensor(buf[:-1], send.reshape(-1, H), group=tp_group)  # bf16, as Megatron
+                else:
+                    buf[:-1].copy_(send[0])
+                dx = mp_unpack_grad(buf, idx)
+            else:
+                if tp > 1:
+                    dist.all_reduce(dx32, group=tp_group)  # fp32: the rank sum rounds to bf16 once, below
+                dx = mp_pack_grad(dx32, idx)
+            dx = dx.view(shape)
+        return dx, dw, None, None, None, None, None, None
+
+
+def megatron_response_logprobs_entropy(hidden_shard, weight_shard, responses, plan, *, temperature: float = 1.0,
+                                       compute_entropy: bool = True, tp_group=None, cp_group=None):
+    """response_logprobs_entropy for Megatron's packed THD batches under tensor, sequence and context parallelism, from
+    each rank's own hidden-state shard: hidden_shard is the decoder output [T_c / tp, 1, H] or [T_c / tp, H] under
+    sequence parallelism, [T_c, 1, H] or [T_c, H] without it (T_c = the CP rank's packed rows), bf16; weight_shard is
+    the rank's vocabulary shard of the output layer; responses = input_ids[:, -response_len:] [bsz, response_len], the
+    targets; plan = response_rows.megatron_parallel(...).  Returns (logprobs [bsz, response_len], entropy or None),
+    fp32, the same on every rank, zeros at j >= r_b - what the reference's loss reads from log_probs[:, -L-1:-1].
+    tp_group / cp_group: None resolves to Megatron's tensor- / context-parallel group when megatron.core's model
+    parallelism is initialised, to one rank when the plan has one rank along that dimension (or without
+    torch.distributed); sizes that disagree with the plan raise ValueError.
+    Collectives: forward, under SP one all-gather of the rank's padded response rows [Rmax_k, H] bf16 over TP, one
+    all-gather of the [R_c, 4] records over TP, one all-gather of [Rmax_c, 2] fp32 values over CP; backward, one bf16
+    reduce-scatter over TP under SP, or an fp32 all-reduce of [R_c, H] without it, and nothing over CP.  As in the
+    reference's postprocess_packed_seqs, other CP ranks' cells arrive detached: a rank's dX comes only from the cells
+    whose rows it holds, its d_weight_shard from all of its CP rank's rows.  Host syncs: none with host lengths; one
+    device-to-host copy of the counts and the plan's verdict with device lengths."""
+    what = "megatron_response_logprobs_entropy"
+    if hidden_shard.dim() not in (2, 3) or (hidden_shard.dim() == 3 and hidden_shard.shape[1] != 1):
+        raise ValueError(f"{what}: hidden_shard must be [rows, H] or [rows, 1, H], got {tuple(hidden_shard.shape)}")
+    _lmhead_check(hidden_shard, weight_shard)
+    tp_group, tp, k = _mp_group(tp_group, "tp", plan.tp_size, what)
+    cp_group, cp, c = _mp_group(cp_group, "cp", plan.cp_size, what)
+    x = hidden_shard.reshape(-1, hidden_shard.shape[-1])
+    resp = L.to_device(responses, x.device, torch.int64)
+    idx = plan.index(resp, x.shape[0], k, c)
+    shape = (plan.bsz, plan.response_len)
+    if all(sum(r) == 0 for r in idx.counts):  # no response row on any rank: no collective on any rank
+        z = torch.zeros(shape, dtype=torch.float32, device=x.device)
+        return z, (torch.zeros_like(z) if compute_entropy else None)
+    lp, ent = _MegatronResponseRows.apply(hidden_shard, weight_shard, idx, tp_group, cp_group, temperature,
+                                          bool(compute_entropy), shape)
+    return lp, (ent if compute_entropy else None)

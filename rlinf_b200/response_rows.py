@@ -18,6 +18,9 @@ Lengths on the host are checked on the host when the plan is built (and against 
 sync.  Lengths on the device are checked by the plan kernel, whose verdict comes back with R in one device-to-host
 copy.  Violations raise ValueError.  `index()` runs the plan kernel (csrc/response_rows.cu) and returns the index maps
 that ops.response_logprobs_entropy gathers with.
+
+megatron_parallel(...) is the Megatron THD layout under sequence and context parallelism, for
+ops.megatron_response_logprobs_entropy: each rank holds a shard of the packed stream (csrc/response_rows_mp.cu).
 """
 from __future__ import annotations
 
@@ -39,6 +42,9 @@ _ERRORS = {
     8: "sequences overlap or are not in ascending order",
     16: "a prompt length exceeds max_prompt_len",
     32: "more response rows than the plan's capacity",
+    64: "the hidden shard has too few rows for the packed stream (T_c < cu_seqlens_padded[-1] / cp_size), or T_c is "
+        "not divisible by tp_size",
+    128: "a padded sequence length (or cu_seqlens_padded[0]) is not a multiple of 2 * cp_size",
 }
 
 
@@ -207,3 +213,187 @@ def megatron_thd(cu_seqlens_padded, seq_lengths, response_lengths, *, response_l
         return ResponseRowPlan(MEGATRON_THD, bsz, response_len, 0, 0, cu.to(dev), n.to(dev), resp.to(dev))
     starts = cu[:-1]
     return _host_plan(MEGATRON_THD, bsz, response_len, 0, 0, cu, n, resp, starts, starts + n - resp, what)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Megatron THD under sequence (SP) and context (CP) parallelism
+# ---------------------------------------------------------------------------------------------------------------
+MP_MAX_RANKS = 64
+
+
+@dataclass(frozen=True)
+class MPIndex:
+    """Index maps of a megatron_parallel plan for rank (tp_rank k, cp_rank c) (int64, device; -1 = pad / zero row).
+    R is R_c, the prediction rows CP rank c holds; counts[c][k] the rows TP shard k of CP rank c holds (SP), or R_c in
+    every k without SP.  Rmax_k / Rmax_c are the padded row counts of the TP row all-gather and the CP value
+    all-gather (at least 1, so every collective has a buffer)."""
+    tp: int
+    cp: int
+    k: int
+    c: int
+    sp: bool
+    T_c: int
+    R: int
+    Rmax_k: int
+    Rmax_c: int
+    counts: tuple
+    rows: torch.Tensor        # [R] CP-local row of each compact row
+    targets: torch.Tensor     # [R] responses[b, j]
+    cells: torch.Tensor       # [R] response cell b * L + j of each compact row
+    unpad: torch.Tensor       # [R] row of the TP-gathered [tp * Rmax_k] buffer (SP), identity without
+    send: Optional[torch.Tensor]      # [Rmax_k] rows of the hidden shard to all-gather (SP), -1 = pad
+    slot_map: Optional[torch.Tensor]  # [tp * Rmax_k] compact row of each reduce-scatter slot (SP), -1 = pad
+    cell_map: torch.Tensor    # [bsz * L] row of the CP-gathered [cp * Rmax_c] values, -1 past r_b
+    hidden_map: torch.Tensor  # [T_c / tp] slot of the reduce-scattered rows (SP) or [T_c] compact row (no SP)
+
+    @property
+    def shard_rows(self) -> int:
+        return self.T_c // self.tp if self.sp else self.T_c
+
+
+def _mp_runs(cu, n, resp, cp: int, c: int):
+    """Per sequence, CP rank c's two runs of prediction rows: (tA, cA, tB, cB), CP-local rows (host tensors)."""
+    N = cu[1:] - cu[:-1]
+    p0 = n - resp - 1
+    p1 = p0 + resp.clamp(min=0)
+    if cp == 1:
+        start, half, a0, a1 = cu[:-1], N, torch.zeros_like(N), N
+        b0 = b1 = torch.zeros_like(N)
+    else:
+        start, half = cu[:-1] // cp, N // (2 * cp)
+        a0 = half * c
+        a1 = a0 + half
+        b0 = N - half * (c + 1)
+        b1 = b0 + half
+    pA, pB = torch.maximum(p0, a0), torch.maximum(p0, b0)
+    cA = (torch.minimum(p1, a1) - pA).clamp(min=0)
+    cB = (torch.minimum(p1, b1) - pB).clamp(min=0)
+    return start + pA - a0, cA, start + half + pB - b0, cB
+
+
+def _overlap(t0, cnt, lo, hi) -> int:
+    return int((torch.minimum(t0 + cnt, torch.full_like(t0, hi)) - t0.clamp(min=lo)).clamp(min=0).sum())
+
+
+@dataclass(frozen=True)
+class MegatronParallelPlan:
+    bsz: int
+    response_len: int
+    tp_size: int
+    cp_size: int
+    sequence_parallel: bool
+    cu: torch.Tensor
+    n: torch.Tensor
+    resp: torch.Tensor
+
+    @property
+    def on_device(self) -> bool:
+        return self.resp.is_cuda
+
+    def counts(self, T_c: int):
+        """Rows of every rank (c, k) as nested tuples [cp][tp] (host plans; no device work)."""
+        tp, cp, sp = self.tp_size, self.cp_size, self.sequence_parallel
+        out = []
+        for c in range(cp):
+            tA, cA, tB, cB = _mp_runs(self.cu, self.n, self.resp, cp, c)
+            if sp:
+                Ts = T_c // tp
+                out.append(tuple(_overlap(tA, cA, k * Ts, (k + 1) * Ts) + _overlap(tB, cB, k * Ts, (k + 1) * Ts)
+                                 for k in range(tp)))
+            else:
+                out.append((int(cA.sum() + cB.sum()),) * tp)
+        return tuple(out)
+
+    def index(self, responses: torch.Tensor, shard_rows: int, tp_rank: int, cp_rank: int) -> MPIndex:
+        """Run the plan kernel for rank (tp_rank, cp_rank) whose hidden shard has `shard_rows` rows; responses
+        [bsz, response_len] int64 on the device."""
+        what = "megatron_response_logprobs_entropy"
+        tp, cp, sp = self.tp_size, self.cp_size, self.sequence_parallel
+        if not (0 <= tp_rank < tp and 0 <= cp_rank < cp):
+            raise ValueError(f"{what}: rank (tp {tp_rank}, cp {cp_rank}) outside the plan's tp {tp} x cp {cp} grid")
+        T_c = shard_rows * tp if sp else shard_rows
+        dev = responses.device
+        if tuple(responses.shape) != (self.bsz, self.response_len):
+            raise ValueError(f"{what}: responses must be [bsz, response_len] = [{self.bsz}, {self.response_len}], "
+                             f"got {tuple(responses.shape)}")
+        if self.on_device:
+            counts = None
+            cap_c = min(T_c, self.bsz * self.response_len)
+            cap_k = min(T_c // tp, cap_c) if sp else 0
+            lens = [t.to(dev) for t in (self.cu, self.n, self.resp)]
+        else:
+            if int(self.cu[-1]) // cp > T_c or T_c <= 0:
+                raise _error(64, what)
+            counts = self.counts(T_c)
+            cap_c = sum(counts[cp_rank]) if sp else counts[cp_rank][0]
+            cap_k = max(1, max(counts[cp_rank])) if sp else 0
+            flat = torch.cat([self.cu, self.n, self.resp]).to(dev, non_blocking=True)  # one copy, no host sync
+            b = self.bsz
+            lens = [flat[:b + 1], flat[b + 1:2 * b + 1], flat[2 * b + 1:]]
+        i64 = dict(dtype=torch.int64, device=dev)
+        rows, targets, cells, unpad = (torch.empty(cap_c, **i64) for _ in range(4))
+        send = torch.empty(cap_k, **i64) if sp else None
+        slot_map = torch.empty(tp * cap_k, **i64) if sp else None
+        cell_map = torch.empty(self.bsz * self.response_len, **i64)
+        hidden_map = torch.empty(shard_rows, **i64)
+        status = torch.empty(1 + cp * tp, **i64)
+        L.check(L.load().rb200_response_rows_mp_plan(
+            L.ptr(lens[0]), L.ptr(lens[1]), L.ptr(lens[2]), L.ptr(responses), self.bsz, self.response_len, T_c, tp,
+            cp, int(sp), tp_rank, cp_rank, cap_c, cap_k, L.ptr(rows), L.ptr(send), L.ptr(unpad), L.ptr(slot_map),
+            L.ptr(targets), L.ptr(cell_map), L.ptr(cells), L.ptr(hidden_map), L.ptr(status), L.stream_ptr(dev)),
+            "response_rows_mp_plan")
+        if counts is None:
+            st = status.tolist()  # the forward's one device-to-host copy
+            if st[0]:
+                raise _error(st[0], what)
+            counts = tuple(tuple(st[1 + c * tp:1 + (c + 1) * tp]) for c in range(cp))
+        R = sum(counts[cp_rank]) if sp else counts[cp_rank][0]
+        Rmax_c = max(1, max(sum(x) if sp else x[0] for x in counts))
+        Rmax_k = max(1, max(counts[cp_rank])) if sp else R
+        nk = Rmax_k if sp else 0
+        return MPIndex(tp, cp, tp_rank, cp_rank, sp, T_c, R, Rmax_k, Rmax_c, counts, rows[:R], targets[:R],
+                       cells[:R], unpad[:R], send[:nk] if sp else None, slot_map[:tp * nk] if sp else None,
+                       cell_map, hidden_map)
+
+
+def megatron_parallel(cu_seqlens_padded, seq_lengths, response_lengths, *, response_len: int, tp_size: int = 1,
+                      cp_size: int = 1, sequence_parallel: bool = False) -> MegatronParallelPlan:
+    """Megatron's custom_forward with pack_seqs under tensor (tp_size), sequence (sequence_parallel) and context
+    (cp_size) parallelism, for ops.megatron_response_logprobs_entropy.  The lengths are megatron_thd's: the
+    cu_seqlens_padded of preprocess_packed_seqs (padded lengths N_b, multiples of 2 * cp_size when cp_size > 1), n_b =
+    attention_mask.sum(-1) and r_b, on the host or the device.  Ownership follows preprocess_packed_seqs: with cp_size 1
+    sequence b sits at rows cu[b] + p of the packed stream; with cp_size > 1, half = N_b / (2 cp), CP rank c holds
+    positions [half c, half (c + 1)) at its rows cu[b] / cp + ... and [N_b - half (c + 1), N_b - half c) at
+    cu[b] / cp + half + ...; under sequence parallelism TP rank k holds rows [k T_c / tp, (k + 1) T_c / tp) of its CP
+    rank's T_c rows.  Every rank must pass the same lengths: they are not compared across ranks (that would cost a
+    collective), and lengths that disagree give wrong collective sizes."""
+    what = "response_rows.megatron_parallel"
+    tp, cp, sp = int(tp_size), int(cp_size), bool(sequence_parallel)
+    if tp < 1 or cp < 1 or tp * cp > MP_MAX_RANKS:
+        raise ValueError(f"{what}: needs tp_size, cp_size >= 1 and tp_size * cp_size <= {MP_MAX_RANKS}, got "
+                         f"{tp} x {cp}")
+    cu = _lengths(cu_seqlens_padded, "cu_seqlens_padded")
+    n = _lengths(seq_lengths, "seq_lengths")
+    resp = _lengths(response_lengths, "response_lengths")
+    bsz, response_len = n.numel(), int(response_len)
+    _check_common(bsz, response_len, what)
+    if cu.numel() != bsz + 1 or resp.numel() != bsz:
+        raise ValueError(f"{what}: needs bsz + 1 = {bsz + 1} cu_seqlens_padded and {bsz} response lengths, got "
+                         f"{cu.numel()} and {resp.numel()}")
+    if cu.is_cuda or n.is_cuda or resp.is_cuda:
+        dev = next(t.device for t in (cu, n, resp) if t.is_cuda)
+        return MegatronParallelPlan(bsz, response_len, tp, cp, sp, cu.to(dev), n.to(dev), resp.to(dev))
+    bits = 0
+    if bool(((resp < 0) | (resp > response_len)).any()):
+        bits |= 1
+    if bool((n - resp < 1).any()):
+        bits |= 2
+    if int(cu[0]) < 0:
+        bits |= 4
+    if bool((cu[:-1] + n > cu[1:]).any()):
+        bits |= 8
+    if cp > 1 and (bool(((cu[1:] - cu[:-1]) % (2 * cp) != 0).any()) or int(cu[0]) % (2 * cp) != 0):
+        bits |= 128
+    if bits:
+        raise _error(bits, what)
+    return MegatronParallelPlan(bsz, response_len, tp, cp, sp, cu, n, resp)
