@@ -306,6 +306,67 @@ typedef struct rb200_token_loss_args {
 int64_t rb200_token_loss_workspace_bytes(int64_t bsz, int64_t L);
 int rb200_token_ppo_loss(const rb200_token_loss_args* args, rb200_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Token-level PPO critic loss of the reasoning workers (csrc/token_critic_loss.cu): compute_ppo_critic_loss
+ *   (losses.py:315-380) as MegatronCritic's loss_func calls it (workers/critic/megatron_critic_worker.py:92-123) on
+ *   [bsz, L] values, returns, prev_values and a loss mask, with huber_delta and value_clip:
+ *     vpc = prev + clamp(values - prev, -value_clip, value_clip)
+ *     loss = masked_mean(max(huber(returns - values), huber(returns - vpc)), mask)  (the plain masked sum, i.e. 0,
+ *            when every cell is masked: masked_mean, utils.py:321-328; the worker's loss_agg_func is not applied)
+ *   and d loss / d values for a unit upstream gradient.  Row i, token j of each input is at ptr[i * <name>_stride + j]
+ *   (strides in elements, >= L); loss_mask is uint8 / bool, the rest fp32.  Four launches (the token loss's mask
+ *   counts and totals, then the critic's main and finish kernels), fp64 partials in fixed slots, no atomics, no host
+ *   sync: two identical calls give the same bits on any SM count.
+ * Outputs: loss [1], metrics [RB200_CM_NUM] (RB200_CM_*), d_values [bsz, L] contiguous or NULL.  workspace:
+ *   rb200_token_loss_workspace_bytes(bsz, L) bytes, 16-byte aligned, no initialisation needed.
+ * ---------------------------------------------------------------------------------------- */
+enum {
+  RB200_CM_VALUE_LOSS = 0,        /* critic/value_loss */
+  RB200_CM_VALUE_CLIP_RATIO = 1,  /* critic/value_clip_ratio: unmasked mean over all bsz L cells */
+  RB200_CM_EV_COUNT = 2,          /* __sum__/_critic_explained_variance/count (masked cells) */
+  RB200_CM_EV_RET_SUM = 3,        /* .../returns_sum */
+  RB200_CM_EV_RET_SQ_SUM = 4,     /* .../returns_sq_sum */
+  RB200_CM_EV_ERR_SUM = 5,        /* .../errors_sum (errors = returns - values) */
+  RB200_CM_EV_ERR_SQ_SUM = 6,     /* .../errors_sq_sum */
+  RB200_CM_FINAL_VALUE_LOSS = 7,  /* critic/final_value_loss (= loss[0]) */
+  RB200_CM_NUM = 8
+};
+typedef struct rb200_token_critic_loss_args {
+  int64_t bsz, L;
+  const float* values;       int64_t values_stride;
+  const float* returns;      int64_t returns_stride;
+  const float* prev_values;  int64_t prev_values_stride;
+  const uint8_t* loss_mask;  int64_t loss_mask_stride;
+  double value_clip, huber_delta;
+  void* workspace;
+  int64_t workspace_bytes;
+  float* loss;
+  float* metrics;
+  float* d_values;
+} rb200_token_critic_loss_args;
+int rb200_token_critic_loss(const rb200_token_critic_loss_args* args, rb200_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Value head of the reasoning critic on a plan's rows (csrc/value_head.cu): the reference's LinearForLastLayer(H, 1)
+ *   (a bf16 nn.Linear without bias, output cast with .float()) evaluated in place on rows of a hidden shard x
+ *   (bf16, unit inner stride, row_stride elements between rows, a multiple of 8; 16-byte aligned), w [1, H] bf16.
+ *   H % 64 == 0, 64 <= H <= 8192.
+ * rb200_value_head_fwd: v[i] = float(bf16(sum_h x[rows[i], h] w[h])) for i < n (fp32 sum in a fixed order, one
+ *   rounding to bf16), v[i] = 0 where rows[i] == -1 (a pad slot).  One launch; reads n H 2 bytes.
+ * rb200_value_head_bwd: g [n] fp32, rounded to bf16 first (the backward of .float()); either output may be NULL.
+ *   dx [T, H] bf16 contiguous: dx[t] = bf16(g_bf16[inv_map[t]] w), exact zeros where inv_map[t] == -1; every row
+ *     written once.  One launch; writes T H 2 bytes.
+ *   dw [H] bf16 = bf16(sum_i g_bf16[i] x[rows[i]]) over rows[i] != -1: fp32 partials over fixed chunks of rows, added
+ *     in a fixed order (two launches; reads n H 2 bytes).  workspace: rb200_value_head_workspace_bytes(n, H) bytes,
+ *     16-byte aligned (-1 = unsupported shape).
+ *   No floating-point atomics and nothing that depends on the SM count: repeat calls give the same bits. */
+int64_t rb200_value_head_workspace_bytes(int64_t n, int64_t H);
+int rb200_value_head_fwd(const void* x, int64_t row_stride, const int64_t* rows, int64_t n, int64_t H, const void* w,
+                         float* v, rb200_stream_t stream);
+int rb200_value_head_bwd(const void* x, int64_t row_stride, const int64_t* rows, int64_t n, int64_t H, const float* g,
+                         const void* w, const int64_t* inv_map, int64_t T, void* dx, void* dw, void* workspace,
+                         int64_t workspace_bytes, rb200_stream_t stream);
+
 /* x[i] *= s (device scalar-free helper for autograd's upstream scalar). */
 int rb200_scale(float* x, int64_t n, float s, rb200_stream_t stream);
 /* x[i] *= *s_dev  (the scalar lives on the device: no host sync in autograd's backward). */

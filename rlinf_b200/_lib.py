@@ -113,6 +113,27 @@ class TokenLossArgs(C.Structure):
     ]
 
 
+# reasoning critic loss (mirror of RB200_CM_* / rb200_token_critic_loss_args)
+CM_NUM = 8
+CM_KEYS = {
+    0: "critic/value_loss", 1: "critic/value_clip_ratio",
+    2: "__sum__/_critic_explained_variance/count",
+    3: "__sum__/_critic_explained_variance/returns_sum",
+    4: "__sum__/_critic_explained_variance/returns_sq_sum",
+    5: "__sum__/_critic_explained_variance/errors_sum",
+    6: "__sum__/_critic_explained_variance/errors_sq_sum",
+    7: "critic/final_value_loss",
+}
+
+
+class TokenCriticLossArgs(C.Structure):
+    _fields_ = [("bsz", c_int64), ("L", c_int64)] + [
+        f for name in ("values", "returns", "prev_values", "loss_mask")
+        for f in ((name, c_void_p), (name + "_stride", c_int64))
+    ] + [("value_clip", c_double), ("huber_delta", c_double), ("workspace", c_void_p), ("workspace_bytes", c_int64),
+         ("loss", c_void_p), ("metrics", c_void_p), ("d_values", c_void_p)]
+
+
 class MlpLayout(C.Structure):
     _fields_ = [
         ("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("value_dim", C.c_int32), ("hidden", C.c_int32),
@@ -195,6 +216,11 @@ SIGNATURES = {
     "rb200_response_rows_mp_plan": (c_int, [c_void_p] * 4 + [c_int64] * 3 + [c_int] * 5 + [c_int64] * 2
                                     + [c_void_p] * 9 + [c_void_p]),
     "rb200_response_rows_mp_pack_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
+    "rb200_token_critic_loss": (c_int, [C.POINTER(TokenCriticLossArgs), c_void_p]),
+    "rb200_value_head_workspace_bytes": (c_int64, [c_int64, c_int64]),
+    "rb200_value_head_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
+    "rb200_value_head_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
+                                     c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "rb200_mlp_value":(c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "rb200_synth_env_step": (c_int, [c_void_p] * 13 + [c_int] * 5 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),
     "rb200_synth_env_chunk_step": (c_int, [c_void_p] * 13 + [c_int] * 6 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),

@@ -395,6 +395,21 @@ def reasoning_actor_loss(logprobs, advantages, loss_mask, *, old_logprobs=None, 
         fast_path_zero_loss_mask=fast_path_zero_loss_mask)
 
 
+def reasoning_critic_loss(values, returns, prev_values, loss_mask, *, value_clip: float,
+                          huber_delta: float = 10000.0) -> tuple[torch.Tensor, dict]:
+    """The loss block of the reasoning critic (MegatronCritic's loss_func, workers/critic/megatron_critic_worker.py:
+    92-123) in one device pass, with the worker's own variables: values = vpreds [bsz, L] (e.g. from
+    ops.megatron_response_values), returns and prev_values = batch["returns"] / batch["values"], loss_mask =
+    response_mask[:, -L:], value_clip = the worker's value_clip; huber_delta is the worker's fixed 10000.  The
+    aggregation is masked_mean whatever the worker's loss_agg_func, as in compute_ppo_critic_loss.
+
+    Returns (loss, metrics): loss differentiable w.r.t. values; metrics are 0-dim device tensors under the worker's keys
+    (critic/value_loss, critic/value_clip_ratio, the five __sum__/_critic_explained_variance/* sums and
+    critic/final_value_loss), before Megatron's data-parallel reductions, which stay with the caller.  No host sync."""
+    return ops.token_critic_loss(values, returns, prev_values, loss_mask, value_clip=value_clip,
+                                 huber_delta=huber_delta)
+
+
 class _FusedOpdLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logprobs, cfg):

@@ -15,6 +15,7 @@
 // Elementwise arithmetic mirrors the reference's fp32 op order (so discrete metrics such as
 // clip_fraction agree); the reductions accumulate in fp64.
 #include "common.cuh"
+#include "critic_unit.cuh"
 #include "ppo_unit.cuh"
 
 namespace {
@@ -68,15 +69,6 @@ __global__ void __launch_bounds__(256) mask_count_kernel(const uint8_t* __restri
   }
   rb::block_sum<1>(v, red);
   if (threadIdx.x == 0 && v[0] != 0.0) atomicAdd(&sums[S_CNT], v[0]);
-}
-
-__device__ __forceinline__ float huber(float e, float delta, float half_delta) {
-  const float a = fabsf(e);
-  return a < delta ? __fmul_rn(0.5f, __fmul_rn(e, e)) : __fmul_rn(delta, __fsub_rn(a, half_delta));
-}
-__device__ __forceinline__ float huber_grad(float e, float delta) {
-  const float a = fabsf(e);
-  return a < delta ? e : (e > 0.0f ? delta : (e < 0.0f ? -delta : 0.0f));
 }
 
 using rb::RatioOut;
@@ -205,28 +197,20 @@ __global__ void __launch_bounds__(256, 3) ppo_main_kernel(rb200_ppo_args a, Hype
 
     if (a.with_critic) {
       const float v = a.values[u], pv = a.prev_values[so], rt = a.returns[so];
-      const float dv = __fsub_rn(v, pv);
-      const float dvc = fminf(fmaxf(dv, -h.value_clip), h.value_clip);
-      const float vpc = __fadd_rn(pv, dvc);
-      const float e1 = __fsub_rn(rt, v), e2 = __fsub_rn(rt, vpc);
-      const float lo = huber(e1, h.huber_delta, h.half_huber_delta);
-      const float lc = huber(e2, h.huber_delta, h.half_huber_delta);
-      const float vl = fmaxf(lo, lc);
+      const rb::CriticOut o = rb::critic_terms(v, pv, rt, h.value_clip, h.huber_delta, h.half_huber_delta);
+      const float vl = o.vl;
       const float term = has_mask ? (ratio_agg ? __fmul_rn(__fdiv_rn(vl, w), mf) : __fmul_rn(vl, mf)) : vl;
       acc[S_VL] += term;
-      acc[S_VCLIP] += (fabsf(__fsub_rn(vpc, pv)) > h.value_clip) ? 1.0f : 0.0f;
+      acc[S_VCLIP] += rb::critic_clip_hit(o, pv, h.value_clip) ? 1.0f : 0.0f;
       if (m) {
         acc[S_EV_N] += 1.0f;
         acc[S_EV_R] += rt;
         acc[S_EV_R2] += __fmul_rn(rt, rt);
-        acc[S_EV_E] += e1;
-        acc[S_EV_E2] += __fmul_rn(e1, e1);
+        acc[S_EV_E] += o.e1;
+        acc[S_EV_E2] += __fmul_rn(o.e1, o.e1);
       }
       if (a.d_values) {
-        const float g1 = lo > lc ? 1.0f : (lo == lc ? 0.5f : 0.0f);
-        const float g2 = lc > lo ? 1.0f : (lo == lc ? 0.5f : 0.0f);
-        const bool pass_c = (dv >= -h.value_clip) && (dv <= h.value_clip);
-        const float dvl = -(g1 * huber_grad(e1, h.huber_delta)) - (pass_c ? g2 * huber_grad(e2, h.huber_delta) : 0.0f);
+        const float dvl = rb::critic_dvl(o, h.value_clip, h.huber_delta);
         const float cw = has_mask ? (ratio_agg ? coef_unit / w : coef_unit) * mf : coef_unit;
         a.d_values[u] = scale * cw * dvl;
       }

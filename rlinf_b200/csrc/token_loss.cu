@@ -17,6 +17,7 @@
 #include "common.cuh"
 #include "kl_unit.cuh"
 #include "ppo_unit.cuh"
+#include "token_counts.cuh"
 
 namespace {
 
@@ -240,6 +241,24 @@ __global__ void __launch_bounds__(kThreads) finalize_kernel(rb200_token_loss_arg
 int64_t num_segments(int64_t L) { return (L + kSeg - 1) / kSeg; }
 
 }  // namespace
+
+static_assert(kSeg == rb::kTokenSeg && kThreads == rb::kTokenThreads && kNS == rb::kTokenSlots,
+              "token_counts.cuh describes this file's segments and workspace");
+
+rb::TokenCounts rb::token_mask_counts(const uint8_t* mask, int64_t mask_stride, int64_t bsz, int64_t L,
+                                      void* workspace, cudaStream_t st) {
+  const int64_t nseg = num_segments(L);
+  const WsLayout w = ws_layout(bsz, nseg);
+  char* ws = static_cast<char*>(workspace);
+  Totals* tot = reinterpret_cast<Totals*>(ws);
+  int* seg_cnt = reinterpret_cast<int*>(ws + w.seg_cnt);
+  long long* row_cnt = reinterpret_cast<long long*>(ws + w.row_cnt);
+  count_kernel<<<dim3((unsigned)nseg, (unsigned)bsz), kThreads, 0, st>>>(mask, mask_stride, L, seg_cnt);
+  rb::count_launch();
+  totals_kernel<<<1, 1024, 0, st>>>(seg_cnt, bsz, (int)nseg, row_cnt, tot);
+  rb::count_launch();
+  return {nseg, row_cnt, &tot->total, reinterpret_cast<double*>(ws + w.partials)};
+}
 
 extern "C" int64_t rb200_token_loss_workspace_bytes(int64_t bsz, int64_t L) {
   if (bsz <= 0 || L <= 0 || bsz > 65535) return -1;

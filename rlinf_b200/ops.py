@@ -1340,3 +1340,245 @@ def megatron_response_logprobs_entropy(hidden_shard, weight_shard, responses, pl
     lp, ent = _MegatronResponseRows.apply(hidden_shard, weight_shard, idx, tp_group, cp_group, temperature,
                                           bool(compute_entropy), shape)
     return lp, (ent if compute_entropy else None)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Reasoning PPO critic: the value head on the response rows of Megatron packed batches under TP / SP / CP
+# (csrc/value_head.cu) and the token-level critic loss (csrc/token_critic_loss.cu)
+# ---------------------------------------------------------------------------------------------------------------
+def _value_head_check(hidden: torch.Tensor, weight: torch.Tensor, what: str):
+    if hidden.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16:
+        raise ValueError(f"{what}: hidden and value weight must be bfloat16, got {hidden.dtype} / {weight.dtype}")
+    if weight.dim() != 2 or weight.shape[0] != 1:
+        raise ValueError(f"{what}: the value weight must be [1, H], got shape {tuple(weight.shape)}")
+    H = weight.shape[1]
+    if hidden.shape[-1] != H:
+        raise ValueError(f"{what}: hidden size {hidden.shape[-1]} != the value weight's {H}")
+    if H % 64 != 0 or not 64 <= H <= 8192:
+        raise ValueError(f"{what}: needs H % 64 == 0 and 64 <= H <= 8192, got H = {H}")
+
+
+def _value_head_rows(x: torch.Tensor):
+    """(tensor, row stride) of [rows, H] hidden states: read in place when rows are 16-byte aligned."""
+    if x.stride(-1) == 1 and x.stride(0) % 8 == 0 and x.stride(0) >= x.shape[1] and x.data_ptr() % 16 == 0:
+        return x, x.stride(0)
+    x = x.contiguous()
+    return x, x.shape[1]
+
+
+def value_head_rows(x: torch.Tensor, rows: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """v [n] fp32 = float(bf16(x[rows] @ weight[0])) on rows of x [T, H] bf16 read in place; 0 where rows == -1."""
+    x, rs = _value_head_rows(x)
+    H = x.shape[1]
+    v = torch.empty(rows.numel(), dtype=torch.float32, device=x.device)
+    if rows.numel():
+        w = weight.contiguous()
+        L.check(L.load().rb200_value_head_fwd(L.ptr(x), rs, L.ptr(rows), rows.numel(), H, L.ptr(w), L.ptr(v),
+                                              L.stream_ptr(x.device)), "value_head_fwd")
+    return v
+
+
+def value_head_backward(x, rows, grad, weight, inv_map, need_x: bool, need_w: bool):
+    """Backward of value_head_rows for grad [n] fp32 (rounded to bf16 first): dX [inv_map.numel(), H] bf16 =
+    bf16(grad[inv_map[t]] * weight), zeros where inv_map == -1, and dW [1, H] bf16 = bf16(sum_i grad[i] x[rows[i]]);
+    either is None when not needed."""
+    x, rs = _value_head_rows(x)
+    H, n, T = x.shape[1], rows.numel(), inv_map.numel()
+    dev = x.device
+    w = weight.contiguous()
+    if n == 0 or T == 0:  # no row: every inv_map entry is -1, and dW is an empty sum
+        return (torch.zeros((T, H), dtype=torch.bfloat16, device=dev) if need_x else None,
+                torch.zeros((1, H), dtype=torch.bfloat16, device=dev) if need_w else None)
+    dx = torch.empty((T, H), dtype=torch.bfloat16, device=dev) if need_x else None
+    dw = torch.empty((1, H), dtype=torch.bfloat16, device=dev) if need_w else None
+    if not (need_x or need_w):
+        return dx, dw
+    wsb = L.load().rb200_value_head_workspace_bytes(n, H) if need_w else 0
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if need_w else None
+    g = grad.reshape(-1).float().contiguous()
+    L.check(L.load().rb200_value_head_bwd(L.ptr(x), rs, L.ptr(rows), n, H, L.ptr(g), L.ptr(w), L.ptr(inv_map), T,
+                                          L.ptr(dx), L.ptr(dw), L.ptr(ws), wsb, L.stream_ptr(dev)), "value_head_bwd")
+    return dx, dw
+
+
+def mp_value_head(hidden_shard, value_weight, idx):
+    """One rank's values: under SP [Rmax_k] fp32 for its own response rows in pad-slot order (the buffer of the TP
+    all-gather, zeros in pad slots); without SP [R_c], its CP rank's compact rows."""
+    x = hidden_shard.reshape(-1, hidden_shard.shape[-1])
+    return value_head_rows(x, idx.send if idx.sp else idx.rows, value_weight)
+
+
+def mp_value_unpad(gathered, idx):
+    """TP-gathered values [tp, Rmax_k] -> the CP rank's compact values [R_c] (SP)."""
+    return mp_unpad(gathered.reshape(-1, 1), idx).reshape(-1)
+
+
+def mp_value_head_backward(grad, hidden_shard, value_weight, idx, need_x: bool = True, need_w: bool = True):
+    """One rank's backward from the gradients of its CP rank's compact values [R_c] (mp_cell_grads): (dX of the hidden
+    shard, in its shape, or None; d value_weight [1, H] or None).  Under SP the rank takes its own slots' gradients
+    and its dW is its share of the TP sum; without SP every TP rank computes the full dW and the full dX."""
+    x = hidden_shard.reshape(-1, hidden_shard.shape[-1])
+    if idx.sp:
+        ext = torch.cat([grad.reshape(-1).float(), grad.new_zeros(1, dtype=torch.float32)])  # -1: the zero slot
+        own = idx.slot_map[idx.k * idx.Rmax_k:(idx.k + 1) * idx.Rmax_k]
+        g, rows = gather_rows(ext, own), idx.send
+    else:
+        g, rows = grad, idx.rows
+    dx, dw = value_head_backward(x, rows, g, value_weight, idx.hidden_map, need_x, need_w)
+    return (None if dx is None else dx.view(hidden_shard.shape)), dw
+
+
+class _MegatronResponseValues(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, hidden, value_weight, idx, tp_group, cp_group, shape):
+        import torch.distributed as dist
+
+        v = mp_value_head(hidden, value_weight, idx)
+        if idx.sp:
+            if idx.tp > 1:
+                gathered = torch.empty((idx.tp, idx.Rmax_k), dtype=v.dtype, device=v.device)
+                dist.all_gather_into_tensor(gathered, v, group=tp_group)
+            else:
+                gathered = v[None]
+            v = mp_value_unpad(gathered, idx)
+        vals = mp_values(v, None, idx)
+        if idx.cp > 1:
+            allv = torch.empty((idx.cp, *vals.shape), dtype=vals.dtype, device=vals.device)
+            dist.all_gather_into_tensor(allv, vals, group=cp_group)
+        else:
+            allv = vals[None]
+        out, _ = mp_to_cells(allv, idx, shape, False)
+        ctx.save_for_backward(hidden, value_weight)
+        ctx.idx = idx
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        hidden, w = ctx.saved_tensors
+        idx, ctx.idx = ctx.idx, None
+        need_x, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (need_x or need_w):
+            return (None,) * 6
+        grad, _ = mp_cell_grads(g, None, idx)
+        dx, dw = mp_value_head_backward(grad, hidden, w, idx, need_x, need_w)
+        return dx, dw, None, None, None, None
+
+
+def megatron_response_values(hidden_shard, value_weight, plan, *, tp_group=None, cp_group=None):
+    """The reasoning critic's values at the response tokens of a Megatron packed batch, from each rank's own
+    hidden-state shard: the reference's LinearForLastLayer(H, 1) value head (a bf16 Linear without bias, cast with
+    .float()) read at log_probs[:, -L-1:-1], computed on the response rows only.  hidden_shard is the decoder output
+    without the output layer, [T_c / tp, 1, H] or [T_c / tp, H] under sequence parallelism, [T_c, 1, H] or [T_c, H]
+    without it, bf16; value_weight is output_layer.weight [1, H] bf16; plan = response_rows.megatron_parallel(...)
+    (tp = cp = 1 is the megatron_thd layout).  Returns values [bsz, response_len] fp32, the same on every rank, zeros
+    at j >= r_b: the reference's inference output vpreds * mask, and the vpreds its loss reads.  Differentiable w.r.t.
+    hidden_shard and value_weight (only where required).
+    tp_group / cp_group resolve as in megatron_response_logprobs_entropy.  Collectives: forward, under SP one
+    all-gather of [Rmax_k] fp32 values over TP, and one all-gather of [Rmax_c, 2] fp32 over CP; backward none.  Under
+    SP a rank's dX comes from its own rows and its d value_weight is its share, which Megatron sums over TP (the weight
+    carries sequence_parallel); without SP every TP rank computes the full, identical d value_weight.  Other CP ranks'
+    cells arrive detached, as in postprocess_packed_seqs.  No response row on any rank: zeros and no collective.
+    Host syncs: none with host lengths; one device-to-host copy of the counts and the plan's verdict with device
+    lengths."""
+    from .response_rows import MegatronParallelPlan
+
+    what = "megatron_response_values"
+    if not isinstance(plan, MegatronParallelPlan):
+        raise ValueError(f"{what}: plan must be a response_rows.megatron_parallel plan, got {type(plan).__name__}")
+    if hidden_shard.dim() not in (2, 3) or (hidden_shard.dim() == 3 and hidden_shard.shape[1] != 1):
+        raise ValueError(f"{what}: hidden_shard must be [rows, H] or [rows, 1, H], got {tuple(hidden_shard.shape)}")
+    _value_head_check(hidden_shard, value_weight, what)
+    tp_group, tp, k = _mp_group(tp_group, "tp", plan.tp_size, what)
+    cp_group, cp, c = _mp_group(cp_group, "cp", plan.cp_size, what)
+    if not (hidden_shard.is_cuda and value_weight.is_cuda):
+        raise L.Rb200Error("rlinf_b200 kernels take CUDA tensors; move inputs with to_device() first")
+    rows = hidden_shard.shape[0]
+    no_targets = torch.zeros((plan.bsz, plan.response_len), dtype=torch.int64, device=hidden_shard.device)
+    idx = plan.index(no_targets, rows, k, c)
+    shape = (plan.bsz, plan.response_len)
+    if all(sum(r) == 0 for r in idx.counts):  # no response row on any rank: no collective on any rank
+        return torch.zeros(shape, dtype=torch.float32, device=hidden_shard.device)
+    return _MegatronResponseValues.apply(hidden_shard, value_weight, idx, tp_group, cp_group, shape)
+
+
+def _critic_rows(t, name, shape, dev, dtype):
+    if t is None or tuple(t.shape) != shape:
+        raise ValueError(f"token_critic_loss: {name} has shape {None if t is None else tuple(t.shape)}, expected "
+                         f"{shape} (that of values)")
+    if t.dtype != dtype:
+        raise ValueError(f"token_critic_loss: {name} must be {dtype}, got {t.dtype}")
+    if t.device != dev:
+        raise ValueError(f"token_critic_loss: {name} is on {t.device}, values on {dev}")
+    if t.stride(1) != 1 or t.stride(0) < shape[1]:
+        t = t.contiguous()
+    return t
+
+
+def _token_critic_launch(v, ins, value_clip, huber_delta, want_d):
+    lib = L.load()
+    dev = v.device
+    bsz, Ln = v.shape
+    a = L.TokenCriticLossArgs()
+    a.bsz, a.L = bsz, Ln
+    for name, t in (("values", v), *ins.items()):
+        setattr(a, name, C.c_void_p(t.data_ptr()))
+        setattr(a, name + "_stride", t.stride(0))
+    a.value_clip, a.huber_delta = float(value_clip), float(huber_delta)
+    wsb = lib.rb200_token_loss_workspace_bytes(bsz, Ln)
+    if wsb < 0:
+        raise ValueError(f"token_critic_loss: unsupported shape bsz={bsz} L={Ln} (bsz <= 65535)")
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+    loss = torch.empty(1, dtype=torch.float32, device=dev)
+    metrics = torch.empty(L.CM_NUM, dtype=torch.float32, device=dev)
+    d_v = torch.empty((bsz, Ln), dtype=torch.float32, device=dev) if want_d else None
+    a.workspace, a.workspace_bytes = L.ptr(ws), wsb
+    a.loss, a.metrics, a.d_values = L.ptr(loss), L.ptr(metrics), L.ptr(d_v)
+    L.check(lib.rb200_token_critic_loss(C.byref(a), L.stream_ptr(dev)), "token_critic_loss")
+    return loss.reshape(()), metrics, d_v
+
+
+class _TokenCriticLoss(torch.autograd.Function):
+    """forward: one launch group writes the loss, the metrics and d values; backward: d values times the upstream
+    scalar, read on the device."""
+
+    @staticmethod
+    def forward(ctx, values, ins, value_clip, huber_delta):
+        loss, metrics, d_v = _token_critic_launch(values.detach(), ins, value_clip, huber_delta, True)
+        ctx.grad = d_v
+        ctx.mark_non_differentiable(metrics)
+        return loss, metrics
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_metrics):
+        d_v, ctx.grad = ctx.grad, None
+        return scale_by_(d_v, g_loss), None, None, None
+
+
+def token_critic_loss(values, returns, prev_values, loss_mask, *, value_clip: float, huber_delta: float = 10000.0):
+    """Token-level PPO critic loss of the reasoning critic, in one device pass: compute_ppo_critic_loss as
+    MegatronCritic's loss_func calls it.  values, returns, prev_values (fp32) and loss_mask (bool / uint8) are
+    [bsz, L] CUDA tensors; slices whose tokens are contiguous are read in place.  The aggregation is masked_mean, as
+    in the reference whatever the worker's loss_agg_func (an all-masked batch gives 0).
+    Returns (loss, metrics): loss as a 0-dim tensor, differentiable w.r.t. values; metrics maps critic/value_loss,
+    critic/value_clip_ratio (unmasked mean over all cells), the five __sum__/_critic_explained_variance/* sums (masked
+    cells) and critic/final_value_loss to 0-dim device tensors.  Four launches, no host sync."""
+    if values.dim() != 2:
+        raise ValueError(f"token_critic_loss: values must be [bsz, L], got {tuple(values.shape)}")
+    shape, dev = tuple(values.shape), values.device
+    if 0 in shape:
+        raise ValueError(f"token_critic_loss: empty values {shape}")
+    if loss_mask is not None and loss_mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"token_critic_loss: loss_mask must be bool or uint8, got {loss_mask.dtype}")
+    if value_clip is None:
+        raise ValueError("token_critic_loss: value_clip is required")
+    v = _critic_rows(values, "values", shape, dev, torch.float32)
+    ins = {"returns": _critic_rows(returns, "returns", shape, dev, torch.float32),
+           "prev_values": _critic_rows(prev_values, "prev_values", shape, dev, torch.float32),
+           "loss_mask": _critic_rows(L.as_u8(loss_mask), "loss_mask", shape, dev, torch.uint8)}
+    if not values.is_cuda:
+        raise L.Rb200Error("token_critic_loss takes CUDA tensors; there is no CPU path")
+    if torch.is_grad_enabled() and values.requires_grad:
+        loss, metrics = _TokenCriticLoss.apply(v, ins, value_clip, huber_delta)
+    else:
+        loss, metrics, _ = _token_critic_launch(v, ins, value_clip, huber_delta, False)
+    return loss, {k: metrics[s] for s, k in L.CM_KEYS.items()}
