@@ -347,6 +347,109 @@ typedef struct rb200_token_critic_loss_args {
 int rb200_token_critic_loss(const rb200_token_critic_loss_args* args, rb200_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Reasoning step bookkeeping (csrc/reasoning_stats.cu): the reasoning rollout metrics (rlinf/utils/distributed.py
+ *   compute_rollout_metrics / compute_rollout_metrics_dynamic) and the tail of the Megatron workers' loss_func and
+ *   _process_fwd_bwd_outputs, on the device.  No floating-point atomics; partials go to fixed slots and are added in a
+ *   fixed order, so two identical calls give the same bits.
+ *
+ * rb200_reasoning_rollout_record: one rank's fixed-layout fp64 record [RB200_RR_NUM] (RB200_RR_*) from
+ *   advantages [bsz, L] fp32 and the response mask [bsz, L] (uint8 / bool), both read through row strides (elements,
+ *   >= L), optional values [bsz, L] fp32, and [bsz] prompt / response lengths (int64), rewards (fp32) and is_end
+ *   (uint8); idx_to_traj [bsz] (int64) or NULL selects the multi-turn fields.  The SUM fields are rounded to fp32 as
+ *   the reference rounds its reduction vector.  Two launches.  workspace: rb200_reasoning_record_workspace_bytes.
+ * rb200_reasoning_rollout_finish: P records, gathered in rank order ([P, RB200_RR_NUM] fp64), -> the metric vector
+ *   [RB200_RM_NUM + P] fp64 (RB200_RM_*, then each record's num_seq) with the reference's fp32 reduction and fp64
+ *   host arithmetic.  values_world_sum:
+ *   NULL = the values mean is averaged over the P records; else a device fp32 sum over the default group of
+ *   world_size ranks' RB200_RR_VALUES_MEAN.  One launch.
+ * ---------------------------------------------------------------------------------------- */
+enum {
+  RB200_RR_SUM_PLEN = 0, RB200_RR_SUM_RLEN = 1, RB200_RR_SUM_REWARDS = 2, RB200_RR_SUM_END = 3,
+  RB200_RR_SUM_ADV = 4, RB200_RR_NUM_SEQ = 5, RB200_RR_N_VALID = 6, RB200_RR_SUM_TRAJ_REWARDS = 7,
+  RB200_RR_NUM_TRAJ = 8,       /* 0-8: fp32-rounded SUM fields */
+  RB200_RR_ADV_NEG_MIN = 9, RB200_RR_ADV_MAX = 10, RB200_RR_MAX_PLEN = 11, RB200_RR_MAX_RLEN = 12,
+  RB200_RR_MAX_TOTAL = 13, RB200_RR_VAL_NEG_MIN = 14, RB200_RR_VAL_MAX = 15,  /* 9-15: fp32 MAX fields */
+  RB200_RR_VALUES_MEAN = 16,   /* fp32 masked mean of this rank's values */
+  RB200_RR_RLEN_SUM = 17, RB200_RR_RLEN_SQ_SUM = 18, RB200_RR_RLEN_MIN = 19, RB200_RR_RLEN_MAX = 20,  /* exact */
+  RB200_RR_VERDICT = 21,       /* RB200_RV_* bits */
+  RB200_RR_NUM = 24
+};
+enum { RB200_RV_EMPTY = 1, RB200_RV_BAD_TRAJ = 2 };  /* no valid advantage; idx_to_traj entry < 0 */
+enum {
+  RB200_RM_NUM_SEQ = 0, RB200_RM_PROMPT_LENGTH, RB200_RM_RESPONSE_LENGTH, RB200_RM_AVG_RESPONSE_LENGTH,
+  RB200_RM_VAR_RESPONSE_LENGTH, RB200_RM_MAX_OF_RESPONSE_LENGTH, RB200_RM_MIN_OF_RESPONSE_LENGTH,
+  RB200_RM_TOTAL_LENGTH, RB200_RM_REWARD_SCORES, RB200_RM_PROPERLY_ENDED, RB200_RM_ADV_MEAN, RB200_RM_ADV_MAX,
+  RB200_RM_ADV_MIN, RB200_RM_VALUES_MEAN, RB200_RM_VALUES_MAX, RB200_RM_VALUES_MIN, RB200_RM_MAX_PROMPT_LENGTH,
+  RB200_RM_MAX_RESPONSE_LENGTH, RB200_RM_MAX_TOTAL_LENGTH, RB200_RM_REWARD_SCORES_TRAJ, RB200_RM_REWARD_SCORES_TURN,
+  RB200_RM_AVG_TURNS_PER_TRAJ, RB200_RM_VERDICT, RB200_RM_NUM_LENGTHS_MAX,  /* largest num_seq of a record */
+  RB200_RM_NUM = 24
+};
+typedef struct rb200_reasoning_record_args {
+  int64_t bsz, L;
+  const float* advantages;    int64_t advantages_stride;
+  const uint8_t* mask;        int64_t mask_stride;
+  const float* values;        int64_t values_stride;  /* NULL: no values fields */
+  const int64_t* prompt_lengths;
+  const int64_t* response_lengths;
+  const float* rewards;
+  const uint8_t* is_end;
+  const int64_t* idx_to_traj;  /* NULL: single-turn batch */
+  void* workspace;
+  int64_t workspace_bytes;
+  double* record;              /* [RB200_RR_NUM] */
+} rb200_reasoning_record_args;
+int64_t rb200_reasoning_record_workspace_bytes(int64_t bsz, int64_t L);
+int rb200_reasoning_rollout_record(const rb200_reasoning_record_args* args, rb200_stream_t stream);
+int rb200_reasoning_rollout_finish(const double* records, int32_t P, const float* values_world_sum,
+                                   int32_t world_size, double* metrics, rb200_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Megatron loss_func epilogue, one micro-batch (megatron_actor_worker.py:258-307, megatron_critic_worker.py:104-121),
+ *   in two launches around ONE data-parallel SUM all-reduce of `pack` that the caller makes:
+ * rb200_mb_epilogue_pack: pack[k] = *src[k] for the n_avg averaged keys then the n_sum SUM keys (the explained-
+ *   variance sums); pack[final_slot] = loss s and pack[n_avg + n_sum] = (loss 0) s, where the scale
+ *   s = fp32(fp32(fp32(mask_sum / global_valid_token) dp) num_microbatches) when global_valid_token is given, else 1;
+ *   s goes to scale[0].  With global_valid_token the mask is counted (two more launches; workspace
+ *   rb200_token_loss_workspace_bytes(bsz, L) bytes), else workspace needs RB200_EPI_WS_MIN bytes.
+ * rb200_mb_epilogue_apply (after the all-reduce): averaged keys = pack / dp (Megatron's average), SUM keys = pack;
+ *   early stop when has_early_stop and pack[ratio_slot] / dp > early_stop_imp_ratio (fp32 compare), in which case
+ *   scale[0] = 0 and the final loss is the stopped variant; metrics [n_avg + n_sum] and row mb of step_acc
+ *   [n_mb, n_avg + n_sum] get the reduced values.  One launch.
+ * rb200_step_metrics_finish: _process_fwd_bwd_outputs (megatron_worker.py:550-599) for a training step: out[k] = the
+ *   fp32 mean over the n_mb rows in index order for k < n_avg, the fp32 sum for the n_sum keys, and when n_sum == 5
+ *   out[n_avg + 5] = compute_critic_explained_variance_from_stats in fp32 (NaN for count < 2 or a zero / NaN centred
+ *   returns sum or a NaN centred errors sum).  One launch.
+ * ---------------------------------------------------------------------------------------- */
+#define RB200_EPI_MAX_KEYS 24
+#define RB200_EPI_WS_MIN 64
+typedef struct rb200_mb_epilogue_args {
+  int32_t n_avg, n_sum;
+  int32_t final_slot, ratio_slot;          /* indices among the averaged keys, -1 = none */
+  const float* src[RB200_EPI_MAX_KEYS];    /* 0-dim fp32 device metrics: averaged keys, then the SUM keys */
+  const float* loss;                       /* the unscaled loss, fp32 [1] */
+  const uint8_t* mask;  int64_t mask_stride;  int64_t bsz, L;
+  const float* global_valid_token;         /* fp32 [1] or NULL (no valid-token scale) */
+  int32_t dp, num_microbatches;
+  int32_t has_early_stop, mb;
+  double early_stop_imp_ratio;
+  void* workspace;
+  int64_t workspace_bytes;
+  float* pack;       /* [n_avg + n_sum + 1] */
+  float* scale;      /* [1] */
+  float* metrics;    /* [n_avg + n_sum] */
+  float* step_acc;   /* [n_mb, n_avg + n_sum] */
+  int32_t n_mb, reserved;
+} rb200_mb_epilogue_args;
+/* mask.to(float32).sum() of _setup_valid_token_scale (megatron_worker.py:640-654): out[0] = the mask count rounded
+ * once to fp32.  workspace: rb200_token_loss_workspace_bytes(bsz, L) bytes.  Three launches. */
+int rb200_mask_count_f32(const uint8_t* mask, int64_t mask_stride, int64_t bsz, int64_t L, void* workspace,
+                         int64_t workspace_bytes, float* out, rb200_stream_t stream);
+int rb200_mb_epilogue_pack(const rb200_mb_epilogue_args* args, rb200_stream_t stream);
+int rb200_mb_epilogue_apply(const rb200_mb_epilogue_args* args, rb200_stream_t stream);
+int rb200_step_metrics_finish(const float* step_acc, int32_t n_mb, int32_t n_avg, int32_t n_sum, float* out,
+                              rb200_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Value head of the reasoning critic on a plan's rows (csrc/value_head.cu): the reference's LinearForLastLayer(H, 1)
  *   (a bf16 nn.Linear without bias, output cast with .float()) evaluated in place on rows of a hidden shard x
  *   (bf16, unit inner stride, row_stride elements between rows, a multiple of 8; 16-byte aligned), w [1, H] bf16.

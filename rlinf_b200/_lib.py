@@ -134,6 +134,41 @@ class TokenCriticLossArgs(C.Structure):
          ("loss", c_void_p), ("metrics", c_void_p), ("d_values", c_void_p)]
 
 
+# reasoning step bookkeeping (mirror of RB200_RR_* / RB200_RM_* / rb200_reasoning_record_args /
+# rb200_mb_epilogue_args)
+RR_NUM = 24
+RM_NUM = 24
+RM_SLOTS = {
+    "total_num_sequence": 0, "prompt_length": 1, "response_length": 2, "average_response_length": 3,
+    "variance_of_response_length": 4, "max_of_response_length": 5, "min_of_response_length": 6, "total_length": 7,
+    "reward_scores": 8, "fraction_of_samples_properly_ended": 9, "advantages_mean": 10, "advantages_max": 11,
+    "advantages_min": 12, "values_mean": 13, "values_max": 14, "values_min": 15, "max_prompt_length": 16,
+    "max_response_length": 17, "max_total_length": 18, "reward_scores_traj": 19, "reward_scores_turn": 20,
+    "avg_turns_per_traj": 21,
+}
+RM_VERDICT, RM_NUM_LENGTHS_MAX = 22, 23
+RR_VALUES_MEAN = 16
+RV_EMPTY, RV_BAD_TRAJ = 1, 2
+EPI_MAX_KEYS = 24
+EPI_WS_MIN = 64
+
+
+class ReasoningRecordArgs(C.Structure):
+    _fields_ = [("bsz", c_int64), ("L", c_int64)] + [
+        f for name in ("advantages", "mask", "values") for f in ((name, c_void_p), (name + "_stride", c_int64))
+    ] + [(n, c_void_p) for n in ("prompt_lengths", "response_lengths", "rewards", "is_end", "idx_to_traj",
+                                 "workspace")] + [("workspace_bytes", c_int64), ("record", c_void_p)]
+
+
+class MbEpilogueArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_avg", "n_sum", "final_slot", "ratio_slot")] + [
+        ("src", c_void_p * EPI_MAX_KEYS), ("loss", c_void_p), ("mask", c_void_p), ("mask_stride", c_int64),
+        ("bsz", c_int64), ("L", c_int64), ("global_valid_token", c_void_p)] + [
+        (n, C.c_int32) for n in ("dp", "num_microbatches", "has_early_stop", "mb")] + [
+        ("early_stop_imp_ratio", c_double), ("workspace", c_void_p), ("workspace_bytes", c_int64)] + [
+        (n, c_void_p) for n in ("pack", "scale", "metrics", "step_acc")] + [("n_mb", C.c_int32), ("reserved", C.c_int32)]
+
+
 class MlpLayout(C.Structure):
     _fields_ = [
         ("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("value_dim", C.c_int32), ("hidden", C.c_int32),
@@ -217,6 +252,13 @@ SIGNATURES = {
                                     + [c_void_p] * 9 + [c_void_p]),
     "rb200_response_rows_mp_pack_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "rb200_token_critic_loss": (c_int, [C.POINTER(TokenCriticLossArgs), c_void_p]),
+    "rb200_reasoning_record_workspace_bytes": (c_int64, [c_int64, c_int64]),
+    "rb200_reasoning_rollout_record": (c_int, [C.POINTER(ReasoningRecordArgs), c_void_p]),
+    "rb200_reasoning_rollout_finish": (c_int, [c_void_p, C.c_int32, c_void_p, C.c_int32, c_void_p, c_void_p]),
+    "rb200_mask_count_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
+    "rb200_mb_epilogue_pack": (c_int, [C.POINTER(MbEpilogueArgs), c_void_p]),
+    "rb200_mb_epilogue_apply": (c_int, [C.POINTER(MbEpilogueArgs), c_void_p]),
+    "rb200_step_metrics_finish": (c_int, [c_void_p, C.c_int32, C.c_int32, C.c_int32, c_void_p, c_void_p]),
     "rb200_value_head_workspace_bytes": (c_int64, [c_int64, c_int64]),
     "rb200_value_head_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "rb200_value_head_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p,

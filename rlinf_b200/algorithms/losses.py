@@ -379,8 +379,9 @@ def reasoning_actor_loss(logprobs, advantages, loss_mask, *, old_logprobs=None, 
     actor/rollout_train_kl (compute_rollout_train_kl, fsdp_actor_worker.py:75-93).
 
     Returns (loss, metrics): loss before 1/gradient_accumulation (and before Megatron's early-stop and valid-token
-    scales, which stay with the caller), differentiable w.r.t. logprobs and entropy; metrics are 0-dim device tensors
-    under the workers' keys, actor/final_loss, actor/entropy_loss and actor/kl_loss included.  No host sync."""
+    scales: algorithms.MegatronLossEpilogue applies them and the data-parallel metric average on the device),
+    differentiable w.r.t. logprobs and entropy; metrics are 0-dim device tensors under the workers' keys,
+    actor/final_loss, actor/entropy_loss and actor/kl_loss included.  No host sync."""
     if old_logprobs is None:
         old_logprobs = recomputed_logprobs if recomputed_logprobs is not None else rollout_logprobs
     if old_logprobs is None:
@@ -405,7 +406,8 @@ def reasoning_critic_loss(values, returns, prev_values, loss_mask, *, value_clip
 
     Returns (loss, metrics): loss differentiable w.r.t. values; metrics are 0-dim device tensors under the worker's keys
     (critic/value_loss, critic/value_clip_ratio, the five __sum__/_critic_explained_variance/* sums and
-    critic/final_value_loss), before Megatron's data-parallel reductions, which stay with the caller.  No host sync."""
+    critic/final_value_loss), before Megatron's data-parallel reductions (algorithms.MegatronLossEpilogue("critic")
+    makes them in one all-reduce, and algorithms.step_metrics finishes the explained variance).  No host sync."""
     return ops.token_critic_loss(values, returns, prev_values, loss_mask, value_clip=value_clip,
                                  huber_delta=huber_delta)
 

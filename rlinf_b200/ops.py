@@ -1582,3 +1582,121 @@ def token_critic_loss(values, returns, prev_values, loss_mask, *, value_clip: fl
     else:
         loss, metrics, _ = _token_critic_launch(v, ins, value_clip, huber_delta, False)
     return loss, {k: metrics[s] for s, k in L.CM_KEYS.items()}
+
+
+# ---- reasoning step bookkeeping (csrc/reasoning_stats.cu) ----------------------------------------------------------
+
+def _cells(t, name, shape, dev, dtype):
+    """A [bsz, L] operand read in place through its row stride when its tokens are contiguous."""
+    if tuple(t.shape) != shape:
+        raise ValueError(f"reasoning rollout metrics: {name} has shape {tuple(t.shape)}, expected {shape}")
+    t = L.to_device(t, dev) if t.device != dev else t
+    if t.dtype != dtype:
+        t = t.to(dtype)
+    if t.stride(1) != 1 or t.stride(0) < shape[1]:
+        t = t.contiguous()
+    return t
+
+
+def _per_seq(t, name, bsz, dev, dtype):
+    t = t.reshape(-1)
+    if t.numel() != bsz:
+        raise ValueError(f"reasoning rollout metrics: {name} has {t.numel()} entries, expected {bsz}")
+    return L.to_device(t, dev, dtype)
+
+
+def reasoning_rollout_record(advantages, response_mask, prompt_lengths, response_lengths, rewards, is_end, *,
+                             values=None, idx_to_traj=None) -> torch.Tensor:
+    """This rank's fixed-layout record, float64 [RR_NUM] on the device, for compute_rollout_metrics(_dynamic):
+    advantages / response_mask / values are [bsz, L] (the mask read in place, e.g. response_mask[:, -L:]),
+    prompt / response lengths, rewards and is_end [bsz]; idx_to_traj [bsz] (list or tensor) selects the multi-turn
+    fields.  Two launches, no host sync."""
+    if advantages.dim() != 2 or 0 in advantages.shape:
+        raise ValueError(f"reasoning rollout metrics: advantages must be a non-empty [bsz, L], got "
+                         f"{tuple(advantages.shape)}")
+    dev = advantages.device if advantages.is_cuda else L.default_device()
+    shape = tuple(advantages.shape)
+    bsz, Ln = shape
+    adv = _cells(advantages, "advantages", shape, dev, torch.float32)
+    mask = _cells(L.as_u8(response_mask), "response_mask", shape, dev, torch.uint8)
+    val = None if values is None else _cells(values, "values", shape, dev, torch.float32)
+    a = L.ReasoningRecordArgs()
+    a.bsz, a.L = bsz, Ln
+    keep = [adv, mask, val]
+    for name, t in (("advantages", adv), ("mask", mask), ("values", val)):
+        setattr(a, name, None if t is None else C.c_void_p(t.data_ptr()))
+        setattr(a, name + "_stride", 0 if t is None else t.stride(0))
+    seq = {"prompt_lengths": _per_seq(prompt_lengths, "prompt_lengths", bsz, dev, torch.int64),
+           "response_lengths": _per_seq(response_lengths, "response_lengths", bsz, dev, torch.int64),
+           "rewards": _per_seq(rewards, "rewards", bsz, dev, torch.float32),
+           "is_end": _per_seq(L.as_u8(torch.as_tensor(is_end)), "is_end", bsz, dev, torch.uint8)}
+    if idx_to_traj is not None:
+        seq["idx_to_traj"] = _per_seq(torch.as_tensor(idx_to_traj, dtype=torch.int64), "idx_to_traj", bsz, dev,
+                                      torch.int64)
+    for name, t in seq.items():
+        setattr(a, name, L.ptr(t))
+    keep.append(seq)
+    lib = L.load()
+    wsb = lib.rb200_reasoning_record_workspace_bytes(bsz, Ln)
+    if wsb < 0:
+        raise ValueError(f"reasoning rollout metrics: unsupported shape bsz={bsz} L={Ln} (bsz <= 65535)")
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+    rec = torch.empty(L.RR_NUM, dtype=torch.float64, device=dev)
+    a.workspace, a.workspace_bytes, a.record = L.ptr(ws), wsb, L.ptr(rec)
+    L.check(lib.rb200_reasoning_rollout_record(C.byref(a), L.stream_ptr(dev)), "reasoning_rollout_record")
+    return rec
+
+
+def reasoning_rollout_finish(records: torch.Tensor, values_world_sum: Optional[torch.Tensor] = None,
+                             world_size: int = 0) -> torch.Tensor:
+    """[P, RR_NUM] records in rank order -> float64 [RM_NUM + P]: the metric slots (L.RM_SLOTS), the verdict, the
+    largest num_seq, then each rank's num_seq.  values_world_sum: fp32 [1] sum of RR_VALUES_MEAN over the default
+    group of world_size ranks (None: the values mean is averaged over the P records).  One launch."""
+    if records.dim() != 2 or records.shape[1] != L.RR_NUM or records.dtype != torch.float64:
+        raise ValueError(f"reasoning_rollout_finish: records must be float64 [P, {L.RR_NUM}]")
+    records = records.contiguous()
+    P = records.shape[0]
+    out = torch.empty(L.RM_NUM + P, dtype=torch.float64, device=records.device)
+    ws = None if values_world_sum is None else values_world_sum.contiguous()
+    L.check(L.load().rb200_reasoning_rollout_finish(L.ptr(records), P, L.ptr(ws), int(world_size), L.ptr(out),
+                                                    L.stream_ptr(records.device)), "reasoning_rollout_finish")
+    return out
+
+
+def mask_count_f32(mask: torch.Tensor) -> torch.Tensor:
+    """mask.to(float32).sum() as a 0-dim fp32 device tensor (the exact count rounded once); mask [bsz, L] bool /
+    uint8, read in place when its tokens are contiguous.  Three launches, no host sync."""
+    if mask.dim() != 2 or 0 in mask.shape:
+        raise ValueError(f"mask_count_f32: mask must be a non-empty [bsz, L], got {tuple(mask.shape)}")
+    dev = mask.device if mask.is_cuda else L.default_device()
+    m = _cells(L.as_u8(mask), "mask", tuple(mask.shape), dev, torch.uint8)
+    lib = L.load()
+    wsb = lib.rb200_token_loss_workspace_bytes(*m.shape)
+    if wsb < 0:
+        raise ValueError(f"mask_count_f32: unsupported shape {tuple(m.shape)} (bsz <= 65535)")
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+    out = torch.empty(1, dtype=torch.float32, device=dev)
+    L.check(lib.rb200_mask_count_f32(L.ptr(m) if m.is_contiguous() else C.c_void_p(m.data_ptr()), m.stride(0),
+                                     m.shape[0], m.shape[1], L.ptr(ws), wsb, L.ptr(out), L.stream_ptr(dev)),
+            "mask_count_f32")
+    return out.reshape(())
+
+
+def mb_epilogue_pack(args, stream_dev) -> None:
+    """rb200_mb_epilogue_pack on a filled L.MbEpilogueArgs (see algorithms.MegatronLossEpilogue)."""
+    L.check(L.load().rb200_mb_epilogue_pack(C.byref(args), L.stream_ptr(stream_dev)), "mb_epilogue_pack")
+
+
+def mb_epilogue_apply(args, stream_dev) -> None:
+    L.check(L.load().rb200_mb_epilogue_apply(C.byref(args), L.stream_ptr(stream_dev)), "mb_epilogue_apply")
+
+
+def step_metrics_finish(step_acc: torch.Tensor, n_avg: int, n_sum: int) -> torch.Tensor:
+    """[n_mb, n_avg + n_sum] fp32 per-micro-batch metrics -> fp32 [n_avg + n_sum + 1]: means over micro-batches in
+    index order, sums of the SUM keys, and (n_sum == 5) the explained variance.  One launch."""
+    if step_acc.dim() != 2 or step_acc.shape[1] != n_avg + n_sum or step_acc.dtype != torch.float32:
+        raise ValueError("step_metrics_finish: step_acc must be fp32 [n_mb, n_avg + n_sum]")
+    out = torch.empty(n_avg + n_sum + 1, dtype=torch.float32, device=step_acc.device)
+    L.check(L.load().rb200_step_metrics_finish(L.ptr(step_acc.contiguous()), step_acc.shape[0], n_avg, n_sum,
+                                               L.ptr(out), L.stream_ptr(step_acc.device)), "step_metrics_finish")
+    return out
