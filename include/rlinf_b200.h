@@ -693,6 +693,24 @@ int rb200_logits_logprob_entropy_bwd(const void* logits, int dtype, const int64_
                                      const float* grad_logprob, const float* grad_entropy, void* dlogits,
                                      int64_t d_batch_stride, int64_t d_row_stride, rb200_stream_t stream);
 
+/* The same with top-k filtering over the whole row [0, V) first (csrc/topk.cu), as the OpenVLA action head does with
+ * rollout.sampling_params.top_k > 0 (TopKLogitsWarper, openvla_oft_action_model.py:532-559): threshold[r] (fp32, the
+ * unscaled logit) = the top_k-th largest logit of row r counted with multiplicity; column i is kept iff
+ * v_lo <= i < v_hi and logit_i >= threshold[r] (ties at the k-th value are all kept).  Outputs as above over the kept
+ * columns; a target that is not kept has logprob -inf; a row without a kept column has logprob NaN, entropy -0.0 and
+ * lse -inf.  The backward reads threshold and writes dlogits = 0 at every column that is not kept.
+ * 1 <= top_k < V, else RB200_E_ARG; threshold is required. */
+int rb200_logits_topk_logprob_entropy_fwd(const void* logits, int dtype, const int64_t* target, int64_t N, int64_t L,
+                                          int64_t batch_stride, int64_t row_stride, int V, int v_lo, int v_hi,
+                                          double inv_temperature, int top_k, float* logprob, float* entropy, float* lse,
+                                          float* threshold, rb200_stream_t stream);
+int rb200_logits_topk_logprob_entropy_bwd(const void* logits, int dtype, const int64_t* target, int64_t N, int64_t L,
+                                          int64_t batch_stride, int64_t row_stride, int V, int v_lo, int v_hi,
+                                          double inv_temperature, const float* threshold, const float* lse,
+                                          const float* entropy, const float* grad_logprob, const float* grad_entropy,
+                                          void* dlogits, int64_t d_batch_stride, int64_t d_row_stride,
+                                          rb200_stream_t stream);
+
 /* The same log-probabilities and entropies fused into the LM-head GEMM (csrc/lmhead.cu): z = (X . W^T) * inv_T from
  * the last hidden states X (bf16, row r at hidden + (r / L) * batch_stride + (r % L) * row_stride, strides multiples of
  * 8 elements) and the LM-head weight W [V, H] (bf16 row-major, no bias), H % 64 == 0, 64 <= H <= 8192; the logits are
@@ -713,6 +731,27 @@ int rb200_lmhead_logprob_entropy_bwd(const void* hidden, const void* weight, con
                                      double inv_temperature, const float* lse, const float* entropy,
                                      const float* grad_logprob, const float* grad_entropy, void* d_hidden,
                                      void* d_weight, void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
+
+/* The top-k filtered form of the fused head (csrc/lmhead_topk.cu; semantics of rb200_logits_topk_*): the threshold is
+ * the top_k-th largest fp32 accumulator X.W^T of the row over the whole vocabulary [0, V), before the temperature.
+ * The forward runs in blocks of whole 128-row tiles, as many as workspace_bytes holds of an fp32 [rows, V] block
+ * (RB200_E_ARG below one tile); rb200_lmhead_topk_workspace_bytes() returns what a block of row_block rows (<= 0: a
+ * 512 MiB budget) and a backward with vocabulary chunks of vocab_chunk columns need, or -1 for an unsupported shape.
+ * The backward reads threshold and derives its chunk from workspace_bytes as rb200_lmhead_logprob_entropy_bwd does.
+ * 1 <= top_k < V, else RB200_E_ARG; threshold is required. */
+int64_t rb200_lmhead_topk_workspace_bytes(int64_t N, int64_t L, int H, int V, int v_lo, int v_hi, int64_t row_block,
+                                          int64_t vocab_chunk);
+int rb200_lmhead_topk_logprob_entropy_fwd(const void* hidden, const void* weight, const int64_t* target, int64_t N,
+                                          int64_t L, int64_t batch_stride, int64_t row_stride, int H, int V, int v_lo,
+                                          int v_hi, double inv_temperature, int top_k, float* logprob, float* entropy,
+                                          float* lse, float* threshold, void* workspace, int64_t workspace_bytes,
+                                          rb200_stream_t stream);
+int rb200_lmhead_topk_logprob_entropy_bwd(const void* hidden, const void* weight, const int64_t* target, int64_t N,
+                                          int64_t L, int64_t batch_stride, int64_t row_stride, int H, int V, int v_lo,
+                                          int v_hi, double inv_temperature, const float* threshold, const float* lse,
+                                          const float* entropy, const float* grad_logprob, const float* grad_entropy,
+                                          void* d_hidden, void* d_weight, void* workspace, int64_t workspace_bytes,
+                                          rb200_stream_t stream);
 
 /* Vocabulary-parallel (tensor-parallel) variants of the two ops above (csrc/vocab_parallel.cu, lmhead.cu, logits.cu).
  * Equal shards (Megatron's VocabUtility; the vocabulary is padded so that P divides it): rank k of P owns the global

@@ -231,11 +231,23 @@ SIGNATURES = {
                                                  c_int, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "rb200_logits_logprob_entropy_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                                  c_int, c_int, c_double] + [c_void_p] * 5 + [c_int64, c_int64, c_void_p]),
+    "rb200_logits_topk_logprob_entropy_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                                      c_int, c_int, c_int, c_double, c_int] + [c_void_p] * 5),
+    "rb200_logits_topk_logprob_entropy_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                                      c_int, c_int, c_int, c_double] + [c_void_p] * 6
+                                              + [c_int64, c_int64, c_void_p]),
     "rb200_lmhead_workspace_bytes": (c_int64, [c_int64, c_int64, c_int, c_int, c_int, c_int, c_int64]),
     "rb200_lmhead_logprob_entropy_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                                  c_int, c_int, c_int, c_double] + [c_void_p] * 4 + [c_int64, c_void_p]),
     "rb200_lmhead_logprob_entropy_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                                  c_int, c_int, c_int, c_double] + [c_void_p] * 7 + [c_int64, c_void_p]),
+    "rb200_lmhead_topk_workspace_bytes": (c_int64, [c_int64, c_int64, c_int, c_int, c_int, c_int, c_int64, c_int64]),
+    "rb200_lmhead_topk_logprob_entropy_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                                      c_int, c_int, c_int, c_int, c_double, c_int] + [c_void_p] * 5
+                                              + [c_int64, c_void_p]),
+    "rb200_lmhead_topk_logprob_entropy_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                                      c_int, c_int, c_int, c_int, c_double] + [c_void_p] * 8
+                                              + [c_int64, c_void_p]),
     "rb200_lmhead_vp_workspace_bytes": (c_int64, [c_int64, c_int64, c_int, c_int, c_int64, c_int, c_int, c_int64]),
     "rb200_lmhead_vp_partials_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                              c_int, c_int64, c_int, c_int, c_double, c_void_p, c_void_p, c_int64,

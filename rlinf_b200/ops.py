@@ -6,6 +6,7 @@ outputs (torch.empty) and translate pointers.  Inputs on the host are copied to 
 from __future__ import annotations
 
 import ctypes as C
+import operator
 from typing import Optional
 
 import torch
@@ -569,7 +570,7 @@ def _raw_ptr(t: torch.Tensor):
 
 class _LogitsLogprobEntropy(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, logits, target, temperature, window, want_entropy):
+    def forward(ctx, logits, target, temperature, window, want_entropy, top_k=0):
         lib = L.load()
         if logits.dtype not in (torch.float32, torch.bfloat16):
             raise ValueError(f"logits must be float32 or bfloat16, got {logits.dtype}")
@@ -582,10 +583,19 @@ class _LogitsLogprobEntropy(torch.autograd.Function):
         ent = torch.empty(N, dtype=torch.float32, device=x.device) if want_entropy else None
         lse = torch.empty(N, dtype=torch.float32, device=x.device)
         dt = 0 if x.dtype == torch.float32 else 1
-        L.check(lib.rb200_logits_logprob_entropy_fwd(_raw_ptr(x), dt, L.ptr(tgt), N, Lr, bs, rs, V, lo, hi,
-                                                     1.0 / float(temperature), L.ptr(lp), L.ptr(ent), L.ptr(lse),
-                                                     L.stream_ptr(x.device)), "logits_logprob_entropy_fwd")
-        ctx.save_for_backward(x, tgt, lse, ent if want_entropy else lse)
+        thr = None
+        if 0 < top_k < V:  # csrc/topk.cu: the k-th largest logit of each row, saved for the backward's mask
+            thr = torch.empty(N, dtype=torch.float32, device=x.device)
+            L.check(lib.rb200_logits_topk_logprob_entropy_fwd(_raw_ptr(x), dt, L.ptr(tgt), N, Lr, bs, rs, V, lo, hi,
+                                                              1.0 / float(temperature), int(top_k), L.ptr(lp),
+                                                              L.ptr(ent), L.ptr(lse), L.ptr(thr),
+                                                              L.stream_ptr(x.device)),
+                    "logits_topk_logprob_entropy_fwd")
+        else:
+            L.check(lib.rb200_logits_logprob_entropy_fwd(_raw_ptr(x), dt, L.ptr(tgt), N, Lr, bs, rs, V, lo, hi,
+                                                         1.0 / float(temperature), L.ptr(lp), L.ptr(ent), L.ptr(lse),
+                                                         L.stream_ptr(x.device)), "logits_logprob_entropy_fwd")
+        ctx.save_for_backward(x, tgt, lse, ent if want_entropy else lse, thr)
         ctx.meta = (N, Lr, bs, rs, V, lo, hi, float(temperature), dt, want_entropy, tuple(logits.shape))
         shape = logits.shape[:-1]
         if want_entropy:
@@ -597,24 +607,49 @@ class _LogitsLogprobEntropy(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_lp, g_ent):
         lib = L.load()
-        x, tgt, lse, ent = ctx.saved_tensors
+        x, tgt, lse, ent, thr = ctx.saved_tensors
         N, Lr, bs, rs, V, lo, hi, temp, dt, want_entropy, shape = ctx.meta
         glp = g_lp.reshape(-1).float().contiguous() if g_lp is not None else None
         gh = g_ent.reshape(-1).float().contiguous() if (want_entropy and g_ent is not None) else None
         dx = torch.empty((N, V), dtype=x.dtype, device=x.device)  # contiguous gradient, whatever the logits' strides
-        L.check(lib.rb200_logits_logprob_entropy_bwd(_raw_ptr(x), dt, L.ptr(tgt), N, Lr, bs, rs, V, lo, hi, 1.0 / temp,
-                                                     L.ptr(lse), L.ptr(ent) if gh is not None else None, L.ptr(glp),
-                                                     L.ptr(gh), L.ptr(dx), Lr * V, V, L.stream_ptr(x.device)),
-                "logits_logprob_entropy_bwd")
-        return dx.view(shape), None, None, None, None
+        if thr is not None:
+            L.check(lib.rb200_logits_topk_logprob_entropy_bwd(_raw_ptr(x), dt, L.ptr(tgt), N, Lr, bs, rs, V, lo, hi,
+                                                              1.0 / temp, L.ptr(thr), L.ptr(lse),
+                                                              L.ptr(ent) if gh is not None else None, L.ptr(glp),
+                                                              L.ptr(gh), L.ptr(dx), Lr * V, V, L.stream_ptr(x.device)),
+                    "logits_topk_logprob_entropy_bwd")
+        else:
+            L.check(lib.rb200_logits_logprob_entropy_bwd(_raw_ptr(x), dt, L.ptr(tgt), N, Lr, bs, rs, V, lo, hi,
+                                                         1.0 / temp, L.ptr(lse), L.ptr(ent) if gh is not None else None,
+                                                         L.ptr(glp), L.ptr(gh), L.ptr(dx), Lr * V, V,
+                                                         L.stream_ptr(x.device)),
+                    "logits_logprob_entropy_bwd")
+        return dx.view(shape), None, None, None, None, None
 
 
-def logprobs_entropy_from_logits(logits, target, temperature: float = 1.0, window=None, compute_entropy: bool = True):
+def _top_k_arg(top_k, V: int) -> int:
+    """top_k as the kernels take it: 0 for no filtering (top_k <= 0 or >= V), else top_k."""
+    try:
+        if isinstance(top_k, bool):
+            raise TypeError
+        top_k = operator.index(top_k)
+    except TypeError:
+        raise ValueError(f"top_k must be an integer, got {top_k!r}") from None
+    return top_k if 0 < top_k < V else 0
+
+
+def logprobs_entropy_from_logits(logits, target, temperature: float = 1.0, window=None, compute_entropy: bool = True,
+                                 top_k: int = 0):
     """compute_logprobs_from_logits + compute_entropy_from_logits (rlinf/utils/utils.py:454-512) of `logits / temperature`
     (fsdp_actor_worker.py:478) restricted to the vocabulary window [lo, hi) (OpenVLA action bins,
     openvla_oft_action_model.py:546-551) in ONE pass over the logits, differentiable w.r.t. the raw logits.
-    Returns (logprobs [...], entropy [...] or None), fp32."""
-    lp, ent = _LogitsLogprobEntropy.apply(logits, target, temperature, window, bool(compute_entropy))
+    top_k > 0 first keeps only the logits >= the row's top_k-th largest over the whole vocabulary, ties included, as
+    the OpenVLA heads' TopKLogitsWarper does before the window (openvla_oft_action_model.py:537-551): targets that are
+    not kept get -inf, rows with no kept column NaN log-prob and -0.0 entropy (csrc/topk.cu).  top_k <= 0 or >= V is
+    the unfiltered op.  Returns (logprobs [...], entropy [...] or None), fp32."""
+    k = _top_k_arg(top_k, logits.shape[-1])
+    args = (logits, target, temperature, window, bool(compute_entropy)) + ((k,) if k else ())
+    lp, ent = _LogitsLogprobEntropy.apply(*args)
     return lp, (ent if compute_entropy else None)
 
 
@@ -636,6 +671,7 @@ def compute_entropy_from_logits(logits, dim: int = -1):
 # The same, fused into the LM-head GEMM: hidden states and lm_head.weight in, no logits tensor (csrc/lmhead.cu)
 # ---------------------------------------------------------------------------------------------------------------
 LMHEAD_DZ_BUDGET = 1 << 30  # bytes of the backward's bf16 dZ chunk [N, Vc]
+LMHEAD_TOPK_ROW_BLOCK = 0  # rows per top-k forward block (whole 128-row tiles); 0 = a 512 MiB fp32 accumulator block
 
 
 def _lmhead_check(hidden: torch.Tensor, weight: torch.Tensor):
@@ -685,7 +721,7 @@ def _lmhead_chunk(N: int, lo: int, hi: int) -> int:
 
 class _LinearLogprobEntropy(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, hidden, weight, target, temperature, window, want_entropy):
+    def forward(ctx, hidden, weight, target, temperature, window, want_entropy, top_k=0):
         _lmhead_check(hidden, weight)
         lib = L.load()
         x, N, Lr, bs, rs = _lmhead_geometry(hidden)
@@ -698,17 +734,30 @@ class _LinearLogprobEntropy(torch.autograd.Function):
         if not 0 <= lo < hi <= V:
             raise ValueError(f"linear_logprobs_entropy: window [{lo}, {hi}) must lie inside [0, {V}) and be non-empty")
         vc = _lmhead_chunk(N, lo, hi)
-        wsb = lmhead_workspace_bytes(N, Lr, H, V, lo, hi, vc)
-        ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
         lp = torch.empty(N, dtype=torch.float32, device=x.device)
         ent = torch.empty(N, dtype=torch.float32, device=x.device) if want_entropy else None
         lse = torch.empty(N, dtype=torch.float32, device=x.device)
-        L.check(lib.rb200_lmhead_logprob_entropy_fwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo, hi,
-                                                     1.0 / float(temperature), L.ptr(lp), L.ptr(ent), L.ptr(lse),
-                                                     L.ptr(ws), wsb, L.stream_ptr(x.device)),
-                "lmhead_logprob_entropy_fwd")
+        thr = None
+        if 0 < top_k < V:  # csrc/lmhead_topk.cu: full-vocabulary accumulator blocks, then the row selection
+            wsb = lib.rb200_lmhead_topk_workspace_bytes(N, Lr, H, V, lo, hi, int(LMHEAD_TOPK_ROW_BLOCK), -1)
+            if wsb < 0:
+                raise ValueError(f"linear_logprobs_entropy: unsupported shape N={N} L={Lr} H={H} V={V}")
+            ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+            thr = torch.empty(N, dtype=torch.float32, device=x.device)
+            L.check(lib.rb200_lmhead_topk_logprob_entropy_fwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo,
+                                                              hi, 1.0 / float(temperature), int(top_k), L.ptr(lp),
+                                                              L.ptr(ent), L.ptr(lse), L.ptr(thr), L.ptr(ws), wsb,
+                                                              L.stream_ptr(x.device)),
+                    "lmhead_topk_logprob_entropy_fwd")
+        else:
+            wsb = lmhead_workspace_bytes(N, Lr, H, V, lo, hi, vc)
+            ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+            L.check(lib.rb200_lmhead_logprob_entropy_fwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo, hi,
+                                                         1.0 / float(temperature), L.ptr(lp), L.ptr(ent), L.ptr(lse),
+                                                         L.ptr(ws), wsb, L.stream_ptr(x.device)),
+                    "lmhead_logprob_entropy_fwd")
         del ws
-        ctx.save_for_backward(x, w, tgt, lse, ent if want_entropy else lse)
+        ctx.save_for_backward(x, w, tgt, lse, ent if want_entropy else lse, thr)
         ctx.meta = (N, Lr, bs, rs, H, V, lo, hi, vc, float(temperature), want_entropy, tuple(hidden.shape))
         shape = hidden.shape[:-1]
         if want_entropy:
@@ -720,32 +769,45 @@ class _LinearLogprobEntropy(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_lp, g_ent):
         lib = L.load()
-        x, w, tgt, lse, ent = ctx.saved_tensors
+        x, w, tgt, lse, ent, thr = ctx.saved_tensors
         N, Lr, bs, rs, H, V, lo, hi, vc, temp, want_entropy, shape = ctx.meta
         need_x, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         if not (need_x or need_w):
-            return None, None, None, None, None, None
+            return None, None, None, None, None, None, None
         glp = g_lp.reshape(-1).float().contiguous() if g_lp is not None else None
         gh = g_ent.reshape(-1).float().contiguous() if (want_entropy and g_ent is not None) else None
         dx = torch.empty((N, H), dtype=torch.bfloat16, device=x.device) if need_x else None
         dw = torch.empty((V, H), dtype=torch.bfloat16, device=x.device) if need_w else None
         wsb = lmhead_workspace_bytes(N, Lr, H, V, lo, hi, vc)
         ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
-        L.check(lib.rb200_lmhead_logprob_entropy_bwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo, hi,
-                                                     1.0 / temp, L.ptr(lse), L.ptr(ent) if gh is not None else None,
-                                                     L.ptr(glp), L.ptr(gh), L.ptr(dx), L.ptr(dw), L.ptr(ws), wsb,
-                                                     L.stream_ptr(x.device)),
-                "lmhead_logprob_entropy_bwd")
-        return (dx.view(shape) if need_x else None), dw, None, None, None, None
+        if thr is not None:
+            L.check(lib.rb200_lmhead_topk_logprob_entropy_bwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo,
+                                                              hi, 1.0 / temp, L.ptr(thr), L.ptr(lse),
+                                                              L.ptr(ent) if gh is not None else None, L.ptr(glp),
+                                                              L.ptr(gh), L.ptr(dx), L.ptr(dw), L.ptr(ws), wsb,
+                                                              L.stream_ptr(x.device)),
+                    "lmhead_topk_logprob_entropy_bwd")
+        else:
+            L.check(lib.rb200_lmhead_logprob_entropy_bwd(_raw_ptr(x), L.ptr(w), L.ptr(tgt), N, Lr, bs, rs, H, V, lo, hi,
+                                                         1.0 / temp, L.ptr(lse), L.ptr(ent) if gh is not None else None,
+                                                         L.ptr(glp), L.ptr(gh), L.ptr(dx), L.ptr(dw), L.ptr(ws), wsb,
+                                                         L.stream_ptr(x.device)),
+                    "lmhead_logprob_entropy_bwd")
+        return (dx.view(shape) if need_x else None), dw, None, None, None, None, None
 
 
-def linear_logprobs_entropy(hidden, weight, target, temperature: float = 1.0, window=None, compute_entropy: bool = True):
+def linear_logprobs_entropy(hidden, weight, target, temperature: float = 1.0, window=None, compute_entropy: bool = True,
+                            top_k: int = 0):
     """logprobs_entropy_from_logits(hidden @ weight.T, ...) without the logits tensor: `hidden` [N, H] or [bsz, L, H]
     (e.g. the last hidden state's `[:, -L-1:-1, :]` slice, read in place) and `weight` = lm_head.weight [V, H], both
     bf16, H % 64 == 0.  Temperature and the vocabulary window [lo, hi) act as in logprobs_entropy_from_logits.
     Differentiable w.r.t. hidden and weight (only the gradients whose inputs require them are computed).
+    top_k acts as in logprobs_entropy_from_logits, selected on the fp32 X.W^T before the temperature; it computes the
+    whole vocabulary's logits in blocks of rows (csrc/lmhead_topk.cu) instead of only the window's.
     Returns (logprobs [...], entropy [...] or None), fp32."""
-    lp, ent = _LinearLogprobEntropy.apply(hidden, weight, target, temperature, window, bool(compute_entropy))
+    k = _top_k_arg(top_k, weight.shape[0])
+    args = (hidden, weight, target, temperature, window, bool(compute_entropy)) + ((k,) if k else ())
+    lp, ent = _LinearLogprobEntropy.apply(*args)
     return lp, (ent if compute_entropy else None)
 
 
