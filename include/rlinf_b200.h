@@ -753,6 +753,47 @@ int rb200_lmhead_topk_logprob_entropy_bwd(const void* hidden, const void* weight
                                           void* d_hidden, void* d_weight, void* workspace, int64_t workspace_bytes,
                                           rb200_stream_t stream);
 
+/* Action-token sampling of the OpenVLA-OFT rollout (csrc/action_sample.cu; OpenVLAOFTForRLActionPrediction.
+ * predict_action_batch, openvla_oft_action_model.py:350-410).  Row r (addressed as in rb200_logits_logprob_entropy_fwd)
+ * reads only its window [v_lo, v_hi), 1 <= v_hi - v_lo <= 1024:
+ *  - do_sample != 0: with 1 <= top_k < v_hi - v_lo, column i is kept iff x_i >= the top_k-th largest window value
+ *    (with multiplicity, on the unscaled values; ties are all kept); any other top_k keeps the whole window.
+ *    z = x * inv_temperature (fp32, inv_temperature > 0, else RB200_E_ARG); token[r] is drawn from softmax(z) over the
+ *    kept columns by inverse CDF in column order with one uniform of Philox4_32_10(seed, subsequence r, offset), and
+ *    logprob[r] = z_t - lse(z over the kept columns).
+ *  - do_sample == 0: token[r] = the argmax of x over the window, lowest index on ties; logprob[r] = x_t - lse(x over
+ *    the window) (no temperature, no top-k, as the reference's greedy branch).
+ * token holds absolute vocabulary ids (int64).  A NaN in the window gives a token inside the window and a NaN logprob.
+ * bins (nullable; its arrays are device memory): action[r] (fp64) = the de-tokenised, unnormalised action of position
+ * p = r % L, evaluated in numpy's order without contraction:
+ *   n = bin_centers[clip(vocab_size - token - 1, 0, n_bins - 1)], a = p % action_dim,
+ *   action = mask[a] ? 0.5 * (n + 1) * (high[a] - low[a] + 1e-8) + low[a] : n.
+ * One warp per row, fixed-order warp reductions and scan, no atomics: a row's outputs depend only on (seed, offset, r)
+ * and its values. */
+typedef struct rb200_action_bins {
+  const double* bin_centers; /* [n_bins] */
+  const double* low;         /* [action_dim]: q01 (or min) */
+  const double* high;        /* [action_dim]: q99 (or max) */
+  const uint8_t* mask;       /* [action_dim]: 0 = pass the normalised value through */
+  int64_t vocab_size;        /* the tokenizer's vocabulary (32000 for OpenVLA), not the padded V */
+  int32_t n_bins;
+  int32_t action_dim;
+} rb200_action_bins;
+int rb200_logits_sample_tokens(const void* logits, int dtype, int64_t N, int64_t L, int64_t batch_stride,
+                               int64_t row_stride, int V, int v_lo, int v_hi, int do_sample, double inv_temperature,
+                               int top_k, uint64_t seed, uint64_t offset, const rb200_action_bins* bins, int64_t* token,
+                               float* logprob, double* action, rb200_stream_t stream);
+/* The same fused into the LM head (csrc/lmhead_sample.cu): hidden and weight as in rb200_lmhead_logprob_entropy_fwd;
+ * the lmhead mainloop writes the window's raw fp32 accumulator X . W^T [row tiles * 128, ld] into the workspace (only
+ * the window's rows of W are read), then the sampler above runs on it.  rb200_lmhead_sample_workspace_bytes() returns
+ * the workspace size (about (v_hi - v_lo) * 4 bytes per row), or -1 for an unsupported shape. */
+int64_t rb200_lmhead_sample_workspace_bytes(int64_t N, int64_t L, int H, int V, int v_lo, int v_hi);
+int rb200_lmhead_sample_tokens(const void* hidden, const void* weight, int64_t N, int64_t L, int64_t batch_stride,
+                               int64_t row_stride, int H, int V, int v_lo, int v_hi, int do_sample,
+                               double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
+                               const rb200_action_bins* bins, int64_t* token, float* logprob, double* action,
+                               void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
+
 /* Vocabulary-parallel (tensor-parallel) variants of the two ops above (csrc/vocab_parallel.cu, lmhead.cu, logits.cu).
  * Equal shards (Megatron's VocabUtility; the vocabulary is padded so that P divides it): rank k of P owns the global
  * vocabulary columns [vocab_start, vocab_start + Vs), vocab_start = k * Vs; its weight shard is W[k*Vs:(k+1)*Vs] [Vs, H],

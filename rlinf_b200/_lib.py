@@ -169,6 +169,11 @@ class MbEpilogueArgs(C.Structure):
         (n, c_void_p) for n in ("pack", "scale", "metrics", "step_acc")] + [("n_mb", C.c_int32), ("reserved", C.c_int32)]
 
 
+class ActionBins(C.Structure):
+    _fields_ = [("bin_centers", c_void_p), ("low", c_void_p), ("high", c_void_p), ("mask", c_void_p),
+                ("vocab_size", c_int64), ("n_bins", C.c_int32), ("action_dim", C.c_int32)]
+
+
 class MlpLayout(C.Structure):
     _fields_ = [
         ("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("value_dim", C.c_int32), ("hidden", C.c_int32),
@@ -248,6 +253,13 @@ SIGNATURES = {
     "rb200_lmhead_topk_logprob_entropy_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                                       c_int, c_int, c_int, c_int, c_double] + [c_void_p] * 8
                                               + [c_int64, c_void_p]),
+    "rb200_logits_sample_tokens": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
+                                           c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
+                                   + [c_void_p] * 4),
+    "rb200_lmhead_sample_workspace_bytes": (c_int64, [c_int64, c_int64, c_int, c_int, c_int, c_int]),
+    "rb200_lmhead_sample_tokens": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
+                                           c_int, c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
+                                   + [c_void_p] * 4 + [c_int64, c_void_p]),
     "rb200_lmhead_vp_workspace_bytes": (c_int64, [c_int64, c_int64, c_int, c_int, c_int64, c_int, c_int, c_int64]),
     "rb200_lmhead_vp_partials_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                              c_int, c_int64, c_int, c_int, c_double, c_void_p, c_void_p, c_int64,

@@ -1,6 +1,7 @@
 // The bf16 wgmma mainloop of the fused LM-head kernels, their Params and the host helpers that set them up, shared by
-// lmhead.cu (FWD / DZ / DW / DX epilogues, the log-prob entries) and lmhead_topk.cu (ACC / DZT epilogues, the top-k
-// entries).  Everything sits in an unnamed namespace, so each object instantiates only the epilogues it launches.
+// lmhead.cu (FWD / DZ / DW / DX epilogues, the log-prob entries), lmhead_topk.cu (ACC / DZT epilogues, the top-k
+// entries) and lmhead_sample.cu (ACC, the action-token sampler).  Everything sits in an unnamed namespace, so each
+// object instantiates only the epilogues it launches.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -46,9 +47,10 @@ static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file
 constexpr int kTargetItems = 512;
 constexpr int kGroupRows = 16;
 
-// ACC and DZT are lmhead_topk.cu's: ACC stores the raw fp32 accumulator of a block of row tiles over the whole
-// vocabulary (c0 = 0, width = V); DZT is DZ with the top-k mask acc >= thr[row] on that same raw accumulator.  Their
-// code sits in `if constexpr` branches, so the other four epilogues compile exactly as without them.
+// ACC stores the raw fp32 accumulator of a block of row tiles over the columns [c0, c0 + width), column c at c - c0
+// (lmhead_topk.cu: the whole vocabulary, c0 = 0, width = V; lmhead_sample.cu: the action-bin window).  DZT, in
+// lmhead_topk.cu, is DZ with the top-k mask acc >= thr[row] on that same raw accumulator.  Their code sits in
+// `if constexpr` branches, so the other four epilogues compile exactly as without them.
 enum Mode { FWD = 0, DZ = 1, DW = 2, DX = 3, ACC = 4, DZT = 5 };
 
 struct __align__(16) Bars {
@@ -256,12 +258,12 @@ __global__ void __launch_bounds__(kThreads, 1) lmhead_kernel(const __grid_consta
     // is local row 64 (i >> 1) + rr + 8 (i & 1), local column 128 w + 8 j + 2 t + e ----
     if constexpr (MODE == ACC) {
       const int vt = vbase + tile * BN + 128 * w;
-      const int lim = P.width - vt;
+      const int lim = P.c0 + P.width - vt;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         if (!rok[i]) continue;
         const float* a = acc[i >> 1] + 2 * (i & 1);
-        float* arow = P.acc_out + ((int64_t)(rt - P.rt0) * BM + 64 * (i >> 1) + rr + 8 * (i & 1)) * P.ld + vt;
+        float* arow = P.acc_out + ((int64_t)(rt - P.rt0) * BM + 64 * (i >> 1) + rr + 8 * (i & 1)) * P.ld + (vt - P.c0);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int c = 8 * j + 2 * t;

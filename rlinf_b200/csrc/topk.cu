@@ -22,6 +22,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "radix_key.cuh"
 #include "softmax_acc.cuh"
 
 namespace {
@@ -34,34 +35,6 @@ using rb::smx::Acc;
 using rb::smx::acc_add4;
 using rb::smx::acc_init;
 using rb::smx::warp_merge;
-
-// order-preserving integer keys: a < b as floats (no NaN) <=> key(a) < key(b) as unsigned
-template <typename T>
-struct Key;
-template <>
-struct Key<float> {
-  static constexpr int kBits = 32;
-  __device__ static __forceinline__ uint32_t of(float x) {
-    const uint32_t u = __float_as_uint(x);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-  }
-  __device__ static __forceinline__ float value(uint32_t k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-  }
-  __device__ static __forceinline__ uint32_t raw(const float* p) { return of(*p); }
-};
-template <>
-struct Key<__nv_bfloat16> {
-  static constexpr int kBits = 16;
-  __device__ static __forceinline__ uint32_t of16(uint32_t u) { return (u & 0x8000u) ? (~u & 0xffffu) : (u | 0x8000u); }
-  __device__ static __forceinline__ float value(uint32_t k) {
-    const uint32_t u = (k & 0x8000u) ? (k & 0x7fffu) : (~k & 0xffffu);
-    return __uint_as_float(u << 16);
-  }
-  __device__ static __forceinline__ uint32_t raw(const __nv_bfloat16* p) {
-    return of16(*reinterpret_cast<const unsigned short*>(p));
-  }
-};
 
 template <typename T>
 __device__ __forceinline__ float ld1(const T* p) {

@@ -674,16 +674,16 @@ LMHEAD_DZ_BUDGET = 1 << 30  # bytes of the backward's bf16 dZ chunk [N, Vc]
 LMHEAD_TOPK_ROW_BLOCK = 0  # rows per top-k forward block (whole 128-row tiles); 0 = a 512 MiB fp32 accumulator block
 
 
-def _lmhead_check(hidden: torch.Tensor, weight: torch.Tensor):
+def _lmhead_check(hidden: torch.Tensor, weight: torch.Tensor, what: str = "linear_logprobs_entropy"):
     if hidden.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16:
-        raise ValueError(f"linear_logprobs_entropy: hidden and weight must be bfloat16, got {hidden.dtype} / {weight.dtype}")
+        raise ValueError(f"{what}: hidden and weight must be bfloat16, got {hidden.dtype} / {weight.dtype}")
     if weight.dim() != 2:
-        raise ValueError(f"linear_logprobs_entropy: weight must be [V, H], got shape {tuple(weight.shape)}")
+        raise ValueError(f"{what}: weight must be [V, H], got shape {tuple(weight.shape)}")
     H = weight.shape[1]
     if hidden.shape[-1] != H:
-        raise ValueError(f"linear_logprobs_entropy: hidden size {hidden.shape[-1]} != weight's {H}")
+        raise ValueError(f"{what}: hidden size {hidden.shape[-1]} != weight's {H}")
     if H % 64 != 0 or not 64 <= H <= 8192:
-        raise ValueError(f"linear_logprobs_entropy: needs H % 64 == 0 and 64 <= H <= 8192, got H = {H}")
+        raise ValueError(f"{what}: needs H % 64 == 0 and 64 <= H <= 8192, got H = {H}")
     if not (hidden.is_cuda and weight.is_cuda):
         raise L.Rb200Error("rlinf_b200 kernels take CUDA tensors; move inputs with to_device() first")
 
@@ -809,6 +809,129 @@ def linear_logprobs_entropy(hidden, weight, target, temperature: float = 1.0, wi
     args = (hidden, weight, target, temperature, window, bool(compute_entropy)) + ((k,) if k else ())
     lp, ent = _LinearLogprobEntropy.apply(*args)
     return lp, (ent if compute_entropy else None)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Action-token sampling of the OpenVLA-OFT rollout (predict_action_batch, openvla_oft_action_model.py:350-410): the bin
+# window, temperature, top-k, the draw, its log-prob and the de-tokenised action on the device, from the logits
+# (csrc/action_sample.cu) or fused into the LM head (csrc/lmhead_sample.cu)
+# ---------------------------------------------------------------------------------------------------------------
+SAMPLE_MAX_WINDOW = 1024  # widest vocabulary window the sampler takes (one warp per row)
+
+
+class ActionBins:
+    """The de-tokenisation table of predict_action_batch (:390-404) and _unnormalize_actions (:167-203): the model's
+    `vocab_size` (32000 for OpenVLA, not the padded logits width), its `bin_centers` and the dataset's action statistics
+    `low` / `high` (q01 / q99, or min / max) and `mask` (None = all True), each of length action_dim.  Built once; the
+    fp64 tables are copied to each device on first use."""
+
+    def __init__(self, vocab_size: int, bin_centers, low, high, mask=None):
+        self.vocab_size = operator.index(vocab_size)
+        self.bin_centers = torch.as_tensor(bin_centers, dtype=torch.float64).reshape(-1).cpu().contiguous()
+        self.low = torch.as_tensor(low, dtype=torch.float64).reshape(-1).cpu().contiguous()
+        self.high = torch.as_tensor(high, dtype=torch.float64).reshape(-1).cpu().contiguous()
+        self.action_dim = self.low.numel()
+        if mask is None:
+            mask = torch.ones(self.action_dim, dtype=torch.bool)
+        self.mask = torch.as_tensor(mask).reshape(-1).cpu().to(torch.bool).contiguous()
+        if self.bin_centers.numel() < 1:
+            raise ValueError("ActionBins: bin_centers is empty")
+        if self.action_dim < 1 or self.high.numel() != self.action_dim or self.mask.numel() != self.action_dim:
+            raise ValueError(f"ActionBins: low, high and mask must have the same non-zero length (action_dim), got "
+                             f"{self.low.numel()}, {self.high.numel()} and {self.mask.numel()}")
+        self._dev = {}
+
+    def args(self, device):
+        """(rb200_action_bins, the device tensors it points at) on `device`."""
+        if device not in self._dev:
+            t = [self.bin_centers.to(device), self.low.to(device), self.high.to(device),
+                 self.mask.to(device).view(torch.uint8)]
+            s = L.ActionBins(t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(), self.vocab_size,
+                             self.bin_centers.numel(), self.action_dim)
+            self._dev[device] = (s, t)
+        return self._dev[device]
+
+
+def _sample_args(V: int, window, do_sample: bool, temperature, top_k, seed, offset, bins, Lr: int, what: str):
+    """Validated (lo, hi, inv_temperature, top_k, seed, offset) of the samplers."""
+    lo, hi = (int(window[0]), int(window[1]))
+    if not (0 <= lo < hi <= V and hi - lo <= SAMPLE_MAX_WINDOW):
+        raise ValueError(f"{what}: window [{lo}, {hi}) must lie inside [0, {V}) and hold 1 to {SAMPLE_MAX_WINDOW} "
+                         f"columns")
+    k = _top_k_arg(top_k, hi - lo)
+    temperature = float(temperature)
+    if do_sample and not temperature > 0:
+        raise ValueError(f"{what}: temperature must be > 0 when sampling, got {temperature}")
+    if bins is not None:
+        if not isinstance(bins, ActionBins):
+            raise ValueError(f"{what}: bins must be an ops.ActionBins, got {type(bins).__name__}")
+        if Lr % bins.action_dim != 0:
+            raise ValueError(f"{what}: {Lr} positions per row are not whole actions of {bins.action_dim} dims")
+    seed, offset = operator.index(seed), operator.index(offset)
+    if not (0 <= seed < 1 << 64 and 0 <= offset < 1 << 64):
+        raise ValueError(f"{what}: seed and offset must be integers in [0, 2**64)")
+    return lo, hi, (1.0 / temperature if do_sample else 1.0), k, seed, offset
+
+
+def _sample_outputs(shape, device, bins):
+    tok = torch.empty(shape, dtype=torch.int64, device=device)
+    lp = torch.empty(shape, dtype=torch.float32, device=device)
+    act = torch.empty(shape, dtype=torch.float64, device=device) if bins is not None else None
+    return tok, lp, act
+
+
+def sample_action_tokens(logits, window, *, do_sample: bool, temperature: float = 1.0, top_k: int = 0, seed: int,
+                         offset: int, bins: Optional[ActionBins] = None):
+    """The action-token step of OFT's predict_action_batch (:350-410) on the device, with no host sync.
+    `logits` [bsz, L, V] fp32 / bf16 (a `[:, a:b, :]` slice is read in place); only the window [lo, hi), at most
+    SAMPLE_MAX_WINDOW columns (OpenVLA: [vocab_size - n_action_bins, vocab_size)), is read.
+    do_sample: top_k > 0 and < the window keeps the window's values >= its top_k-th largest (ties kept, selected before
+    the temperature), then the token is drawn from softmax(x / temperature) over the kept columns with Philox(seed,
+    offset, row) (the caller advances `offset` once per call), and its log-prob is over those columns.  Otherwise the
+    token is the window's argmax and its log-prob is over the whole window at temperature 1, as the reference's greedy
+    branch.  top_p is not applied (predict_action_batch ignores it).
+    bins (ops.ActionBins): also the de-tokenised, unnormalised actions, bit for bit with the reference's numpy.
+    Returns (tokens [bsz, L] int64 absolute vocabulary ids, logprobs [bsz, L] fp32, actions [bsz, L] fp64 or None)."""
+    if logits.dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"sample_action_tokens: logits must be float32 or bfloat16, got {logits.dtype}")
+    positions = logits.shape[1] if logits.dim() == 3 else logits[..., 0].numel()  # the rows' position period
+    lo, hi, inv_t, k, seed, offset = _sample_args(logits.shape[-1], window, bool(do_sample), temperature, top_k, seed,
+                                                  offset, bins, positions, "sample_action_tokens")
+    lib = L.load()
+    x, N, Lr, bs, rs, V = _logits_geometry(logits)
+    tok, lp, act = _sample_outputs(logits.shape[:-1], x.device, bins)
+    b = C.byref(bins.args(x.device)[0]) if bins is not None else None
+    L.check(lib.rb200_logits_sample_tokens(_raw_ptr(x), 0 if x.dtype == torch.float32 else 1, N, Lr, bs, rs, V, lo, hi,
+                                           int(bool(do_sample)), inv_t, k, seed, offset, b, L.ptr(tok), L.ptr(lp),
+                                           L.ptr(act), L.stream_ptr(x.device)),
+            "logits_sample_tokens")
+    return tok, lp, act
+
+
+def linear_sample_action_tokens(hidden, weight, window, *, do_sample: bool, temperature: float = 1.0, top_k: int = 0,
+                                seed: int, offset: int, bins: Optional[ActionBins] = None):
+    """sample_action_tokens(hidden @ weight.T, ...) without the logits: `hidden` [bsz, L, H] or [N, H] (the last hidden
+    state at the positions of the reference's logits slice, read in place) and `weight` = lm_head.weight [V, H], both
+    bf16, H % 64 == 0.  Only the window's rows of the weight are read: the LM-head GEMM runs over [lo, hi) into an fp32
+    workspace of about 4 (hi - lo) bytes per row (csrc/lmhead_sample.cu), then the sampler runs on it.  Same outputs."""
+    _lmhead_check(hidden, weight, "linear_sample_action_tokens")
+    lib = L.load()
+    x, N, Lr, bs, rs = _lmhead_geometry(hidden)
+    w = weight.contiguous()
+    V, H = w.shape
+    lo, hi, inv_t, k, seed, offset = _sample_args(V, window, bool(do_sample), temperature, top_k, seed, offset, bins,
+                                                  Lr, "linear_sample_action_tokens")
+    wsb = lib.rb200_lmhead_sample_workspace_bytes(N, Lr, H, V, lo, hi)
+    if wsb < 0:
+        raise ValueError(f"linear_sample_action_tokens: unsupported shape N={N} L={Lr} H={H} V={V}")
+    ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+    tok, lp, act = _sample_outputs(hidden.shape[:-1], x.device, bins)
+    b = C.byref(bins.args(x.device)[0]) if bins is not None else None
+    L.check(lib.rb200_lmhead_sample_tokens(_raw_ptr(x), L.ptr(w), N, Lr, bs, rs, H, V, lo, hi, int(bool(do_sample)),
+                                           inv_t, k, seed, offset, b, L.ptr(tok), L.ptr(lp), L.ptr(act), L.ptr(ws),
+                                           wsb, L.stream_ptr(x.device)),
+            "lmhead_sample_tokens")
+    return tok, lp, act
 
 
 # ---------------------------------------------------------------------------------------------------------------
