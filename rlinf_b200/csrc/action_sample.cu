@@ -12,10 +12,13 @@
 //   top-k: thr = the k-th largest window value, found by a 1-bit-per-pass radix select on topk.cu's integer keys (each
 //          pass counts the keys >= a candidate with an integer warp reduction); kept iff x >= thr, ties all kept;
 //   sample: z = x * inv_T; m = max over kept; e = exp(z - m); an inclusive scan of e in column order (per q a fixed
-//          shuffle scan, plus the carry of the columns before); the token is the first kept column whose prefix sum
-//          reaches u * total, u in (0, 1] from Philox4_32_10(seed, r, offset), and total is the scan's last element,
-//          so u = 1 lands on a kept column (a target past the last kept prefix sum, which the shuffle tree can round
-//          below the total, takes the last kept column); logprob = (z_t - m) - log(total);
+//          shuffle scan, plus the carry of the columns before); the token is the first column of positive weight
+//          (e > 0) whose prefix sum reaches u * total, u in (0, 1] from Philox4_32_10(seed, r, offset), and total is
+//          the scan's last element.  Each lane sums over its own shuffle tree, so the prefix sums are not monotone in
+//          the last bit: a kept column of weight 0 (a -inf logit, or exp(z - m) underflowing) can carry a larger prefix
+//          sum than the positive column before it, and is never a candidate.  A target past every positive column's
+//          prefix sum (the tree can round those below the total) takes the last column of positive weight;
+//          logprob = (z_t - m) - log(total);
 //   greedy: the argmax of x (lowest index on ties, NaN wins, as torch.argmax); logprob over the whole window at T = 1.
 // A NaN in the window makes total NaN: the scan then finds no column and the token falls back to the last kept column,
 // inside the window, with a NaN log-prob.  No floating-point or global atomics; rows are independent, so nothing
@@ -121,12 +124,14 @@ __global__ void __launch_bounds__(kWarps * 32) sample_kernel(const SArgs a) {
     for (int q = 0; q < NJ; ++q)
       if (kept(q)) m = fmaxf(m, x[q] * inv_t);
     m = warp_max(m);
-    // inclusive prefix sums of exp(z - m) in column order
+    // inclusive prefix sums of exp(z - m) in column order, and which columns have a positive weight
     float cum[NJ];
+    bool pos[NJ];
     float carry = 0.f;
 #pragma unroll
     for (int q = 0; q < NJ; ++q) {
       float s = kept(q) ? expf(x[q] * inv_t - m) : 0.f;
+      pos[q] = s > 0.f;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
         const float u = __shfl_up_sync(0xffffffffu, s, o);
@@ -142,18 +147,23 @@ __global__ void __launch_bounds__(kWarps * 32) sample_kernel(const SArgs a) {
       curandStatePhilox4_32_10_t st;
       curand_init(a.seed, (unsigned long long)r, a.offset, &st);
       const float target = curand_uniform(&st) * total;  // (0, total]
-      uint32_t first = 0xffffffffu, last = 0;
+      // only a column of positive weight can be drawn: a zero-weight column's prefix sum, on its own shuffle tree, can
+      // exceed the one of the positive column before it
+      uint32_t first = 0xffffffffu, last_pos = 0, last_kept = 0;
 #pragma unroll
       for (int q = 0; q < NJ; ++q) {
         const uint32_t c = lane + 32 * q;
-        if (kept(q)) {
+        if (pos[q]) {
           if (first == 0xffffffffu && cum[q] >= target) first = c;
-          last = c + 1;
+          last_pos = c + 1;
         }
+        if (kept(q)) last_kept = c + 1;
       }
       first = __reduce_min_sync(0xffffffffu, first);
-      last = __reduce_max_sync(0xffffffffu, last);
-      tok = first != 0xffffffffu ? first : last - 1;
+      last_pos = __reduce_max_sync(0xffffffffu, last_pos);
+      last_kept = __reduce_max_sync(0xffffffffu, last_kept);
+      // total is >= 1 (the maximum's weight) or NaN, which no prefix sum reaches
+      tok = first != 0xffffffffu ? first : (total == total ? last_pos : last_kept) - 1;
     } else {
       // argmax, lowest index on ties, NaN above everything (torch.argmax); within a lane q ascends with the column
       float bv = x[0];

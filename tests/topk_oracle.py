@@ -5,7 +5,9 @@ compute_logprobs_from_logits / compute_entropy_from_logits):
   column i is kept iff lo <= i < hi and x_i >= thr (ties at the k-th value are all kept);
   lse / logprob / entropy over the kept columns; a target that is not kept -> logprob -inf;
   a row with no kept column -> logprob NaN, entropy -0.0 and a zero gradient;
-  grad_i = inv_T (g_lp (1[i = t] - p_i) - g_H p_i (log p_i + H)) at kept columns, 0 elsewhere.
+  grad_i = inv_T (g_lp (1[i = t] - p_i) - g_H p_i (log p_i + H)) at kept columns, 0 elsewhere;
+  a kept -inf logit (thr = -inf once k reaches past the finite logits) has p_i = 0, and p_i log p_i is taken as 0
+  there, as the reference's where(p > 0, ., 0), in the entropy and in the gradient.
 top_k <= 0 or >= V: no filtering (the window only)."""
 from __future__ import annotations
 
@@ -31,7 +33,10 @@ def topk_logprobs_entropy(logits, target, temperature=1.0, window=None, top_k=0,
     lse = torch.logsumexp(z, dim=-1)
     logp = torch.where(kept, z - lse.unsqueeze(-1), torch.tensor(-float("inf"), dtype=torch.float64))
     p = torch.where(kept, logp.exp(), torch.zeros((), dtype=torch.float64))
-    ent = -torch.where(kept, p * logp, torch.zeros((), dtype=torch.float64)).sum(-1)
+    # a kept -inf logit (thr = -inf when k reaches past the finite columns) has p = 0 and logp = -inf: it adds 0, as
+    # the reference's where(p > 0, ., 0), not 0 * -inf
+    plogp = torch.where(p > 0, p * logp, torch.zeros((), dtype=torch.float64))
+    ent = -plogp.sum(-1)
     t = target.to(torch.int64).to(x.device)
     lp = torch.gather(logp, -1, t.clamp(0, V - 1).unsqueeze(-1)).squeeze(-1)
     lp = torch.where((t >= 0) & (t < V), lp, torch.tensor(-float("inf"), dtype=torch.float64))
@@ -43,7 +48,7 @@ def topk_logprobs_entropy(logits, target, temperature=1.0, window=None, top_k=0,
         gh = torch.zeros(x.shape[:-1], dtype=torch.float64) if g_h is None else g_h.to(torch.float64)
         glp, gh = glp.to(x.device), gh.to(x.device)
         onehot = torch.nn.functional.one_hot(t.clamp(0, V - 1), V).to(torch.float64)
-        g = glp.unsqueeze(-1) * (onehot - p) - gh.unsqueeze(-1) * p * (torch.where(kept, logp, 0.0) + ent.unsqueeze(-1))
+        g = glp.unsqueeze(-1) * (onehot - p) - gh.unsqueeze(-1) * (plogp + p * ent.unsqueeze(-1))
         g = torch.where(kept, g / float(temperature), torch.zeros((), dtype=torch.float64))
         out["grad"] = torch.where(empty.unsqueeze(-1), torch.zeros((), dtype=torch.float64), g)
     return out
