@@ -470,6 +470,36 @@ int rb200_value_head_bwd(const void* x, int64_t row_stride, const int64_t* rows,
                          const void* w, const int64_t* inv_map, int64_t T, void* dx, void* dw, void* workspace,
                          int64_t workspace_bytes, rb200_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Value head of the OpenVLA / OpenVLA-OFT policies (csrc/vla_value_head.cu): the reference's
+ *   ValueHead(H, hidden_sizes=(512, 128), output_dim=O, activation="gelu", bias_last=False).mlp, in the module's
+ *   bf16 semantics, on one hidden row per sample.  Every tensor is bf16; H % 64 == 0, 64 <= H <= 8192, 1 <= O <= 32,
+ *   0 <= n < 2^31 - 64.  x: rows of hidden states (unit inner stride, row_stride elements between rows, a multiple of
+ *   8 and >= H).  w0 [512, H], b0 [512], w1 [128, 512], b1 [128], w2 [O, 128]: the module's mlp.0 / 2 / 4 parameters,
+ *   contiguous.  Pointers to x, w0, w1, z0, z1, dx, dw0, dw1 and the workspace are 16-byte aligned.
+ *   gelu(z) = z 0.5 (1 + erf(z / sqrt 2)) and gelu'(z) are evaluated in fp32 on the bf16 value; every sum is fp32.
+ * rb200_vla_value_head_fwd: z0 [n, 512] = bf16(x W0^T + b0) (required: it carries layer 0 to the second launch, and
+ *   it is what the backward reads); z1 [n, 128] = bf16(bf16(gelu(z0)) W1^T + b1), or NULL when not kept;
+ *   v [n, O] = bf16(bf16(gelu(z1)) W2^T).  Two launches (none for n = 0).  Layer 0 adds 8 K slices fixed by H alone
+ *   in slice order, so a row's values are the same bits for any n, position in the batch or row stride.
+ * rb200_vla_value_head_bwd: from gv [n, O] and the forward's z0, z1: da1 = bf16(gv W2), dz1 = bf16(da1 gelu'(z1)),
+ *   da0 = bf16(dz1 W1), dz0 = bf16(da0 gelu'(z0)), then any of (NULL = skipped, at least one given)
+ *   dx [n, H] contiguous = bf16(dz0 W0)                            (needs w0)
+ *   dw0 [512, H] = bf16(dz0^T X), db0 [512] = bf16(sum_i dz0[i])   (dw0 needs x)
+ *   dw1 [128, 512] = bf16(dz1^T bf16(gelu(z0))), db1 [128] = bf16(sum_i dz1[i])
+ *   dw2 [O, 128] = bf16(gv^T bf16(gelu(z1)))
+ *   n = 0 writes zeros to the weight gradients.  At most four launches.  workspace:
+ *   rb200_vla_value_head_workspace_bytes(n, H) bytes (-1 = unsupported shape), sized from (n, H) alone.
+ *   No floating-point atomics; the order of every sum is fixed by (n, H): repeat calls give the same bits. */
+int64_t rb200_vla_value_head_workspace_bytes(int64_t n, int64_t H);
+int rb200_vla_value_head_fwd(const void* x, int64_t row_stride, int64_t n, int64_t H, const void* w0, const void* b0,
+                             const void* w1, const void* b1, const void* w2, int O, void* z0, void* z1, void* v,
+                             rb200_stream_t stream);
+int rb200_vla_value_head_bwd(const void* x, int64_t row_stride, int64_t n, int64_t H, const void* w0, const void* w1,
+                             const void* w2, int O, const void* z0, const void* z1, const void* gv, void* dx,
+                             void* dw0, void* db0, void* dw1, void* db1, void* dw2, void* workspace,
+                             int64_t workspace_bytes, rb200_stream_t stream);
+
 /* x[i] *= s (device scalar-free helper for autograd's upstream scalar). */
 int rb200_scale(float* x, int64_t n, float s, rb200_stream_t stream);
 /* x[i] *= *s_dev  (the scalar lives on the device: no host sync in autograd's backward). */

@@ -287,6 +287,11 @@ SIGNATURES = {
     "rb200_value_head_fwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "rb200_value_head_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
                                      c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "rb200_vla_value_head_workspace_bytes": (c_int64, [c_int64, c_int64]),
+    "rb200_vla_value_head_fwd": (c_int, [c_void_p, c_int64, c_int64, c_int64] + [c_void_p] * 5 + [c_int]
+                                 + [c_void_p] * 4),
+    "rb200_vla_value_head_bwd": (c_int, [c_void_p, c_int64, c_int64, c_int64] + [c_void_p] * 3 + [c_int]
+                                 + [c_void_p] * 10 + [c_int64, c_void_p]),
     "rb200_mlp_value":(c_int, [C.POINTER(MlpLayout), c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "rb200_synth_env_step": (c_int, [c_void_p] * 13 + [c_int] * 5 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),
     "rb200_synth_env_chunk_step": (c_int, [c_void_p] * 13 + [c_int] * 6 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),

@@ -1885,3 +1885,116 @@ def step_metrics_finish(step_acc: torch.Tensor, n_avg: int, n_sum: int) -> torch
     L.check(L.load().rb200_step_metrics_finish(L.ptr(step_acc.contiguous()), step_acc.shape[0], n_avg, n_sum,
                                                L.ptr(out), L.stream_ptr(step_acc.device)), "step_metrics_finish")
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Value head of the OpenVLA / OpenVLA-OFT policies (csrc/vla_value_head.cu): ValueHead(H, (512, 128), O, "gelu",
+# bias_last=False).mlp on one hidden row per sample, forward and backward
+# ---------------------------------------------------------------------------------------------------------------
+VLA_VALUE_HEAD_WIDTHS = (512, 128)
+VLA_VALUE_HEAD_MAX_OUT = 32
+
+
+def _vla_value_head_check(hidden, w0, b0, w1, b1, w2, b2, activation):
+    what = "vla_value_head"
+    if not isinstance(activation, str) or activation.lower() != "gelu":
+        raise ValueError(f"{what}: activation must be 'gelu' (the OpenVLA value head), got {activation!r}")
+    if b2 is not None:
+        raise ValueError(f"{what}: b2 must be None: the OpenVLA value head has no last-layer bias (bias_last=False)")
+    args = {"hidden": hidden, "w0": w0, "b0": b0, "w1": w1, "b1": b1, "w2": w2}
+    for name, t in args.items():
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{what}: {name} must be a tensor, got {type(t).__name__}")
+        if t.dtype != torch.bfloat16:
+            raise ValueError(f"{what}: {name} must be bfloat16, got {t.dtype}")
+    if hidden.dim() != 2:
+        raise ValueError(f"{what}: hidden must be [N, H], got shape {tuple(hidden.shape)}")
+    H = hidden.shape[1]
+    if H % 64 != 0 or not 64 <= H <= 8192:
+        raise ValueError(f"{what}: hidden needs H % 64 == 0 and 64 <= H <= 8192, got H = {H}")
+    D0, D1 = VLA_VALUE_HEAD_WIDTHS
+    O = w2.shape[0] if w2.dim() == 2 else -1
+    for name, t, shape in (("w0", w0, (D0, H)), ("b0", b0, (D0,)), ("w1", w1, (D1, D0)), ("b1", b1, (D1,)),
+                           ("w2", w2, (O, D1))):
+        if tuple(t.shape) != shape:
+            raise ValueError(f"{what}: {name} must be {list(shape)} (hidden_sizes (512, 128), H = {H}), got "
+                             f"{list(t.shape)}")
+    if not 1 <= O <= VLA_VALUE_HEAD_MAX_OUT:
+        raise ValueError(f"{what}: w2 must have 1 to {VLA_VALUE_HEAD_MAX_OUT} output rows, got {O}")
+    for name, t in args.items():
+        if t.device != hidden.device:
+            raise ValueError(f"{what}: {name} is on {t.device}, hidden on {hidden.device}")
+    if hidden.device.type != "cuda":
+        raise ValueError(f"{what}: hidden must be a CUDA tensor, got {hidden.device}")
+
+
+def _vla_value_head_fwd(x, w0, b0, w1, b1, w2, keep_z1: bool):
+    x, rs = _value_head_rows(x)
+    N, H = x.shape
+    O = w2.shape[0]
+    dev = x.device
+    z0 = torch.empty((N, VLA_VALUE_HEAD_WIDTHS[0]), dtype=torch.bfloat16, device=dev)
+    z1 = torch.empty((N, VLA_VALUE_HEAD_WIDTHS[1]), dtype=torch.bfloat16, device=dev) if keep_z1 else None
+    v = torch.empty((N, O), dtype=torch.bfloat16, device=dev)
+    if N == 0:
+        return v, x, z0, z1
+    w0, b0, w1, b1, w2 = (t.contiguous() for t in (w0, b0, w1, b1, w2))
+    L.check(L.load().rb200_vla_value_head_fwd(C.c_void_p(x.data_ptr()), rs, N, H, L.ptr(w0), L.ptr(b0), L.ptr(w1), L.ptr(b1),
+                                              L.ptr(w2), O, L.ptr(z0), L.ptr(z1), L.ptr(v), L.stream_ptr(dev)),
+            "vla_value_head_fwd")
+    return v, x, z0, z1
+
+
+class _VlaValueHead(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, hidden, w0, b0, w1, b1, w2):
+        v, x, z0, z1 = _vla_value_head_fwd(hidden, w0, b0, w1, b1, w2, keep_z1=True)
+        # x is hidden itself when its rows are read in place; only the bf16 pre-activations are new (1280 B a row)
+        ctx.save_for_backward(x, w0, w1, w2, z0, z1)
+        return v
+
+    @staticmethod
+    def backward(ctx, gv):
+        x, w0, w1, w2, z0, z1 = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        N, H = x.shape
+        O = w2.shape[0]
+        dev = x.device
+        D0, D1 = VLA_VALUE_HEAD_WIDTHS
+
+        def out(i, shape):
+            return torch.empty(shape, dtype=torch.bfloat16, device=dev) if need[i] else None
+
+        dx, dw0, db0, dw1, db1, dw2 = (out(0, (N, H)), out(1, (D0, H)), out(2, (D0,)), out(3, (D1, D0)),
+                                       out(4, (D1,)), out(5, (O, D1)))
+        if N == 0:  # empty sums
+            return tuple(None if t is None else t.zero_() for t in (dx, dw0, db0, dw1, db1, dw2))
+        lib = L.load()
+        wsb = lib.rb200_vla_value_head_workspace_bytes(N, H)
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        rs = x.stride(0)
+        g = gv.to(torch.bfloat16).contiguous()
+        w0c, w1c, w2c = w0.contiguous(), w1.contiguous(), w2.contiguous()
+        L.check(lib.rb200_vla_value_head_bwd(C.c_void_p(x.data_ptr()), rs, N, H, L.ptr(w0c), L.ptr(w1c), L.ptr(w2c),
+                                             O, L.ptr(z0), L.ptr(z1), L.ptr(g), L.ptr(dx), L.ptr(dw0), L.ptr(db0),
+                                             L.ptr(dw1), L.ptr(db1), L.ptr(dw2), L.ptr(ws), wsb, L.stream_ptr(dev)),
+                "vla_value_head_bwd")
+        return dx, dw0, db0, dw1, db1, dw2
+
+
+def vla_value_head(hidden: torch.Tensor, w0: torch.Tensor, b0: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor,
+                   w2: torch.Tensor, *, b2: Optional[torch.Tensor] = None, activation: str = "gelu") -> torch.Tensor:
+    """ValueHead(H, (512, 128), O, "gelu", bias_last=False).mlp(hidden) (models/embodiment/modules/value_head.py) in
+    the module's bf16 semantics: values [N, O] bf16 for hidden [N, H] bf16, e.g. the view last_hidden_state[:, p] of a
+    [B, S, H] tensor, whose rows are read in place when their stride is 16-byte aligned (copied once otherwise).
+    w0, b0, w1, b1, w2 are mlp[0].weight, mlp[0].bias, mlp[2].weight, mlp[2].bias, mlp[4].weight.
+
+    A row's values are the same bits for any batch size, position or row stride, so a training recompute under the
+    same weights reproduces the rollout's values exactly; the backward is deterministic.  Under torch.no_grad (or with
+    nothing requiring grad) nothing is saved; otherwise the bf16 pre-activations of both hidden layers are.  Gradients
+    are returned only for the inputs that require them.  b2 and activation exist to refuse the variants this kernel
+    does not compute (a last-layer bias, ReLU / tanh) with a ValueError."""
+    _vla_value_head_check(hidden, w0, b0, w1, b1, w2, b2, activation)
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (hidden, w0, b0, w1, b1, w2)):
+        return _VlaValueHead.apply(hidden, w0, b0, w1, b1, w2)
+    return _vla_value_head_fwd(hidden, w0, b0, w1, b1, w2, keep_z1=False)[0]
