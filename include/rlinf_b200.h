@@ -823,6 +823,38 @@ int rb200_lmhead_sample_tokens(const void* hidden, const void* weight, int64_t N
                                double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
                                const rb200_action_bins* bins, int64_t* token, float* logprob, double* action,
                                void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
+/* One generate step of the plain OpenVLA decode loop (OpenVLAForRLActionPrediction.predict_action_batch,
+ * openvla_action_model.py:610-756: VLALogitsProcessor's window, then temperature, top-k and the draw, one token per
+ * step), and the OFT call under a CUDA graph: rb200_logits_sample_step and rb200_lmhead_sample_step take the arguments
+ * of the two entries above, the same sampler and the same checks, plus a step struct (not NULL, else RB200_E_NULL):
+ *  - offset_dev (nullable; device memory, one int64): the Philox offset is *offset_dev, read on the device, and the
+ *    argument `offset` is ignored; after the sampler the entry adds 1 to *offset_dev on the same stream (as
+ *    rb200_counter_add), with no host sync.  A captured graph therefore draws with fresh offsets on every replay.
+ *    NULL: the offset is the argument, and nothing is advanced.
+ *  - out_row_stride, col0: row r = b * L + p (b = r / L, p = r % L; L as the call's) writes token, logprob and action
+ *    at b * out_row_stride + col0 + p, and de-tokenises with a = (col0 + p) % action_dim.  col0 >= 0 and
+ *    out_row_stride >= col0 + L, else RB200_E_SHAPE.  out_row_stride = L, col0 = 0 is the dense layout of the entries
+ *    above; with offset_dev NULL as well the outputs are theirs bit for bit.
+ * Step j of a [bsz, A] decode is N = bsz, L = 1, out_row_stride = A, col0 = j.  The Philox subsequence stays r, so a
+ * row's draw depends only on (seed, offset, r) and its values, whatever the output layout.
+ * rb200_lmhead_sample_step with L == 1 and N > 1 (rows b at hidden + b * batch_stride) computes the window block as one
+ * item of N positions at row stride batch_stride: its workspace is rb200_lmhead_sample_workspace_bytes(N, N, ...). */
+typedef struct rb200_sample_step {
+  const int64_t* offset_dev; /* nullable device counter of Philox offsets, advanced by 1 per call */
+  int64_t out_row_stride;    /* output elements between consecutive b */
+  int32_t col0;              /* output column (and de-tokenisation position) of p = 0 */
+  int32_t reserved;          /* 0 */
+} rb200_sample_step;
+int rb200_logits_sample_step(const void* logits, int dtype, int64_t N, int64_t L, int64_t batch_stride,
+                             int64_t row_stride, int V, int v_lo, int v_hi, int do_sample, double inv_temperature,
+                             int top_k, uint64_t seed, uint64_t offset, const rb200_action_bins* bins, int64_t* token,
+                             float* logprob, double* action, const rb200_sample_step* step, rb200_stream_t stream);
+int rb200_lmhead_sample_step(const void* hidden, const void* weight, int64_t N, int64_t L, int64_t batch_stride,
+                             int64_t row_stride, int H, int V, int v_lo, int v_hi, int do_sample,
+                             double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
+                             const rb200_action_bins* bins, int64_t* token, float* logprob, double* action,
+                             void* workspace, int64_t workspace_bytes, const rb200_sample_step* step,
+                             rb200_stream_t stream);
 
 /* Vocabulary-parallel (tensor-parallel) variants of the two ops above (csrc/vocab_parallel.cu, lmhead.cu, logits.cu).
  * Equal shards (Megatron's VocabUtility; the vocabulary is padded so that P divides it): rank k of P owns the global

@@ -174,6 +174,10 @@ class ActionBins(C.Structure):
                 ("vocab_size", c_int64), ("n_bins", C.c_int32), ("action_dim", C.c_int32)]
 
 
+class SampleStep(C.Structure):
+    _fields_ = [("offset_dev", c_void_p), ("out_row_stride", c_int64), ("col0", C.c_int32), ("reserved", C.c_int32)]
+
+
 class MlpLayout(C.Structure):
     _fields_ = [
         ("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("value_dim", C.c_int32), ("hidden", C.c_int32),
@@ -260,6 +264,12 @@ SIGNATURES = {
     "rb200_lmhead_sample_tokens": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
                                            c_int, c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
                                    + [c_void_p] * 4 + [c_int64, c_void_p]),
+    "rb200_logits_sample_step": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
+                                         c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
+                                 + [c_void_p] * 3 + [C.POINTER(SampleStep), c_void_p]),
+    "rb200_lmhead_sample_step": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
+                                         c_int, c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
+                                 + [c_void_p] * 4 + [c_int64, C.POINTER(SampleStep), c_void_p]),
     "rb200_lmhead_vp_workspace_bytes": (c_int64, [c_int64, c_int64, c_int, c_int, c_int64, c_int, c_int, c_int64]),
     "rb200_lmhead_vp_partials_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
                                              c_int, c_int64, c_int, c_int, c_double, c_void_p, c_void_p, c_int64,

@@ -23,6 +23,12 @@
 // A NaN in the window makes total NaN: the scan then finds no column and the token falls back to the last kept column,
 // inside the window, with a NaN log-prob.  No floating-point or global atomics; rows are independent, so nothing
 // depends on the grid or the SM count.
+//
+// One generate step (rb200_logits_sample_step, rb200_lmhead_sample_step; the plain OpenVLA decode loop of
+// OpenVLAForRLActionPrediction.predict_action_batch, openvla_action_model.py:610-756): the Philox offset is read from a
+// device counter that the entry then advances by 1 on the same stream (rollout.cu's rb200_counter_add), so a captured
+// graph draws fresh numbers on every replay; and row r = b * L + p writes its outputs at b * out_row_stride + col0 + p
+// and de-tokenises with dimension (col0 + p) % action_dim, so step j of a [bsz, A] buffer is column col0 = j.
 #include <cuda_bf16.h>
 #include <curand_kernel.h>
 
@@ -50,6 +56,11 @@ struct SArgs {
   // (rt % tpb) * 128 + j % 128 < L (padding rows are skipped); its columns are the window's
   int tiled, tpb;
   int64_t rt0;
+  // the step entries: Philox offset from *offset_dev when set; row r (in rows of out_L positions) writes at
+  // (r / out_L) * out_stride + col0 + r % out_L.  The plain entries have out_L = out_stride = L and col0 = 0.
+  const int64_t* offset_dev;
+  int64_t out_L, out_stride;
+  int col0;
 };
 
 template <typename T>
@@ -145,7 +156,8 @@ __global__ void __launch_bounds__(kWarps * 32) sample_kernel(const SArgs a) {
     uint32_t tok;  // window column
     if (a.do_sample) {
       curandStatePhilox4_32_10_t st;
-      curand_init(a.seed, (unsigned long long)r, a.offset, &st);
+      const uint64_t off = a.offset_dev ? (uint64_t)*a.offset_dev : a.offset;
+      curand_init(a.seed, (unsigned long long)r, off, &st);
       const float target = curand_uniform(&st) * total;  // (0, total]
       // only a column of positive weight can be drawn: a zero-weight column's prefix sum, on its own shuffle tree, can
       // exceed the one of the positive column before it
@@ -196,15 +208,17 @@ __global__ void __launch_bounds__(kWarps * 32) sample_kernel(const SArgs a) {
     zt = __shfl_sync(0xffffffffu, zt, tok & 31);
     if (lane == 0) {
       const int64_t id = (int64_t)a.v_lo + tok;
-      a.token[r] = id;
-      a.logprob[r] = (zt - m) - logf(total);
+      const int64_t op = a.col0 + r % a.out_L;  // output column (= p for the plain entries)
+      const int64_t o = (r / a.out_L) * a.out_stride + op;
+      a.token[o] = id;
+      a.logprob[o] = (zt - m) - logf(total);
       if (a.has_bins) {
         const rb200_action_bins& B = a.bins;
         int64_t d = B.vocab_size - id - 1;
         d = d < 0 ? 0 : (d > B.n_bins - 1 ? B.n_bins - 1 : d);
         const double n = B.bin_centers[d];
-        const int ad = (int)(p % B.action_dim);
-        a.action[r] = B.mask[ad] ? unnormalize(n, B.low[ad], B.high[ad]) : n;
+        const int ad = (int)(op % B.action_dim);
+        a.action[o] = B.mask[ad] ? unnormalize(n, B.low[ad], B.high[ad]) : n;
       }
     }
   }
@@ -233,6 +247,30 @@ int check_common(int W, int do_sample, double inv_temperature, const rb200_actio
   return RB200_OK;
 }
 
+// the step struct against the call's L: a layout that every row's outputs fit in, columns not overlapping the next row's
+int check_step(const rb200_sample_step* s, int64_t L) {
+  if (!s) return RB200_E_NULL;
+  if (s->col0 < 0 || s->out_row_stride < (int64_t)s->col0 + L) return RB200_E_SHAPE;
+  return RB200_OK;
+}
+
+void apply_step(SArgs& a, const rb200_sample_step* s, int64_t L) {
+  a.out_L = L;
+  if (s) {
+    a.offset_dev = s->offset_dev;
+    a.out_stride = s->out_row_stride;
+    a.col0 = s->col0;
+  } else {
+    a.out_stride = L;
+  }
+}
+
+// the counter advance after the sampler's launch: every row has read the offset before it runs
+int advance(const rb200_sample_step* s, cudaStream_t st) {
+  if (!s || !s->offset_dev) return RB200_OK;
+  return rb200_counter_add(reinterpret_cast<uint64_t*>(const_cast<int64_t*>(s->offset_dev)), 1, st);
+}
+
 SArgs make_args(int v_lo, int v_hi, int do_sample, double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
                 const rb200_action_bins* bins, int64_t* token, float* logprob, double* action) {
   SArgs a{};
@@ -250,18 +288,23 @@ SArgs make_args(int v_lo, int v_hi, int do_sample, double inv_temperature, int t
 namespace rb {
 namespace asmp {
 // the sampler over a block of nt row tiles of the window's raw fp32 logits [nt * 128, ld] (lmhead_sample.cu's ACC
-// pass), writing row r's outputs at r
+// pass), writing row r's outputs at r; with a step struct (nullable) at its layout in rows of out_L positions, out_L
+// being the caller's L (the tiles may group the rows differently), then the counter advance
 int sample_tiles(const float* block, int64_t ld, int v_lo, int v_hi, int do_sample, double inv_temperature, int top_k,
                  uint64_t seed, uint64_t offset, const rb200_action_bins* bins, int64_t rt0, int64_t nt, int tpb,
-                 int64_t L_rows, int64_t* token, float* logprob, double* action, cudaStream_t st) {
+                 int64_t L_rows, int64_t* token, float* logprob, double* action, const rb200_sample_step* step,
+                 int64_t out_L, cudaStream_t st) {
   SArgs a = make_args(v_lo, v_hi, do_sample, inv_temperature, top_k, seed, offset, bins, token, logprob, action);
   a.x = block; a.N = nt * 128; a.L = L_rows; a.row_stride = ld; a.tiled = 1; a.tpb = tpb; a.rt0 = rt0;
-  return launch<float>(a, st);
+  apply_step(a, step, step ? out_L : L_rows);
+  int e = launch<float>(a, st);
+  return e ? e : advance(step, st);
 }
 int check_sample(int W, int do_sample, double inv_temperature, const rb200_action_bins* bins, const int64_t* token,
                  const float* logprob, const double* action) {
   return check_common(W, do_sample, inv_temperature, bins, token, logprob, action);
 }
+int check_sample_step(const rb200_sample_step* step, int64_t L) { return check_step(step, L); }
 }  // namespace asmp
 }  // namespace rb
 
@@ -277,6 +320,25 @@ extern "C" int rb200_logits_sample_tokens(const void* logits, int dtype, int64_t
   if (e) return e;
   SArgs a = make_args(v_lo, v_hi, do_sample, inv_temperature, top_k, seed, offset, bins, token, logprob, action);
   a.x = logits; a.N = N; a.L = L; a.batch_stride = batch_stride; a.row_stride = row_stride;
+  apply_step(a, nullptr, L);
   cudaStream_t st = rb::as_stream(stream);
   return dtype == 0 ? launch<float>(a, st) : launch<__nv_bfloat16>(a, st);
+}
+
+extern "C" int rb200_logits_sample_step(const void* logits, int dtype, int64_t N, int64_t L, int64_t batch_stride,
+                                        int64_t row_stride, int V, int v_lo, int v_hi, int do_sample,
+                                        double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
+                                        const rb200_action_bins* bins, int64_t* token, float* logprob, double* action,
+                                        const rb200_sample_step* step, rb200_stream_t stream) {
+  if (!logits) return RB200_E_NULL;
+  if (dtype != 0 && dtype != 1) return RB200_E_UNSUPPORTED;
+  if (N <= 0 || L <= 0 || N % L != 0 || V <= 0 || v_lo < 0 || v_hi > V || v_lo >= v_hi) return RB200_E_SHAPE;
+  int e = check_common(v_hi - v_lo, do_sample, inv_temperature, bins, token, logprob, action);
+  if (e || (e = check_step(step, L))) return e;
+  SArgs a = make_args(v_lo, v_hi, do_sample, inv_temperature, top_k, seed, offset, bins, token, logprob, action);
+  a.x = logits; a.N = N; a.L = L; a.batch_stride = batch_stride; a.row_stride = row_stride;
+  apply_step(a, step, L);
+  cudaStream_t st = rb::as_stream(stream);
+  e = dtype == 0 ? launch<float>(a, st) : launch<__nv_bfloat16>(a, st);
+  return e ? e : advance(step, st);
 }

@@ -852,8 +852,9 @@ class ActionBins:
         return self._dev[device]
 
 
-def _sample_args(V: int, window, do_sample: bool, temperature, top_k, seed, offset, bins, Lr: int, what: str):
-    """Validated (lo, hi, inv_temperature, top_k, seed, offset) of the samplers."""
+def _sample_args(V: int, window, do_sample: bool, temperature, top_k, seed, offset, bins, Lr, what: str):
+    """Validated (lo, hi, inv_temperature, top_k, seed, offset) of the samplers; Lr None skips the whole-actions check
+    (a generate step de-tokenises by its output column), offset None is a device counter's call."""
     lo, hi = (int(window[0]), int(window[1]))
     if not (0 <= lo < hi <= V and hi - lo <= SAMPLE_MAX_WINDOW):
         raise ValueError(f"{what}: window [{lo}, {hi}) must lie inside [0, {V}) and hold 1 to {SAMPLE_MAX_WINDOW} "
@@ -865,9 +866,10 @@ def _sample_args(V: int, window, do_sample: bool, temperature, top_k, seed, offs
     if bins is not None:
         if not isinstance(bins, ActionBins):
             raise ValueError(f"{what}: bins must be an ops.ActionBins, got {type(bins).__name__}")
-        if Lr % bins.action_dim != 0:
+        if Lr is not None and Lr % bins.action_dim != 0:
             raise ValueError(f"{what}: {Lr} positions per row are not whole actions of {bins.action_dim} dims")
-    seed, offset = operator.index(seed), operator.index(offset)
+    seed = operator.index(seed)
+    offset = 0 if offset is None else operator.index(offset)
     if not (0 <= seed < 1 << 64 and 0 <= offset < 1 << 64):
         raise ValueError(f"{what}: seed and offset must be integers in [0, 2**64)")
     return lo, hi, (1.0 / temperature if do_sample else 1.0), k, seed, offset
@@ -880,57 +882,148 @@ def _sample_outputs(shape, device, bins):
     return tok, lp, act
 
 
-def sample_action_tokens(logits, window, *, do_sample: bool, temperature: float = 1.0, top_k: int = 0, seed: int,
-                         offset: int, bins: Optional[ActionBins] = None):
-    """The action-token step of OFT's predict_action_batch (:350-410) on the device, with no host sync.
+def _step_mode(offset, counter, out, column, top_p, device, bins, what: str):
+    """Validates the generate-step arguments.  Returns (step: bool, column or None); a step call goes through the
+    *_sample_step entries (a device counter, an output column, or both)."""
+    if float(top_p) != 1.0:
+        raise ValueError(f"{what}: top_p must be 1.0 (no nucleus filter is applied), got {top_p}")
+    if (offset is None) == (counter is None):
+        raise ValueError(f"{what}: give exactly one of offset= (a host integer) and counter= (a device int64 tensor)")
+    if counter is not None:
+        if not isinstance(counter, torch.Tensor) or counter.dtype != torch.int64 or counter.numel() != 1:
+            raise ValueError(f"{what}: counter must be a 1-element int64 tensor")
+        if not counter.is_cuda or counter.device != device:
+            raise ValueError(f"{what}: counter must be a CUDA tensor on {device}, got {counter.device}")
+    if (out is None) != (column is None):
+        raise ValueError(f"{what}: out= and column= go together")
+    if out is None:
+        return counter is not None, None
+    try:
+        if isinstance(column, bool):
+            raise TypeError
+        column = operator.index(column)
+    except TypeError:
+        raise ValueError(f"{what}: column must be an integer, got {column!r}") from None
+    if not isinstance(out, (tuple, list)) or len(out) != 3:
+        raise ValueError(f"{what}: out must be (tokens, logprobs, actions or None)")
+    tok, lp, act = out
+    if (act is None) != (bins is None):
+        raise ValueError(f"{what}: out's actions buffer must be given exactly when bins is")
+    for name, t, dt in (("tokens", tok, torch.int64), ("logprobs", lp, torch.float32), ("actions", act, torch.float64)):
+        if name == "actions" and t is None:
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != dt or t.dim() != 2:
+            raise ValueError(f"{what}: out's {name} must be a [bsz, A] {dt} tensor")
+        if t.device != device or not t.is_contiguous():
+            raise ValueError(f"{what}: out's {name} must be contiguous and on {device}")
+        if t.shape != tok.shape:
+            raise ValueError(f"{what}: out's buffers must share one [bsz, A] shape, got {tuple(t.shape)} and "
+                             f"{tuple(tok.shape)}")
+    if not 0 <= column < tok.shape[1]:
+        raise ValueError(f"{what}: column {column} is outside [0, {tok.shape[1]})")
+    return True, column
+
+
+def _step_struct(counter, Lr: int, out, column):
+    """The rb200_sample_step of a step call: the counter, and column `column` of the [bsz, A] buffers or the dense
+    [bsz, Lr] layout."""
+    return L.SampleStep(counter.data_ptr() if counter is not None else None,
+                        out[0].shape[1] if out is not None else Lr, column or 0, 0)
+
+
+def sample_action_tokens(logits, window, *, do_sample: bool, temperature: float = 1.0, top_k: int = 0, top_p=1.0,
+                         seed: int, offset: Optional[int] = None, counter: Optional[torch.Tensor] = None,
+                         bins: Optional[ActionBins] = None, out=None, column: Optional[int] = None):
+    """The action-token step of OFT's predict_action_batch (:350-410), and one generate step of plain OpenVLA's
+    (openvla_action_model.py:610-756), on the device, with no host sync.
     `logits` [bsz, L, V] fp32 / bf16 (a `[:, a:b, :]` slice is read in place); only the window [lo, hi), at most
-    SAMPLE_MAX_WINDOW columns (OpenVLA: [vocab_size - n_action_bins, vocab_size)), is read.
+    SAMPLE_MAX_WINDOW columns, is read.  OpenVLA and OFT: [vocab_size - n_action_bins, vocab_size) = [31744, 32000) of
+    the padded 32064 (plain OpenVLA's VLALogitsProcessor, :453-471, masks the same window before the warpers).
     do_sample: top_k > 0 and < the window keeps the window's values >= its top_k-th largest (ties kept, selected before
     the temperature), then the token is drawn from softmax(x / temperature) over the kept columns with Philox(seed,
-    offset, row) (the caller advances `offset` once per call), and its log-prob is over those columns.  Otherwise the
-    token is the window's argmax and its log-prob is over the whole window at temperature 1, as the reference's greedy
-    branch.  top_p is not applied (predict_action_batch ignores it).
-    bins (ops.ActionBins): also the de-tokenised, unnormalised actions, bit for bit with the reference's numpy.
-    Returns (tokens [bsz, L] int64 absolute vocabulary ids, logprobs [bsz, L] fp32, actions [bsz, L] fp64 or None)."""
+    offset, row), and its log-prob is over those columns.  Otherwise the token is the window's argmax and its log-prob
+    is over the whole window at temperature 1, as the reference's greedy branch.  top_p must be 1.0: OFT's
+    predict_action_batch ignores it, and plain OpenVLA's generate would apply TopPLogitsWarper, which this op does not.
+    The Philox offset is either `offset` (the caller advances it once per call) or `counter`, a 1-element int64 CUDA
+    tensor read on the device and advanced by 1 after the call on the current stream: a CUDA graph that captures the
+    call draws with fresh offsets on every replay.  Exactly one of the two.
+    bins (ops.ActionBins): also the de-tokenised, unnormalised actions, bit for bit with the reference's numpy.  Its
+    tables are copied to the device on the first call there, so make one call before capturing a graph.
+    Returns (tokens [bsz, L] int64 absolute vocabulary ids, logprobs [bsz, L] fp32, actions [bsz, L] fp64 or None).
+    Generate step (plain OpenVLA): `logits` [bsz, 1, V] (or [bsz, V]) is step j's last-position logits; with
+    out=(tokens, logprobs, actions or None), [bsz, A] buffers allocated once per env step (actions exactly when bins),
+    and column=j, the call writes column j of them and de-tokenises with dimension j % bins.action_dim, and returns
+    `out`.  The value row of ops.vla_value_head is step 0's last-position hidden state (:732-737)."""
+    what = "sample_action_tokens"
     if logits.dtype not in (torch.float32, torch.bfloat16):
-        raise ValueError(f"sample_action_tokens: logits must be float32 or bfloat16, got {logits.dtype}")
+        raise ValueError(f"{what}: logits must be float32 or bfloat16, got {logits.dtype}")
+    step, column = _step_mode(offset, counter, out, column, top_p, logits.device, bins, what)
+    if column is not None:
+        if logits.dim() == 2:
+            logits = logits.unsqueeze(1)
+        if logits.dim() != 3 or logits.shape[1] != 1 or logits.shape[0] != out[0].shape[0]:
+            raise ValueError(f"{what}: a step call takes logits [bsz, 1, V] with bsz = out's {out[0].shape[0]} rows, "
+                             f"got {tuple(logits.shape)}")
     positions = logits.shape[1] if logits.dim() == 3 else logits[..., 0].numel()  # the rows' position period
     lo, hi, inv_t, k, seed, offset = _sample_args(logits.shape[-1], window, bool(do_sample), temperature, top_k, seed,
-                                                  offset, bins, positions, "sample_action_tokens")
+                                                  offset, bins, None if column is not None else positions, what)
     lib = L.load()
     x, N, Lr, bs, rs, V = _logits_geometry(logits)
-    tok, lp, act = _sample_outputs(logits.shape[:-1], x.device, bins)
+    tok, lp, act = out if column is not None else _sample_outputs(logits.shape[:-1], x.device, bins)
     b = C.byref(bins.args(x.device)[0]) if bins is not None else None
-    L.check(lib.rb200_logits_sample_tokens(_raw_ptr(x), 0 if x.dtype == torch.float32 else 1, N, Lr, bs, rs, V, lo, hi,
-                                           int(bool(do_sample)), inv_t, k, seed, offset, b, L.ptr(tok), L.ptr(lp),
-                                           L.ptr(act), L.stream_ptr(x.device)),
-            "logits_sample_tokens")
+    args = (_raw_ptr(x), 0 if x.dtype == torch.float32 else 1, N, Lr, bs, rs, V, lo, hi, int(bool(do_sample)), inv_t,
+            k, seed, offset, b, L.ptr(tok), L.ptr(lp), L.ptr(act))
+    if step:
+        st = _step_struct(counter, Lr, out, column)
+        L.check(lib.rb200_logits_sample_step(*args, C.byref(st), L.stream_ptr(x.device)), "logits_sample_step")
+    else:
+        L.check(lib.rb200_logits_sample_tokens(*args, L.stream_ptr(x.device)), "logits_sample_tokens")
     return tok, lp, act
 
 
 def linear_sample_action_tokens(hidden, weight, window, *, do_sample: bool, temperature: float = 1.0, top_k: int = 0,
-                                seed: int, offset: int, bins: Optional[ActionBins] = None):
+                                top_p=1.0, seed: int, offset: Optional[int] = None,
+                                counter: Optional[torch.Tensor] = None, bins: Optional[ActionBins] = None, out=None,
+                                column: Optional[int] = None):
     """sample_action_tokens(hidden @ weight.T, ...) without the logits: `hidden` [bsz, L, H] or [N, H] (the last hidden
     state at the positions of the reference's logits slice, read in place) and `weight` = lm_head.weight [V, H], both
     bf16, H % 64 == 0.  Only the window's rows of the weight are read: the LM-head GEMM runs over [lo, hi) into an fp32
-    workspace of about 4 (hi - lo) bytes per row (csrc/lmhead_sample.cu), then the sampler runs on it.  Same outputs."""
-    _lmhead_check(hidden, weight, "linear_sample_action_tokens")
+    workspace of about 4 (hi - lo) bytes per row (csrc/lmhead_sample.cu), then the sampler runs on it.  Same outputs,
+    and the same offset / counter, top_p, out and column arguments.
+    Generate step (plain OpenVLA): `hidden` [bsz, H] (or [bsz, 1, H]) is step j's last-position hidden state, and
+    out / column write column j of the caller's [bsz, A] buffers; the bsz rows share the GEMM's 128-row tiles.  The
+    plain OpenVLA window is [31744, 32000): 256 of the 32064 rows of lm_head.weight."""
+    what = "linear_sample_action_tokens"
+    step, column = _step_mode(offset, counter, out, column, top_p, hidden.device, bins, what)
+    _lmhead_check(hidden, weight, what)
+    if column is not None:
+        if hidden.dim() == 3 and hidden.shape[1] == 1:
+            hidden = hidden[:, 0]
+        if hidden.dim() != 2 or hidden.shape[0] != out[0].shape[0]:
+            raise ValueError(f"{what}: a step call takes hidden [bsz, H] with bsz = out's {out[0].shape[0]} rows, got "
+                             f"{tuple(hidden.shape)}")
     lib = L.load()
     x, N, Lr, bs, rs = _lmhead_geometry(hidden)
+    if column is not None:  # one position per sample: N rows of one position, b at x + b * rs
+        Lr, bs = 1, rs
     w = weight.contiguous()
     V, H = w.shape
     lo, hi, inv_t, k, seed, offset = _sample_args(V, window, bool(do_sample), temperature, top_k, seed, offset, bins,
-                                                  Lr, "linear_sample_action_tokens")
-    wsb = lib.rb200_lmhead_sample_workspace_bytes(N, Lr, H, V, lo, hi)
+                                                  None if column is not None else Lr, what)
+    Lw = N if step and Lr == 1 else Lr  # a step call with L == 1 tiles the N rows as one item of N positions
+    wsb = lib.rb200_lmhead_sample_workspace_bytes(N, Lw, H, V, lo, hi)
     if wsb < 0:
-        raise ValueError(f"linear_sample_action_tokens: unsupported shape N={N} L={Lr} H={H} V={V}")
+        raise ValueError(f"{what}: unsupported shape N={N} L={Lr} H={H} V={V}")
     ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
-    tok, lp, act = _sample_outputs(hidden.shape[:-1], x.device, bins)
+    tok, lp, act = out if column is not None else _sample_outputs(hidden.shape[:-1], x.device, bins)
     b = C.byref(bins.args(x.device)[0]) if bins is not None else None
-    L.check(lib.rb200_lmhead_sample_tokens(_raw_ptr(x), L.ptr(w), N, Lr, bs, rs, H, V, lo, hi, int(bool(do_sample)),
-                                           inv_t, k, seed, offset, b, L.ptr(tok), L.ptr(lp), L.ptr(act), L.ptr(ws),
-                                           wsb, L.stream_ptr(x.device)),
-            "lmhead_sample_tokens")
+    args = (_raw_ptr(x), L.ptr(w), N, Lr, bs, rs, H, V, lo, hi, int(bool(do_sample)), inv_t, k, seed, offset, b,
+            L.ptr(tok), L.ptr(lp), L.ptr(act), L.ptr(ws), wsb)
+    if step:
+        st = _step_struct(counter, Lr, out, column)
+        L.check(lib.rb200_lmhead_sample_step(*args, C.byref(st), L.stream_ptr(x.device)), "lmhead_sample_step")
+    else:
+        L.check(lib.rb200_lmhead_sample_tokens(*args, L.stream_ptr(x.device)), "lmhead_sample_tokens")
     return tok, lp, act
 
 
