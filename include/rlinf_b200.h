@@ -40,8 +40,6 @@ typedef void* rb200_stream_t; /* cudaStream_t */
 
 int rb200_abi_version(void);
 const char* rb200_strerror(int code);
-/* sm count / compute capability of the current device (host-side query). */
-int rb200_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* kernels launched by this library in this process so far (host counter; launches replayed from a
  * captured CUDA graph are counted once, at capture). */
 uint64_t rb200_launch_count(void);
@@ -516,17 +514,11 @@ int rb200_scale_by(float* x, int64_t n, const float* s_dev, rb200_stream_t strea
  * ---------------------------------------------------------------------------------------- */
 int rb200_grad_sqnorm(const float* grads, int64_t n, double* out_sq /*[1], reset by kernel*/,
                       rb200_stream_t stream);
-int rb200_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq,
-                     int64_t n, const int64_t* group_end_host, const double* group_lr_host,
-                     int n_groups, double beta1, double beta2, double eps, double weight_decay,
-                     float max_grad_norm, float grad_scale, const double* grad_sq /*[1]*/,
-                     double* state /*[4]*/, rb200_stream_t stream);
-/* Same step with the per-group learning rates read from DEVICE memory (double[n_groups]) at execution time, so a
- * captured CUDA graph follows an LR schedule (LambdaLR stepped once per run_training,
- * workers/actor/embodied_fsdp_actor_worker.py:571, hybrid_engines/fsdp/utils.py:522) without re-capture.
- * In both entries lr < 0 marks a FROZEN group: its parameters and moments are left untouched - what
- * torch.optim.AdamW does for parameters outside its param groups (the actor during critic warm-up,
- * fsdp_model_manager.py:523-531) or whose grad is None. */
+/* The per-group learning rates are read from DEVICE memory (double[n_groups]) at execution time, so a captured CUDA
+ * graph follows an LR schedule (LambdaLR stepped once per run_training, workers/actor/embodied_fsdp_actor_worker.py:571,
+ * hybrid_engines/fsdp/utils.py:522) without re-capture.  lr < 0 marks a FROZEN group: its parameters and moments are
+ * left untouched - what torch.optim.AdamW does for parameters outside its param groups (the actor during critic
+ * warm-up, fsdp_model_manager.py:523-531) or whose grad is None. */
 int rb200_adamw_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq,
                          int64_t n, const int64_t* group_end_host, const double* group_lr_dev,
                          int n_groups, double beta1, double beta2, double eps, double weight_decay,
@@ -624,7 +616,7 @@ int rb200_debug_set_flags(int flags);
  * MultiStepRolloutWorker.generate (rlinf/workers/env/env_worker.py:1059-1349,
  * rlinf/workers/rollout/hf/huggingface_worker.py:678-781) for the MLP-policy + device-resident env case, with the same
  * buffers, row alignment and random streams as the per-kernel path (rb200_mlp_sample + rb200_synth_env_step or
- * rb200_synth_env_chunk_step + rb200_mlp_value + rb200_bootstrap_rewards[_ld] per step).  Both kernels take everything
+ * rb200_synth_env_chunk_step + rb200_mlp_value + rb200_bootstrap_rewards_ld per step).  Both kernels take everything
  * but the weights in one rb200_rollout_args (pointers, then 64-bit, then 32-bit integers, then doubles: no padding). */
 typedef struct rb200_rollout_args {
   /* buffers; T = chunk steps, C = num_action_chunks, act = act_dim = C*A, obs = obs_dim */
@@ -809,36 +801,20 @@ typedef struct rb200_action_bins {
   int32_t n_bins;
   int32_t action_dim;
 } rb200_action_bins;
-int rb200_logits_sample_tokens(const void* logits, int dtype, int64_t N, int64_t L, int64_t batch_stride,
-                               int64_t row_stride, int V, int v_lo, int v_hi, int do_sample, double inv_temperature,
-                               int top_k, uint64_t seed, uint64_t offset, const rb200_action_bins* bins, int64_t* token,
-                               float* logprob, double* action, rb200_stream_t stream);
-/* The same fused into the LM head (csrc/lmhead_sample.cu): hidden and weight as in rb200_lmhead_logprob_entropy_fwd;
- * the lmhead mainloop writes the window's raw fp32 accumulator X . W^T [row tiles * 128, ld] into the workspace (only
- * the window's rows of W are read), then the sampler above runs on it.  rb200_lmhead_sample_workspace_bytes() returns
- * the workspace size (about (v_hi - v_lo) * 4 bytes per row), or -1 for an unsupported shape. */
-int64_t rb200_lmhead_sample_workspace_bytes(int64_t N, int64_t L, int H, int V, int v_lo, int v_hi);
-int rb200_lmhead_sample_tokens(const void* hidden, const void* weight, int64_t N, int64_t L, int64_t batch_stride,
-                               int64_t row_stride, int H, int V, int v_lo, int v_hi, int do_sample,
-                               double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
-                               const rb200_action_bins* bins, int64_t* token, float* logprob, double* action,
-                               void* workspace, int64_t workspace_bytes, rb200_stream_t stream);
-/* One generate step of the plain OpenVLA decode loop (OpenVLAForRLActionPrediction.predict_action_batch,
+/* step (nullable): NULL writes row r's outputs at r with the argument `offset` as the Philox offset.  A step struct
+ * serves one generate step of the plain OpenVLA decode loop (OpenVLAForRLActionPrediction.predict_action_batch,
  * openvla_action_model.py:610-756: VLALogitsProcessor's window, then temperature, top-k and the draw, one token per
- * step), and the OFT call under a CUDA graph: rb200_logits_sample_step and rb200_lmhead_sample_step take the arguments
- * of the two entries above, the same sampler and the same checks, plus a step struct (not NULL, else RB200_E_NULL):
+ * step), and the OFT call under a CUDA graph; the sampler and the checks are the same:
  *  - offset_dev (nullable; device memory, one int64): the Philox offset is *offset_dev, read on the device, and the
  *    argument `offset` is ignored; after the sampler the entry adds 1 to *offset_dev on the same stream (as
  *    rb200_counter_add), with no host sync.  A captured graph therefore draws with fresh offsets on every replay.
  *    NULL: the offset is the argument, and nothing is advanced.
  *  - out_row_stride, col0: row r = b * L + p (b = r / L, p = r % L; L as the call's) writes token, logprob and action
  *    at b * out_row_stride + col0 + p, and de-tokenises with a = (col0 + p) % action_dim.  col0 >= 0 and
- *    out_row_stride >= col0 + L, else RB200_E_SHAPE.  out_row_stride = L, col0 = 0 is the dense layout of the entries
- *    above; with offset_dev NULL as well the outputs are theirs bit for bit.
+ *    out_row_stride >= col0 + L, else RB200_E_SHAPE.  out_row_stride = L, col0 = 0 is the dense layout of a NULL
+ *    step; with offset_dev NULL as well the outputs are a NULL step's bit for bit.
  * Step j of a [bsz, A] decode is N = bsz, L = 1, out_row_stride = A, col0 = j.  The Philox subsequence stays r, so a
- * row's draw depends only on (seed, offset, r) and its values, whatever the output layout.
- * rb200_lmhead_sample_step with L == 1 and N > 1 (rows b at hidden + b * batch_stride) computes the window block as one
- * item of N positions at row stride batch_stride: its workspace is rb200_lmhead_sample_workspace_bytes(N, N, ...). */
+ * row's draw depends only on (seed, offset, r) and its values, whatever the output layout. */
 typedef struct rb200_sample_step {
   const int64_t* offset_dev; /* nullable device counter of Philox offsets, advanced by 1 per call */
   int64_t out_row_stride;    /* output elements between consecutive b */
@@ -849,6 +825,13 @@ int rb200_logits_sample_step(const void* logits, int dtype, int64_t N, int64_t L
                              int64_t row_stride, int V, int v_lo, int v_hi, int do_sample, double inv_temperature,
                              int top_k, uint64_t seed, uint64_t offset, const rb200_action_bins* bins, int64_t* token,
                              float* logprob, double* action, const rb200_sample_step* step, rb200_stream_t stream);
+/* The same fused into the LM head (csrc/lmhead_sample.cu): hidden and weight as in rb200_lmhead_logprob_entropy_fwd;
+ * the lmhead mainloop writes the window's raw fp32 accumulator X . W^T [row tiles * 128, ld] into the workspace (only
+ * the window's rows of W are read), then the sampler above runs on it.  rb200_lmhead_sample_workspace_bytes() returns
+ * the workspace size (about (v_hi - v_lo) * 4 bytes per row), or -1 for an unsupported shape.
+ * With a step struct, L == 1 and N > 1 (rows b at hidden + b * batch_stride), the window block is computed as one
+ * item of N positions at row stride batch_stride: the workspace is rb200_lmhead_sample_workspace_bytes(N, N, ...). */
+int64_t rb200_lmhead_sample_workspace_bytes(int64_t N, int64_t L, int H, int V, int v_lo, int v_hi);
 int rb200_lmhead_sample_step(const void* hidden, const void* weight, int64_t N, int64_t L, int64_t batch_stride,
                              int64_t row_stride, int H, int V, int v_lo, int v_hi, int do_sample,
                              double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
@@ -990,14 +973,11 @@ int rb200_synth_env_chunk_step(const float* w_s, const float* w_a, const float* 
                                int B, int obs, int act, int C, int max_episode_steps, int auto_reset, float p_term,
                                float noise_std, float reward_noise_std, uint64_t seed, const uint64_t* counter_dev,
                                rb200_stream_t stream);
-/* strided form of rb200_bootstrap_rewards for the last sub-step of a chunk:
- * rewards[b*ld_rewards] += gamma * final_values[b*value_dim] where flag[b*ld_flag]  (env_worker.py:736-758) */
+/* rewards[b*ld_rewards] += gamma * final_values[b*value_dim] where flag[b*ld_flag]  (compute_bootstrap_rewards,
+ * workers/env/env_worker.py:736-758; flag = truncations ("standard") or dones ("always")).  ld = 1 for one-step
+ * actions; ld = C, with rewards and flag offset to column C-1, for the last sub-step of a chunk. */
 int rb200_bootstrap_rewards_ld(float* rewards, int ld_rewards, const float* final_values, int value_dim,
                                const uint8_t* flag, int ld_flag, int B, double gamma, rb200_stream_t stream);
-/* rewards[b] += gamma * final_values[b*value_dim] where flag[b]  (compute_bootstrap_rewards,
- * workers/env/env_worker.py:736-758; flag = truncations ("standard") or dones ("always")). */
-int rb200_bootstrap_rewards(float* rewards, const float* final_values, const uint8_t* flag, int B,
-                            int value_dim, double gamma, rb200_stream_t stream);
 /* counter_dev[0] += inc (device-side RNG step counter so captured CUDA graphs replay fresh noise). */
 int rb200_counter_add(uint64_t* counter_dev, uint64_t inc, rb200_stream_t stream);
 

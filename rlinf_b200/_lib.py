@@ -193,7 +193,6 @@ class MlpLayout(C.Structure):
 SIGNATURES = {
     "rb200_abi_version": (c_int, []),
     "rb200_strerror": (C.c_char_p, [c_int]),
-    "rb200_device_info": (c_int, [C.POINTER(c_int)] * 3),
     "rb200_launch_count": (c_uint64, []),
     "rb200_loss_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "rb200_gae": (c_int, [c_void_p] * 7 + [c_int, c_int, c_double, c_double, c_void_p]),
@@ -210,9 +209,6 @@ SIGNATURES = {
     "rb200_scale": (c_int, [c_void_p, c_int64, c_float, c_void_p]),
     "rb200_scale_by": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "rb200_grad_sqnorm": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
-    "rb200_adamw_step": (c_int, [c_void_p] * 4 + [c_int64, C.POINTER(c_int64), C.POINTER(c_double), c_int,
-                                                  c_double, c_double, c_double, c_double, c_float, c_float,
-                                                  c_void_p, c_void_p, c_void_p]),
     "rb200_adamw_step_dev": (c_int, [c_void_p] * 4 + [c_int64, C.POINTER(c_int64), c_void_p, c_int,
                                                       c_double, c_double, c_double, c_double, c_float, c_float,
                                                       c_void_p, c_void_p, c_void_p]),
@@ -257,13 +253,7 @@ SIGNATURES = {
     "rb200_lmhead_topk_logprob_entropy_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                                       c_int, c_int, c_int, c_int, c_double] + [c_void_p] * 8
                                               + [c_int64, c_void_p]),
-    "rb200_logits_sample_tokens": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
-                                           c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
-                                   + [c_void_p] * 4),
     "rb200_lmhead_sample_workspace_bytes": (c_int64, [c_int64, c_int64, c_int, c_int, c_int, c_int]),
-    "rb200_lmhead_sample_tokens": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
-                                           c_int, c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
-                                   + [c_void_p] * 4 + [c_int64, c_void_p]),
     "rb200_logits_sample_step": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int,
                                          c_int, c_double, c_int, c_uint64, c_uint64, C.POINTER(ActionBins)]
                                  + [c_void_p] * 3 + [C.POINTER(SampleStep), c_void_p]),
@@ -306,7 +296,6 @@ SIGNATURES = {
     "rb200_synth_env_step": (c_int, [c_void_p] * 13 + [c_int] * 5 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),
     "rb200_synth_env_chunk_step": (c_int, [c_void_p] * 13 + [c_int] * 6 + [c_float] * 3 + [c_uint64, c_void_p, c_void_p]),
     "rb200_bootstrap_rewards_ld": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_double, c_void_p]),
-    "rb200_bootstrap_rewards": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_double, c_void_p]),
     "rb200_reward_filter": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float, c_float, c_void_p]),
     "rb200_kl_penalty": (c_int, [c_void_p] * 4 + [c_int64, c_int, c_void_p]),
     "rb200_masked_stats": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),

@@ -1,4 +1,4 @@
-// ABI bookkeeping: version, error strings, device info, per-device scratch.
+// ABI bookkeeping: version, error strings, launch count, per-device scratch.
 #include "common.cuh"
 
 namespace rb {
@@ -54,14 +54,4 @@ extern "C" const char* rb200_strerror(int code) {
       if (code > 0) return cudaGetErrorString((cudaError_t)code);
       return "unknown rlinf_b200 error";
   }
-}
-
-extern "C" int rb200_device_info(int* sm_count, int* cc_major, int* cc_minor) {
-  int dev = 0;
-  RB_CHECK_CUDA(cudaGetDevice(&dev));
-  int v = 0;
-  if (sm_count) { RB_CHECK_CUDA(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev)); *sm_count = v; }
-  if (cc_major) { RB_CHECK_CUDA(cudaDeviceGetAttribute(&v, cudaDevAttrComputeCapabilityMajor, dev)); *cc_major = v; }
-  if (cc_minor) { RB_CHECK_CUDA(cudaDeviceGetAttribute(&v, cudaDevAttrComputeCapabilityMinor, dev)); *cc_minor = v; }
-  return RB200_OK;
 }

@@ -1,5 +1,5 @@
 // Action-token sampling of the OpenVLA-OFT rollout: the bin window, temperature, top-k, the draw, its log-prob and the
-// de-tokenised action, from the logits (rb200_logits_sample_tokens) or from the fused LM head's window block
+// de-tokenised action, from the logits (rb200_logits_sample_step) or from the fused LM head's window block
 // (lmhead_sample.cu, through rb::asmp::sample_tiles).
 //
 // Reference (OpenVLAOFTForRLActionPrediction.predict_action_batch, openvla_oft_action_model.py:350-410): -inf outside
@@ -24,8 +24,8 @@
 // inside the window, with a NaN log-prob.  No floating-point or global atomics; rows are independent, so nothing
 // depends on the grid or the SM count.
 //
-// One generate step (rb200_logits_sample_step, rb200_lmhead_sample_step; the plain OpenVLA decode loop of
-// OpenVLAForRLActionPrediction.predict_action_batch, openvla_action_model.py:610-756): the Philox offset is read from a
+// With a step struct (one generate step of the plain OpenVLA decode loop, OpenVLAForRLActionPrediction.
+// predict_action_batch, openvla_action_model.py:610-756, or the OFT call under a graph): the Philox offset is read from a
 // device counter that the entry then advances by 1 on the same stream (rollout.cu's rb200_counter_add), so a captured
 // graph draws fresh numbers on every replay; and row r = b * L + p writes its outputs at b * out_row_stride + col0 + p
 // and de-tokenises with dimension (col0 + p) % action_dim, so step j of a [bsz, A] buffer is column col0 = j.
@@ -56,8 +56,8 @@ struct SArgs {
   // (rt % tpb) * 128 + j % 128 < L (padding rows are skipped); its columns are the window's
   int tiled, tpb;
   int64_t rt0;
-  // the step entries: Philox offset from *offset_dev when set; row r (in rows of out_L positions) writes at
-  // (r / out_L) * out_stride + col0 + r % out_L.  The plain entries have out_L = out_stride = L and col0 = 0.
+  // a step struct: Philox offset from *offset_dev when set; row r (in rows of out_L positions) writes at
+  // (r / out_L) * out_stride + col0 + r % out_L.  Without a step struct out_L = out_stride = L and col0 = 0.
   const int64_t* offset_dev;
   int64_t out_L, out_stride;
   int col0;
@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(kWarps * 32) sample_kernel(const SArgs a) {
     zt = __shfl_sync(0xffffffffu, zt, tok & 31);
     if (lane == 0) {
       const int64_t id = (int64_t)a.v_lo + tok;
-      const int64_t op = a.col0 + r % a.out_L;  // output column (= p for the plain entries)
+      const int64_t op = a.col0 + r % a.out_L;  // output column (= p without a step struct)
       const int64_t o = (r / a.out_L) * a.out_stride + op;
       a.token[o] = id;
       a.logprob[o] = (zt - m) - logf(total);
@@ -232,26 +232,6 @@ int launch(const SArgs& a, cudaStream_t st) {
   else sample_kernel<T, 32><<<grid, kWarps * 32, 0, st>>>(a);
   rb::count_launch();
   RB_RETURN_LAUNCH();
-}
-
-// everything but the row addressing; the caller checks the window against its V
-int check_common(int W, int do_sample, double inv_temperature, const rb200_action_bins* bins, const int64_t* token,
-                 const float* logprob, const double* action) {
-  if (!token || !logprob) return RB200_E_NULL;
-  if (W < 1 || W > kMaxWindow) return RB200_E_SHAPE;
-  if (do_sample && !(inv_temperature > 0.0 && (float)inv_temperature < INFINITY)) return RB200_E_ARG;
-  if (bins) {
-    if (!action || !bins->bin_centers || !bins->low || !bins->high || !bins->mask) return RB200_E_NULL;
-    if (bins->n_bins < 1 || bins->action_dim < 1) return RB200_E_SHAPE;
-  }
-  return RB200_OK;
-}
-
-// the step struct against the call's L: a layout that every row's outputs fit in, columns not overlapping the next row's
-int check_step(const rb200_sample_step* s, int64_t L) {
-  if (!s) return RB200_E_NULL;
-  if (s->col0 < 0 || s->out_row_stride < (int64_t)s->col0 + L) return RB200_E_SHAPE;
-  return RB200_OK;
 }
 
 void apply_step(SArgs& a, const rb200_sample_step* s, int64_t L) {
@@ -287,6 +267,27 @@ SArgs make_args(int v_lo, int v_hi, int do_sample, double inv_temperature, int t
 
 namespace rb {
 namespace asmp {
+// everything but the row addressing; the caller checks the window against its V
+int check_common(int W, int do_sample, double inv_temperature, const rb200_action_bins* bins, const int64_t* token,
+                 const float* logprob, const double* action) {
+  if (!token || !logprob) return RB200_E_NULL;
+  if (W < 1 || W > kMaxWindow) return RB200_E_SHAPE;
+  if (do_sample && !(inv_temperature > 0.0 && (float)inv_temperature < INFINITY)) return RB200_E_ARG;
+  if (bins) {
+    if (!action || !bins->bin_centers || !bins->low || !bins->high || !bins->mask) return RB200_E_NULL;
+    if (bins->n_bins < 1 || bins->action_dim < 1) return RB200_E_SHAPE;
+  }
+  return RB200_OK;
+}
+
+// the step struct against the call's L: a layout that every row's outputs fit in, columns not overlapping the next row's;
+// NULL is the dense layout
+int check_step(const rb200_sample_step* s, int64_t L) {
+  if (!s) return RB200_OK;
+  if (s->col0 < 0 || s->out_row_stride < (int64_t)s->col0 + L) return RB200_E_SHAPE;
+  return RB200_OK;
+}
+
 // the sampler over a block of nt row tiles of the window's raw fp32 logits [nt * 128, ld] (lmhead_sample.cu's ACC
 // pass), writing row r's outputs at r; with a step struct (nullable) at its layout in rows of out_L positions, out_L
 // being the caller's L (the tiles may group the rows differently), then the counter advance
@@ -300,30 +301,8 @@ int sample_tiles(const float* block, int64_t ld, int v_lo, int v_hi, int do_samp
   int e = launch<float>(a, st);
   return e ? e : advance(step, st);
 }
-int check_sample(int W, int do_sample, double inv_temperature, const rb200_action_bins* bins, const int64_t* token,
-                 const float* logprob, const double* action) {
-  return check_common(W, do_sample, inv_temperature, bins, token, logprob, action);
-}
-int check_sample_step(const rb200_sample_step* step, int64_t L) { return check_step(step, L); }
 }  // namespace asmp
 }  // namespace rb
-
-extern "C" int rb200_logits_sample_tokens(const void* logits, int dtype, int64_t N, int64_t L, int64_t batch_stride,
-                                          int64_t row_stride, int V, int v_lo, int v_hi, int do_sample,
-                                          double inv_temperature, int top_k, uint64_t seed, uint64_t offset,
-                                          const rb200_action_bins* bins, int64_t* token, float* logprob,
-                                          double* action, rb200_stream_t stream) {
-  if (!logits) return RB200_E_NULL;
-  if (dtype != 0 && dtype != 1) return RB200_E_UNSUPPORTED;
-  if (N <= 0 || L <= 0 || N % L != 0 || V <= 0 || v_lo < 0 || v_hi > V || v_lo >= v_hi) return RB200_E_SHAPE;
-  int e = check_common(v_hi - v_lo, do_sample, inv_temperature, bins, token, logprob, action);
-  if (e) return e;
-  SArgs a = make_args(v_lo, v_hi, do_sample, inv_temperature, top_k, seed, offset, bins, token, logprob, action);
-  a.x = logits; a.N = N; a.L = L; a.batch_stride = batch_stride; a.row_stride = row_stride;
-  apply_step(a, nullptr, L);
-  cudaStream_t st = rb::as_stream(stream);
-  return dtype == 0 ? launch<float>(a, st) : launch<__nv_bfloat16>(a, st);
-}
 
 extern "C" int rb200_logits_sample_step(const void* logits, int dtype, int64_t N, int64_t L, int64_t batch_stride,
                                         int64_t row_stride, int V, int v_lo, int v_hi, int do_sample,
@@ -333,8 +312,8 @@ extern "C" int rb200_logits_sample_step(const void* logits, int dtype, int64_t N
   if (!logits) return RB200_E_NULL;
   if (dtype != 0 && dtype != 1) return RB200_E_UNSUPPORTED;
   if (N <= 0 || L <= 0 || N % L != 0 || V <= 0 || v_lo < 0 || v_hi > V || v_lo >= v_hi) return RB200_E_SHAPE;
-  int e = check_common(v_hi - v_lo, do_sample, inv_temperature, bins, token, logprob, action);
-  if (e || (e = check_step(step, L))) return e;
+  int e = rb::asmp::check_common(v_hi - v_lo, do_sample, inv_temperature, bins, token, logprob, action);
+  if (e || (e = rb::asmp::check_step(step, L))) return e;
   SArgs a = make_args(v_lo, v_hi, do_sample, inv_temperature, top_k, seed, offset, bins, token, logprob, action);
   a.x = logits; a.N = N; a.L = L; a.batch_stride = batch_stride; a.row_stride = row_stride;
   apply_step(a, step, L);

@@ -15,7 +15,6 @@ namespace {
 constexpr int kMaxGroups = 8;
 struct Groups {
   int64_t end[kMaxGroups];
-  double lr[kMaxGroups];
   int n;
 };
 
@@ -66,10 +65,6 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
                                                     double beta2, double eps, double wd, float grad_scale,
                                                     const double* __restrict__ state) {
   if (state[3] != 0.0) return;  // non-finite grad norm: skip the whole step
-  if (lr_dev != nullptr) {      // learning rates live in device memory (LR schedules under CUDA-graph replay)
-#pragma unroll
-    for (int k = 0; k < kMaxGroups; ++k) grp.lr[k] = k < grp.n ? lr_dev[k] : 0.0;
-  }
   const double step = state[0];
   const float gmul = (float)state[2] * grad_scale;  // clip coefficient x (1/world_size etc.)
   // scalar factors are formed in double (as Python floats in torch.optim) and rounded once
@@ -83,8 +78,9 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
   float decay[kMaxGroups], step_size[kMaxGroups];
 #pragma unroll
   for (int k = 0; k < kMaxGroups; ++k) {
-    decay[k] = (float)(1.0 - grp.lr[k] * wd);
-    step_size[k] = grp.lr[k] < 0.0 ? __int_as_float(0x7fc00000) : (float)(grp.lr[k] / bc1);
+    const double lr = k < grp.n ? lr_dev[k] : 0.0;  // read at execution time: LR schedules under CUDA-graph replay
+    decay[k] = (float)(1.0 - lr * wd);
+    step_size[k] = lr < 0.0 ? __int_as_float(0x7fc00000) : (float)(lr / bc1);
   }
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
@@ -126,28 +122,20 @@ extern "C" int rb200_grad_sqnorm(const float* grads, int64_t n, double* out_sq, 
   RB_RETURN_LAUNCH();
 }
 
-static int adamw_step_impl(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
-                           const int64_t* group_end_host, const double* group_lr_host, const double* group_lr_dev,
-                           int n_groups, double beta1, double beta2, double eps, double weight_decay,
-                           float max_grad_norm, float grad_scale, const double* grad_sq, double* state,
-                           rb200_stream_t stream) {
-  if (!params || !grads || !exp_avg || !exp_avg_sq || !group_end_host || (!group_lr_host && !group_lr_dev) || !grad_sq ||
-      !state)
+extern "C" int rb200_adamw_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
+                                    const int64_t* group_end_host, const double* group_lr_dev, int n_groups,
+                                    double beta1, double beta2, double eps, double weight_decay, float max_grad_norm,
+                                    float grad_scale, const double* grad_sq, double* state, rb200_stream_t stream) {
+  if (!params || !grads || !exp_avg || !exp_avg_sq || !group_end_host || !group_lr_dev || !grad_sq || !state)
     return RB200_E_NULL;
   if (n <= 0 || n_groups <= 0 || n_groups > kMaxGroups) return RB200_E_SHAPE;
   Groups grp;
   grp.n = n_groups;
   int64_t prev = 0;
   for (int k = 0; k < kMaxGroups; ++k) {
-    if (k < n_groups) {
-      if (group_end_host[k] < prev || group_end_host[k] > n) return RB200_E_SHAPE;
-      prev = group_end_host[k];
-      grp.end[k] = group_end_host[k];
-      grp.lr[k] = group_lr_host ? group_lr_host[k] : 0.0;
-    } else {
-      grp.end[k] = n;
-      grp.lr[k] = 0.0;
-    }
+    grp.end[k] = k < n_groups ? group_end_host[k] : n;
+    if (grp.end[k] < prev || grp.end[k] > n) return RB200_E_SHAPE;
+    prev = grp.end[k];
   }
   if (grp.end[n_groups - 1] != n) return RB200_E_SHAPE;
   cudaStream_t st = rb::as_stream(stream);
@@ -158,21 +146,4 @@ static int adamw_step_impl(float* params, const float* grads, float* exp_avg, fl
   adamw_kernel<<<(int)blocks, 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, n, grp, group_lr_dev, beta1, beta2, eps,
                                             weight_decay, grad_scale, state); rb::count_launch();
   RB_RETURN_LAUNCH();
-}
-
-extern "C" int rb200_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
-                                const int64_t* group_end_host, const double* group_lr_host, int n_groups, double beta1,
-                                double beta2, double eps, double weight_decay, float max_grad_norm, float grad_scale,
-                                const double* grad_sq, double* state, rb200_stream_t stream) {
-  return adamw_step_impl(params, grads, exp_avg, exp_avg_sq, n, group_end_host, group_lr_host, nullptr, n_groups, beta1,
-                         beta2, eps, weight_decay, max_grad_norm, grad_scale, grad_sq, state, stream);
-}
-
-extern "C" int rb200_adamw_step_dev(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
-                                    const int64_t* group_end_host, const double* group_lr_dev, int n_groups,
-                                    double beta1, double beta2, double eps, double weight_decay, float max_grad_norm,
-                                    float grad_scale, const double* grad_sq, double* state, rb200_stream_t stream) {
-  if (!group_lr_dev) return RB200_E_NULL;
-  return adamw_step_impl(params, grads, exp_avg, exp_avg_sq, n, group_end_host, nullptr, group_lr_dev, n_groups, beta1,
-                         beta2, eps, weight_decay, max_grad_norm, grad_scale, grad_sq, state, stream);
 }

@@ -179,7 +179,8 @@ __global__ void __launch_bounds__(256) chunk_finish_kernel(ChunkFinishArgs p) {
   }
 }
 
-// rewards[b*ld_r] += gamma * vfinal[b*vdim] where flag[b*ld_f]  (the last sub-step of a chunk: ld = C)
+// rewards[b*ld_r] += gamma * vfinal[b*vdim] where flag[b*ld_f]  (compute_bootstrap_rewards, env_worker.py:736-758;
+// ld = 1 for one-step actions, ld = C at the last sub-step of a chunk)
 __global__ void __launch_bounds__(256) bootstrap_ld_kernel(float* __restrict__ rewards, int ld_r, const float* __restrict__ vfinal,
                                                            int vdim, const uint8_t* __restrict__ flag, int ld_f, int B,
                                                            float gamma) {
@@ -187,14 +188,6 @@ __global__ void __launch_bounds__(256) bootstrap_ld_kernel(float* __restrict__ r
   if (b >= B) return;
   if (flag[(size_t)b * ld_f])
     rewards[(size_t)b * ld_r] = __fadd_rn(rewards[(size_t)b * ld_r], __fmul_rn(gamma, vfinal[(size_t)b * vdim]));
-}
-
-// rewards[b] += gamma * V(final_obs)[b] * flag[b]   (compute_bootstrap_rewards, env_worker.py:736-758)
-__global__ void __launch_bounds__(256) bootstrap_kernel(float* __restrict__ rewards, const float* __restrict__ vfinal,
-                                                        const uint8_t* __restrict__ flag, int B, int vdim, float gamma) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  if (flag[b]) rewards[b] = __fadd_rn(rewards[b], __fmul_rn(gamma, vfinal[(size_t)b * vdim]));
 }
 
 __global__ void counter_add_kernel(uint64_t* ctr, uint64_t inc) {
@@ -225,15 +218,6 @@ extern "C" int rb200_synth_env_step(const float* w_s, const float* w_a, const fl
   p.seed = seed; p.B = B; p.obs = obs; p.act = act; p.max_episode_steps = max_episode_steps; p.auto_reset = auto_reset;
   p.p_term = p_term; p.noise_std = noise_std; p.reward_noise_std = reward_noise_std;
   env_finish_kernel<<<(B + 7) / 8, 256, 0, st>>>(p); rb::count_launch();
-  RB_RETURN_LAUNCH();
-}
-
-extern "C" int rb200_bootstrap_rewards(float* rewards, const float* final_values, const uint8_t* flag, int B,
-                                       int value_dim, double gamma, rb200_stream_t stream) {
-  if (!rewards || !final_values || !flag) return RB200_E_NULL;
-  if (B <= 0 || value_dim <= 0) return RB200_E_SHAPE;
-  bootstrap_kernel<<<(B + 255) / 256, 256, 0, rb::as_stream(stream)>>>(rewards, final_values, flag, B, value_dim,
-                                                                        (float)gamma); rb::count_launch();
   RB_RETURN_LAUNCH();
 }
 

@@ -883,8 +883,8 @@ def _sample_outputs(shape, device, bins):
 
 
 def _step_mode(offset, counter, out, column, top_p, device, bins, what: str):
-    """Validates the generate-step arguments.  Returns (step: bool, column or None); a step call goes through the
-    *_sample_step entries (a device counter, an output column, or both)."""
+    """Validates the generate-step arguments.  Returns (step: bool, column or None); a step call passes the entry an
+    rb200_sample_step (a device counter, an output column, or both), any other call passes NULL."""
     if float(top_p) != 1.0:
         raise ValueError(f"{what}: top_p must be 1.0 (no nucleus filter is applied), got {top_p}")
     if (offset is None) == (counter is None):
@@ -973,11 +973,8 @@ def sample_action_tokens(logits, window, *, do_sample: bool, temperature: float 
     b = C.byref(bins.args(x.device)[0]) if bins is not None else None
     args = (_raw_ptr(x), 0 if x.dtype == torch.float32 else 1, N, Lr, bs, rs, V, lo, hi, int(bool(do_sample)), inv_t,
             k, seed, offset, b, L.ptr(tok), L.ptr(lp), L.ptr(act))
-    if step:
-        st = _step_struct(counter, Lr, out, column)
-        L.check(lib.rb200_logits_sample_step(*args, C.byref(st), L.stream_ptr(x.device)), "logits_sample_step")
-    else:
-        L.check(lib.rb200_logits_sample_tokens(*args, L.stream_ptr(x.device)), "logits_sample_tokens")
+    st = C.byref(_step_struct(counter, Lr, out, column)) if step else None
+    L.check(lib.rb200_logits_sample_step(*args, st, L.stream_ptr(x.device)), "logits_sample_step")
     return tok, lp, act
 
 
@@ -1019,11 +1016,8 @@ def linear_sample_action_tokens(hidden, weight, window, *, do_sample: bool, temp
     b = C.byref(bins.args(x.device)[0]) if bins is not None else None
     args = (_raw_ptr(x), L.ptr(w), N, Lr, bs, rs, H, V, lo, hi, int(bool(do_sample)), inv_t, k, seed, offset, b,
             L.ptr(tok), L.ptr(lp), L.ptr(act), L.ptr(ws), wsb)
-    if step:
-        st = _step_struct(counter, Lr, out, column)
-        L.check(lib.rb200_lmhead_sample_step(*args, C.byref(st), L.stream_ptr(x.device)), "lmhead_sample_step")
-    else:
-        L.check(lib.rb200_lmhead_sample_tokens(*args, L.stream_ptr(x.device)), "lmhead_sample_tokens")
+    st = C.byref(_step_struct(counter, Lr, out, column)) if step else None
+    L.check(lib.rb200_lmhead_sample_step(*args, st, L.stream_ptr(x.device)), "lmhead_sample_step")
     return tok, lp, act
 
 

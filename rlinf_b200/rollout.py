@@ -354,9 +354,9 @@ class RolloutWorker:
                 side.wait_stream(main)
                 with torch.cuda.stream(side):
                     pol.value(buf.final_obs, out=buf.final_values)
-                    L.check(lib.rb200_bootstrap_rewards(L.ptr(buf.rewards[t]), L.ptr(buf.final_values),
-                                                        L.ptr(flag.view(B)), B, pol.value_dim, self.gamma,
-                                                        L.stream_ptr()), "bootstrap_rewards")
+                    L.check(lib.rb200_bootstrap_rewards_ld(L.ptr(buf.rewards[t]), 1, L.ptr(buf.final_values),
+                                                           pol.value_dim, L.ptr(flag.view(B)), 1, B, self.gamma,
+                                                           L.stream_ptr()), "bootstrap_rewards_ld")
                 side_busy = True
         if side_busy:
             main.wait_stream(side)

@@ -1,8 +1,8 @@
 """Action-token sampling of the OpenVLA-OFT rollout without a GPU: the fp64 oracle and the numpy de-tokeniser
 (tests/action_sample_oracle.py) against the reference fixture (tests/golden/golden_action_sample.npz), argument
-validation, the C envelope of both entries, the ctypes signatures and struct against the header, no spills in
-csrc/action_sample.cu and csrc/lmhead_sample.cu and no serialised wgmma in the latter, and the SASS of logits.o, lmhead.o
-and topk.o as at the parent commit (tests/golden/sass_digests_action_sample.json)."""
+validation, the C envelope of both entries, their ctypes signatures and rb200_action_bins against the header, no spills
+in csrc/action_sample.cu and csrc/lmhead_sample.cu and no serialised wgmma in the latter, and the SASS of logits.o,
+lmhead.o and topk.o as at the parent commit (tests/golden/sass_digests_action_sample.json)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -118,8 +118,8 @@ def _lib_loaded():
     return _lib.load()
 
 
-@pytest.mark.parametrize("name", ["rb200_logits_sample_tokens", "rb200_lmhead_sample_workspace_bytes",
-                                  "rb200_lmhead_sample_tokens"])
+@pytest.mark.parametrize("name", ["rb200_logits_sample_step", "rb200_lmhead_sample_workspace_bytes",
+                                  "rb200_lmhead_sample_step"])
 def test_ctypes_signature_matches_header(name):
     src = open(os.path.join(ROOT, "include", "rlinf_b200.h")).read()
     m = re.search(rf"(int|int64_t) {name}\((.*?)\);", src, flags=re.S)
@@ -129,6 +129,8 @@ def test_ctypes_signature_matches_header(name):
     for q in params:
         if q.startswith("const rb200_action_bins*"):
             want.append(C.POINTER(_lib.ActionBins))
+        elif q.startswith("const rb200_sample_step*"):
+            want.append(C.POINTER(_lib.SampleStep))
         elif "*" in q or q.startswith("rb200_stream_t"):
             want.append(_lib.c_void_p)
         else:
@@ -160,10 +162,10 @@ def test_struct_layout_matches_ctypes(tmp_path):
 def test_c_envelope_returns_invalid_argument():
     lib = _lib_loaded()
     p = _lib.c_void_p(1 << 20)
-    f = lib.rb200_logits_sample_tokens
+    f = lib.rb200_logits_sample_step
 
     def call(lo=44, hi=300, V=320, do_sample=1, inv_t=1.0, bins=None, tok=p, lp=p, act=p, dtype=1, N=14, L=7):
-        return f(p, dtype, N, L, 7 * V, V, V, lo, hi, do_sample, inv_t, 8, 1, 2, bins, tok, lp, act, None)
+        return f(p, dtype, N, L, 7 * V, V, V, lo, hi, do_sample, inv_t, 8, 1, 2, bins, tok, lp, act, None, None)
 
     assert call(lo=44, hi=44) == -2                          # W = 0
     assert call(lo=0, hi=1025, V=2000) == -2                 # W > 1024
@@ -180,10 +182,10 @@ def test_c_envelope_returns_invalid_argument():
     assert ws(256, 256, 1000, 320, 44, 300) == -1            # H % 64 != 0
     assert ws(256, 256, 64, 320, 44, 300) == 2 * 128 * 256 * 4
     assert ws(300, 300, 64, 320, 44, 301) == 3 * 128 * 260 * 4
-    fused = lib.rb200_lmhead_sample_tokens
+    fused = lib.rb200_lmhead_sample_step
 
     def fcall(H=64, lo=44, hi=300, V=320, inv_t=1.0, wsb=1 << 30):
-        return fused(p, p, 256, 256, 256 * H, H, H, V, lo, hi, 1, inv_t, 8, 1, 2, None, p, p, None, p, wsb, None)
+        return fused(p, p, 256, 256, 256 * H, H, H, V, lo, hi, 1, inv_t, 8, 1, 2, None, p, p, None, p, wsb, None, None)
 
     assert fcall(H=96) == -2 and fcall(H=8256) == -2          # H % 64, H > 8192
     assert fcall(lo=44, hi=44) == -2 and fcall(lo=0, hi=1025, V=2000) == -2 and fcall(hi=321) == -2

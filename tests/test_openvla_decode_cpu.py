@@ -1,7 +1,7 @@
 """Plain OpenVLA's generate step without a GPU: the restatement (tests/openvla_decode_oracle.py) against the
-transformers-generate fixture (tests/golden/golden_openvla_decode.npz), HF's processor order, the step entries'
-ctypes signatures and rb200_sample_step against the header, the argument checks of the step and counter modes, and
-ptxas on the sampler objects (no spills, no serialised wgmma)."""
+transformers-generate fixture (tests/golden/golden_openvla_decode.npz), HF's processor order, rb200_sample_step against
+the header, the argument checks of the step and counter modes, and ptxas on the sampler objects (no spills, no
+serialised wgmma)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -93,32 +93,6 @@ def test_hidden_rows_and_window_weight_give_the_logits(g):
 
 
 # ------------------------------------------------------------------ ABI
-def _header():
-    return open(os.path.join(ROOT, "include", "rlinf_b200.h")).read()
-
-
-@pytest.mark.parametrize("name", ["rb200_logits_sample_step", "rb200_lmhead_sample_step"])
-def test_ctypes_signature_matches_header(name):
-    m = re.search(rf"(int|int64_t) {name}\((.*?)\);", _header(), flags=re.S)
-    params = [q.strip() for q in m.group(2).split(",")]
-    ctype = {"int": _lib.c_int, "int64_t": _lib.c_int64, "uint64_t": _lib.c_uint64, "double": _lib.c_double}
-    want = []
-    for q in params:
-        if q.startswith("const rb200_action_bins*"):
-            want.append(C.POINTER(_lib.ActionBins))
-        elif q.startswith("const rb200_sample_step*"):
-            want.append(C.POINTER(_lib.SampleStep))
-        elif "*" in q or q.startswith("rb200_stream_t"):
-            want.append(_lib.c_void_p)
-        else:
-            want.append(ctype[q.rsplit(" ", 1)[0]])
-    res, args = _lib.SIGNATURES[name]
-    assert res is ctype[m.group(1)] and args == want
-    # the step entries take the plain entries' arguments, then the step struct, then the stream
-    base = _lib.SIGNATURES[name.replace("_step", "_tokens")][1]
-    assert args[:-2] == base[:-1] and args[-1] == base[-1]
-
-
 def test_sample_step_layout_matches_ctypes(tmp_path):
     cls, cname = _lib.SampleStep, "rb200_sample_step"
     lines = [f'  printf("sizeof %zu\\n", sizeof({cname}));']
@@ -146,7 +120,7 @@ def _lib_loaded():
 
 
 def test_step_envelope_returns_invalid_argument():
-    """The checks that fail before any launch: a NULL step struct, and an output layout that does not hold the rows."""
+    """The checks that fail before any launch: an output layout that does not hold the rows."""
     lib = _lib_loaded()
     p = _lib.c_void_p(1 << 20)
     f = lib.rb200_logits_sample_step
@@ -154,7 +128,6 @@ def test_step_envelope_returns_invalid_argument():
     def call(step, L=1, N=4):
         return f(p, 1, N, L, 320, 320, 320, 44, 300, 1, 1.0, 8, 1, 2, None, p, p, None, step, None)
 
-    assert call(None) == -1
     assert call(C.byref(_lib.SampleStep(None, 7, -1, 0))) == -2          # col0 < 0
     assert call(C.byref(_lib.SampleStep(None, 7, 7, 0))) == -2           # col0 + L past the row stride
     assert call(C.byref(_lib.SampleStep(None, 13, 7, 0)), L=7, N=14) == -2
@@ -163,7 +136,6 @@ def test_step_envelope_returns_invalid_argument():
     def fcall(step, H=64):
         return fused(p, p, 256, 1, H, H, H, 320, 44, 300, 1, 1.0, 8, 1, 2, None, p, p, None, p, 1 << 30, step, None)
 
-    assert fcall(None) == -1
     assert fcall(C.byref(_lib.SampleStep(None, 7, 7, 0))) == -2
     assert fcall(C.byref(_lib.SampleStep(None, 7, 0, 0)), H=96) == -2   # H % 64
 
